@@ -1,4 +1,4 @@
-"""ctypes binding of libbanet_sm100.so (C-ABI declared in include/banet_abi.h).
+"""ctypes binding of libbanet.so (C-ABI declared in include/banet_abi.h).
 
 There is NO fallback: if the shared library is missing or a call fails, an exception is raised.
 """
@@ -9,7 +9,7 @@ import os
 from typing import Optional
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("BANET_LIB_PATH") or os.path.join(_HERE, "libbanet_sm100.so")      # the override is for kernel-variant timing scripts only
+LIB_PATH = os.environ.get("BANET_LIB_PATH") or os.path.join(_HERE, "libbanet.so")      # the override is for kernel-variant timing scripts only
 
 BANET_OK = 0
 PREC_AUTO, PREC_FP32_SIMT, PREC_TF32X1, PREC_TF32X2, PREC_TF32X3, PREC_TF32_LEVELWISE = -1, 0, 1, 2, 3, 4
@@ -126,5 +126,5 @@ def set_tuning(tc_generation: int = 0, tc7_force_direct: bool = False, tc7_band_
 
 
 def require_device() -> None:
-    """Raise unless the current CUDA device is a compute-capability-10.x part (B200)."""
+    """Raise unless the current CUDA device is a compute-capability-9.0 part (H100)."""
     check(load().banet_device_check(), "banet_device_check")

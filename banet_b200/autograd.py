@@ -1,7 +1,7 @@
 """Differentiable BundleIteration / CameraIteration.
 
 Two training paths:
-  * `iteration_fused` (default): torch.autograd.Functions over the fused sm_100a kernels — forward banet_lm_build /
+  * `iteration_fused` (default): torch.autograd.Functions over the fused sm_90a kernels — forward banet_lm_build /
     banet_lm_solve_update, backward banet_lm_build_bwd / banet_lm_solve_update_bwd (banet_b200/csrc/lm_bwd.cu): nothing per-pixel
     (J, G, d, the tiled upstream gradients of utils.cu:613-617) is materialised, so it runs at any N and K <= 256.  The lambda-MLP
     (5 dense layers on a [nb,C] vector, bundlenet.py:244-248) stays stock torch in between.  Gradient signature = the reference's:
@@ -11,7 +11,7 @@ Two training paths:
     reference:  TF graph ops (warp, resampler, Jacobians, damping, solve, update; TF autodiff)  +  native op
                 `equation_construction` with its registered native gradient (bundlenet.py:76-82, 263)
     here:       the same graph in stock torch CUDA ops (torch autograd)                          +  native op
-                `ops.equation_construction` = banet_eqc_fwd / banet_eqc_bwd (sm_100a)
+                `ops.equation_construction` = banet_eqc_fwd / banet_eqc_bwd (sm_90a)
 
 This is the TRAINING path: it materialises J[nb,N,2,P], G[nb,N,C,2], d[nb,N,C,1] exactly like the reference does
 (so it is meant for the reference's training regime, N <= a few thousand sampled points).  The fused kernels

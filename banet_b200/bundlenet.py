@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's BA-layer interface (reference bundlenet.py:86-399), backed by the
-sm_100a kernels.  Same method names, argument order, tensor layouts and return values as the reference's
-`BundleNet`; arithmetic happens in libbanet_sm100.so (no torch maths on the hot path, no CPU fallback).
+sm_90a kernels.  Same method names, argument order, tensor layouts and return values as the reference's
+`BundleNet`; arithmetic happens in libbanet.so (no torch maths on the hot path, no CPU fallback).
 
 Differences a reference user should know (all documented in DESIGN.md):
   * fx,fy,ox,oy may be passed as the reference does ([nb,N], constant along N) — column 0 is used;

@@ -1,4 +1,4 @@
-// extern "C" entry points of libbanet_sm100.so (see include/banet_abi.h) + the LM driver loop.
+// extern "C" entry points of libbanet.so (see include/banet_abi.h) + the LM driver loop.
 #include "common.cuh"
 #include "lm_build.h"
 #include <string.h>
@@ -111,7 +111,7 @@ extern "C" int banet_device_check(void)
     int major = 0, minor = 0;
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-    BANET_REQUIRE(major == 10, BANET_ERR_UNSUPPORTED, "device compute capability %d.%d; this library is built for sm_100a only", major, minor);
+    BANET_REQUIRE(major == 9 && minor == 0, BANET_ERR_UNSUPPORTED, "device compute capability %d.%d; this library is built for sm_90a only", major, minor);
     return BANET_OK;
 }
 

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of libbanet_sm100.so.
+// Shared helpers for the sm_90a kernels of libbanet.so.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -20,7 +20,7 @@ void set_error(const char* fmt, ...);
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-constexpr int kMaxSMs = 148;          // B200: 2 dies x 74 SMs
+constexpr int kMaxSMs = 132;          // H100 SXM
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

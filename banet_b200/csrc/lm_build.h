@@ -1,4 +1,4 @@
-// Internal interfaces between the translation units of libbanet_sm100.so.
+// Internal interfaces between the translation units of libbanet.so.
 #pragma once
 #include "common.cuh"
 
@@ -15,7 +15,7 @@ struct BuildParams {
     int band_rows;                    // dense-grid tensor-core kernels: tiles are walked in bands of this many tile rows, column by column inside a band
     int tap_prefetch;                 // generation 6: 0 off, 1 the geometry warps prefetch the tap footprint into L2 (halo from the tile's border pixels), 2 = every pixel also fetches its lower row
     int l2_hints;                     // generation 6: 0 none, 1 read-once streams evict-first, 2 = 1 + taps evict-last
-    int hdd_transposed;               // tensor-core path stores the H_dd block of a slot column-major (coalesced TMEM drains)
+    int hdd_transposed;               // tensor-core path stores the H_dd block of a slot column-major
     int force_direct;                 // generation 7, testing: take the global-tap fallback for every tile
     long long* trace;                 // optional debug timeline buffer (NULL in production)
 };

@@ -1,17 +1,20 @@
 // lm_build_tc6.cu — tensor-core build kernel, generation 6: every phase has its own warpgroup, phases of different tiles overlap.
 //
-// Contract, slot layout and precision modes: see lm_build_tc_host.cu.  Roles (896 threads, 1 CTA / SM; register budgets by setmaxnreg,
-// 48 / 88 / 72 / 32 = 64 512 of the SM's 65 536 registers):
+// Contract, slot layout and precision modes: see lm_build_tc_host.cu.  Roles (640 threads, 1 CTA / SM; register budgets by setmaxnreg,
+// 48 / 112 / 72 / 136 = 61 440 registers, the CTA's allocation at 96 per thread):
 //
 //   warpgroup 0    4 geometry warps, 16 pixels each per tile, run ahead of everybody:                              (48 regs)
 //                    b.W from the TMA-staged basis tile, warp / mask / tap offsets -> pixel records (ring of NREC)
-//   warpgroups 1-4 16 gather warps, 4 pixels each per tile: records -> 13 tap loads -> blend / accumulate -> M, q  (88 regs)
-//   warpgroup 5    4 algebra warps, 16 pixels each per tile:                                                        (72 regs)
+//   warpgroups 1-2 8 gather warps, 8 pixels each per tile: records -> 13 tap loads -> blend / accumulate -> M, q  (112 regs)
+//   warpgroup 3    4 algebra warps, 16 pixels each per tile:                                                        (72 regs)
 //                    2x7 per-pixel algebra (H_cc / g_c partials in registers), R rows (A_lo, R_lo) into smem,
-//                    then ONE elected thread issues the tile's tcgen05.mma and refills the freed basis stage by TMA
-//   warpgroup 6    4 drainer warps (one TMEM lane quadrant each): TMEM chains -> partial slots (L2 evict-last), asynchronous (32 regs)
+//                    refill of the freed basis stage by TMA (one elected thread)
+//   warpgroup 4    4 MMA warps: D = A^T R of every tile by mma.sync tf32 (each 8-pixel step added round-to-nearest) into register
+//                    accumulators that live for the whole pair span (lower block triangle of H_dd + the [v | t] columns, 80 floats per
+//                    thread); one slot write per span (136 regs)
+//   The accumulators take the registers the 5th-generation tensor core kept in tensor memory; half of the gather warps give them up.
 //   mbarriers: fullB[NST] TMA landed | recs[NREC] geometry->gather | gath[NREC] gather->algebra | recfree[NREC] algebra->geometry |
-//              rfree MMAs of the tile done (R, A_lo and the A stage reusable) | chain_done/drained[2], flushb, tmemfree issuer<->drainers |
+//              rready R (A_lo, R_lo) of the tile written | rfree MMAs of the tile done (R, A_lo and the A stage reusable) |
 //              rbdump/rbfree gather<->algebra hand-over of the |diff| sums at a pair change.
 #include "common.cuh"
 #include "lm_build.h"
@@ -22,25 +25,27 @@
 namespace banet { namespace v6 {
 using namespace tc;
 
-constexpr int TILE = 64, W0 = 4, GW = 16, AW = 4, DW = 4;      // geometry | gather | algebra | drainer warps
-constexpr int THREADS = (W0 + GW + AW + DW) * 32;               // 896
-constexpr int KB = 128, NN = 160;
+constexpr int TILE = 64, W0 = 4, GW = 8, AW = 4, MW = 4;       // geometry | gather | algebra | MMA warps
+constexpr int THREADS = (W0 + GW + AW + MW) * 32;               // 640
 constexpr int STAGE_A = 4 * TILE * 128, STAGE_R = 5 * TILE * 128;
 constexpr int REC = 16;
-constexpr int CHAIN = 8, TMEM_COLS = 512, ACCL = 320;
 
 template <int MODE, bool FLY> struct Smem {
-#ifndef BANET_TC6_NST
-#define BANET_TC6_NST 4
+#ifndef BANET_TC6_NST1
+#define BANET_TC6_NST1 4
+#endif
+#ifndef BANET_TC6_NST2
+#define BANET_TC6_NST2 3
+#endif
+#ifndef BANET_TC6_NST3
+#define BANET_TC6_NST3 2
 #endif
 #ifndef BANET_TC6_NREC
 #define BANET_TC6_NREC 3
 #endif
-    // basis-tile stages (TMA ring) and pixel-record buffers.  Deeper rings decouple the roles, but whatever smem the CTA takes is lost
-    // to the L1 that catches the tap overlap of neighbouring pixels: measured best per mode / layout (640x480, 32 pairs):
-    //   TF32X2 + [F2|gx|gy] layout: 3 stages (192 KB -> 196 KB carve-out, 60 KB L1) 7.4 ms vs 4 stages (228 KB) 8.6 ms
-    //   TF32X2 + F2-only layout   : 4 stages 7.2 ms vs 3 stages 8.8 ms;  TF32X1: 4 stages 5.6 ms vs 3 stages 6.1 ms
-    static constexpr int NST = MODE == 3 ? 3 : (MODE == 2 && !FLY) ? 3 : BANET_TC6_NST;
+    // basis-tile stages (TMA ring) and pixel-record buffers per precision mode.  Deeper rings decouple the roles, but whatever smem the
+    // CTA takes is lost to the L1, which holds the gather warps' tap loads in flight and catches the tap overlap of neighbouring pixels.
+    static constexpr int NST = MODE == 1 ? BANET_TC6_NST1 : MODE == 2 ? BANET_TC6_NST2 : BANET_TC6_NST3;
     static constexpr int NREC = MODE == 3 ? 2 : BANET_TC6_NREC;
     static constexpr int off_A = 0;
     static constexpr int off_R = NST * STAGE_A;
@@ -48,7 +53,6 @@ template <int MODE, bool FLY> struct Smem {
     static constexpr int off_Rlo = off_Alo + (MODE >= 2 ? STAGE_A : 0);
     static constexpr int off_misc = off_Rlo + (MODE == 3 ? STAGE_R : 0);
     static constexpr int off_bar = off_misc;                           // 22 mbarriers
-    static constexpr int off_tmem = off_bar + 22 * 8;
     static constexpr int off_tile = off_misc + 192;                    // [NREC][4] ints: pair index of the tile in record buffer s
     static constexpr int off_pose = off_tile + 64;                     // [W0][16] floats (private to each geometry warp)
     static constexpr int off_w = off_pose + W0 * 16 * 4;               // [W0][128] floats: W of the pair (private to each geometry warp)
@@ -56,7 +60,7 @@ template <int MODE, bool FLY> struct Smem {
     static constexpr int off_rbs = off_rec + NREC * TILE * REC * 4;    // [GW][128] floats: rbar hand-over gather -> algebra
     static constexpr int off_ccs = off_rbs + GW * 128 * 4;             // [AW][28] floats: H_cc / g_c / nvalid partials per algebra warp
     static constexpr int total = off_ccs + AW * 28 * 4;
-    static constexpr int slack = MODE == 3 ? 0 : 512;                  // MODE 3 fills the SM: the (512-B) base alignment is checked, not padded
+    static constexpr int slack = 1024;                                 // stage bases 1024-B aligned (128B swizzle atoms)
     static constexpr int bytes = total + slack;
 };
 
@@ -101,26 +105,21 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
 {
     using SM = Smem<MODE, FLY>;
     constexpr int NST = SM::NST, NREC = SM::NREC;
-    // KBLK = K / 32 basis blocks actually present (K = 128, 64 or 32).  The smem / TMEM geometry stays that of K = 128 (M = 128 rows of D,
-    // 32-KB stages); blocks >= KBLK are never loaded, read by the SIMT loops or drained, and the [v | t] block of R follows the last one.
-    constexpr int KR = 32 * KBLK, EXTB = KBLK, NMMA = KBLK == 4 ? NN : KR + 16;
+    // KBLK = K / 32 basis blocks actually present (K = 128, 64 or 32).  The smem geometry stays that of K = 128 (32-KB stages); blocks
+    // >= KBLK are never loaded or read, and the [v | t] block of R follows the last one.
+    constexpr int KR = 32 * KBLK, EXTB = KBLK;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     // align through the 32-bit shared address so that the compiler keeps every access in the shared state space (LDS/STS, not generic LD/ST)
-    unsigned char* base = smem_raw + (SM::slack ? ((512u - (smem_u32(smem_raw) & 511u)) & 511u) : 0u);
-    if (SM::slack == 0 && (smem_u32(smem_raw) & 511u)) __trap();      // fail loudly: swizzle atoms need 512-B aligned stage bases
+    unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint64_t* bars = reinterpret_cast<uint64_t*>(base + SM::off_bar);
     uint64_t* fullB = bars;            // [NST]  TMA landed
-    uint64_t* rfree = bars + 4;        //        MMAs of the tile completed
-    uint64_t* flushb = bars + 5;       //        every MMA of the span completed
-    uint64_t* tmemfree = bars + 6;     //        lo accumulator drained
-    uint64_t* chain_done = bars + 7;   // [2]
-    uint64_t* drained = bars + 9;      // [2]
+    uint64_t* rfree = bars + 4;        //        MMAs of the tile completed (count MW)
+    uint64_t* rready = bars + 5;       //        R (A_lo, R_lo) of the tile written (count AW)
     uint64_t* recs = bars + 11;        // [NREC] records of the tile in buffer s written (count W0)
     uint64_t* gath = bars + 14;        // [NREC] M,q of the tile in buffer s written (count GW)
     uint64_t* recfree = bars + 17;     // [NREC] records of the tile in buffer s consumed by the algebra warps (count AW)
     uint64_t* rbdump = bars + 20;      //        gather warps parked their rbar partials (count GW)
     uint64_t* rbfree = bars + 21;      //        algebra warps consumed them (count AW)
-    uint32_t* s_tmem = reinterpret_cast<uint32_t*>(base + SM::off_tmem);
     int* sTile = reinterpret_cast<int*>(base + SM::off_tile);
     float* sPose = reinterpret_cast<float*>(base + SM::off_pose);
     float* sW = reinterpret_cast<float*>(base + SM::off_w);
@@ -139,26 +138,21 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
     if (tid == 0) {
         for (int i = 0; i < NST; ++i) mbar_init(&fullB[i], 1);
         for (int i = 0; i < NREC; ++i) { mbar_init(&recs[i], W0); mbar_init(&gath[i], GW); mbar_init(&recfree[i], AW); }
-        mbar_init(rfree, 1); mbar_init(flushb, 1); mbar_init(tmemfree, DW);
-        mbar_init(&chain_done[0], 1); mbar_init(&chain_done[1], 1); mbar_init(&drained[0], DW); mbar_init(&drained[1], DW);
+        mbar_init(rfree, MW); mbar_init(rready, AW);
         mbar_init(rbdump, GW); mbar_init(rbfree, AW);
         fence_barrier_init();
         prefetch_tmap(&tmapB);
     }
-    if (warp == 0) tmem_alloc<TMEM_COLS>(s_tmem);
     for (int i = tid; i < TILE * 8; i += THREADS) {       // pad chunks of R / R_lo's 5th block stay zero
         const int r = i >> 3, c = i & 7;
-        *reinterpret_cast<float4*>(base + SM::off_R + EXTB * 8192 + sw128_32b_off(r, c)) = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (MODE == 3) *reinterpret_cast<float4*>(base + SM::off_Rlo + EXTB * 8192 + sw128_32b_off(r, c)) = make_float4(0.f, 0.f, 0.f, 0.f);
+        *reinterpret_cast<float4*>(base + SM::off_R + EXTB * 8192 + sw128_off(r, c)) = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (MODE == 3) *reinterpret_cast<float4*>(base + SM::off_Rlo + EXTB * 8192 + sw128_off(r, c)) = make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    fence_proxy_async_smem();
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem = *s_tmem;
 
-    // lane -> (row r of the warp's 16, half hf of the 128 basis columns); 16-B chunk walk rotated by the row so that every
-    // quarter-warp touches 8 distinct bank groups of the swizzled tile (used by the b.W and the R-row loops)
+    // lane -> (row r of the warp's 16, half hf of the 128 basis columns).  Every quarter-warp touches 8 distinct bank groups of the
+    // swizzled tile: the b.W loop walks logical chunks in step (the swizzle spreads them; the W reads are broadcasts), the R-row loop
+    // walks physical slots rotated by the row
     const int r16 = lane & 15, hf = lane >> 4;
 
     if (warp < W0) {
@@ -239,9 +233,9 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                 float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
                 for (int i = 0; i < 16; ++i) {
-                    const int blk = 2 * hf + (i >> 3), c = ((i & 7) + r16) & 7;
+                    const int blk = 2 * hf + (i >> 3), c = i & 7;
                     if (KBLK != 4 && blk >= KBLK) continue;
-                    const float4 bv = *reinterpret_cast<const float4*>(As + blk * 8192 + sw128_32b_off(nlr, c));
+                    const float4 bv = *reinterpret_cast<const float4*>(As + blk * 8192 + sw128_off(nlr, c));
                     const float4 w4 = *reinterpret_cast<const float4*>(myW + blk * 32 + c * 4);
                     acc.x = fmaf(bv.x, w4.x, acc.x); acc.y = fmaf(bv.y, w4.y, acc.y); acc.z = fmaf(bv.z, w4.z, acc.z); acc.w = fmaf(bv.w, w4.w, acc.w);
                     if constexpr (MODE == 1) {
@@ -253,14 +247,14 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                         uint32_t hsh = dseed ^ ((uint32_t)n * 0x9E3779B1u) ^ ((uint32_t)(blk * 8 + c) * 0x85EBCA77u);
                         hsh ^= hsh >> 16; hsh *= 0x7FEB352Du; hsh ^= hsh >> 15;
                         uint32_t hs2 = hsh * 0x846CA68Bu; hs2 ^= hs2 >> 16;
-                        *reinterpret_cast<float4*>(const_cast<unsigned char*>(As) + blk * 8192 + sw128_32b_off(nlr, c)) =
+                        *reinterpret_cast<float4*>(const_cast<unsigned char*>(As) + blk * 8192 + sw128_off(nlr, c)) =
                             make_float4(__uint_as_float((__float_as_uint(bv.x) + (hsh & 0x1fffu)) & 0xFFFFE000u),
                                         __uint_as_float((__float_as_uint(bv.y) + ((hsh >> 13) & 0x1fffu)) & 0xFFFFE000u),
                                         __uint_as_float((__float_as_uint(bv.z) + (hs2 & 0x1fffu)) & 0xFFFFE000u),
                                         __uint_as_float((__float_as_uint(bv.w) + ((hs2 >> 13) & 0x1fffu)) & 0xFFFFE000u));
                     }
                 }
-                if constexpr (MODE == 1) fence_proxy_async_smem();      // the MMA reads this stage through the async proxy
+                if constexpr (MODE == 1) fence_proxy_async_smem();      // generic writes before the TMA refill of this stage
                 mydot = (acc.x + acc.y) + (acc.z + acc.w);
                 mydot += __shfl_xor_sync(0xffffffffu, mydot, 16);
             }
@@ -335,9 +329,9 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
         }
     } else if (warp < W0 + GW) {
         // ===================================================================== gather warps: records -> taps -> M, q
-        setmaxnreg_inc<88>();
+        setmaxnreg_inc<112>();
         const int g = warp - W0, hw = lane >> 4, hl = lane & 15;
-        constexpr int PXW = TILE / GW;                       // 4 pixels per warp and tile
+        constexpr int PXW = TILE / GW;                       // 8 pixels per warp and tile
         constexpr int NUNIT = (PXW / 2) * NCH;
         float rb[NCH * 4];
 #pragma unroll
@@ -450,7 +444,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
         }
         if (cur_b >= 0) dump_rb();
     } else if (warp < W0 + GW + AW) {
-        // ===================================================================== algebra warps: 2x7 algebra, R rows, MMA + TMA issue
+        // ===================================================================== algebra warps: 2x7 algebra, R rows, TMA issue
         setmaxnreg_dec<72>();
         const int awi = warp - (W0 + GW);                    // 0..3: pixels / rows 16*awi .. 16*awi+15
         const int atid = tid - (W0 + GW) * 32;
@@ -463,12 +457,6 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
         int scale_b = -1, sspan = -1;
         float fx = 0.f, fy = 0.f;
         int rr = (ntiles > 0) ? (int)((unsigned)t_begin % (unsigned)prm.tiles_per_pair) : 0;
-        // issuer state (kept by every lane of warp 0, used by its lane 0)
-        constexpr uint32_t idesc = make_idesc_tf32_mn_mn(128, NMMA);
-        int chain = -1, tic = 0, set = 0, mspan = 0;
-        bool new_span = true;
-        uint32_t accH = 0, accL = 0;
-
         const uint64_t pol_basis = prm.l2_hints >= 1 ? l2_policy_evict_first() : l2_policy_evict_normal();     // the basis is read exactly once
         auto issue_tma = [&](int t) {                        // basis tile t -> stage t % NST (elected thread)
             const int st = t % NST;
@@ -484,7 +472,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                 for (int blk = 0; blk < KBLK; ++blk) tma_load_2d_hint(dst + blk * 8192, &tmapB, blk * 32, row, &fullB[st], pol_basis);
             }
         };
-        auto flush = [&](int sp) {
+        auto flush = [&](int sp) {               // H_cc / g_c / nvalid and rbar of the span (the MMA warps write H_dd and the [v | t] columns)
             float* slot = prm.partials + ((size_t)blockIdx.x * prm.max_span + sp) * prm.slot_floats;
             // H_cc / g_c / nvalid: 16 pixel-lanes -> warp total (fixed shuffle tree) -> 4 warp partials summed in fixed order
 #pragma unroll
@@ -563,11 +551,11 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
             if (lane < 16) {                                 // R columns 128..134 = [v(6) | t], column 135 stays zero
                 const float4 e0 = make_float4(tf32_rna(ext[0]), tf32_rna(ext[1]), tf32_rna(ext[2]), tf32_rna(ext[3]));
                 const float4 e1 = make_float4(tf32_rna(ext[4]), tf32_rna(ext[5]), tf32_rna(ext[6]), 0.f);
-                *reinterpret_cast<float4*>(Rs + EXTB * 8192 + sw128_32b_off(nlr, 0)) = e0;
-                *reinterpret_cast<float4*>(Rs + EXTB * 8192 + sw128_32b_off(nlr, 1)) = e1;
+                *reinterpret_cast<float4*>(Rs + EXTB * 8192 + sw128_off(nlr, 0)) = e0;
+                *reinterpret_cast<float4*>(Rs + EXTB * 8192 + sw128_off(nlr, 1)) = e1;
                 if constexpr (MODE == 3) {
-                    *reinterpret_cast<float4*>(base + SM::off_Rlo + EXTB * 8192 + sw128_32b_off(nlr, 0)) = make_float4(ext[0] - e0.x, ext[1] - e0.y, ext[2] - e0.z, ext[3] - e0.w);
-                    *reinterpret_cast<float4*>(base + SM::off_Rlo + EXTB * 8192 + sw128_32b_off(nlr, 1)) = make_float4(ext[4] - e1.x, ext[5] - e1.y, ext[6] - e1.z, 0.f);
+                    *reinterpret_cast<float4*>(base + SM::off_Rlo + EXTB * 8192 + sw128_off(nlr, 0)) = make_float4(ext[0] - e0.x, ext[1] - e0.y, ext[2] - e0.z, ext[3] - e0.w);
+                    *reinterpret_cast<float4*>(base + SM::off_Rlo + EXTB * 8192 + sw128_off(nlr, 1)) = make_float4(ext[4] - e1.x, ext[5] - e1.y, ext[6] - e1.z, 0.f);
                 }
             }
             // R rows (and the split parts): elementwise on the lane's half row, so walk the PHYSICAL 16-B slots (rotated by the row: every
@@ -588,117 +576,77 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                 if constexpr (MODE == 3)
                     *reinterpret_cast<float4*>(base + SM::off_Rlo + off) = make_float4(pv.x - hv.x, pv.y - hv.y, pv.z - hv.z, pv.w - hv.w);
             }
-            fence_proxy_async_smem();
             if (awi == 0) TC6_TRACE(1, j, 4);
-            team_bar<AW * 32>();                           // all 64 rows written
-            if (awi == 0) {
-                if (lane == 0) {                             // ---- tcgen05.mma issue for this tile
-                    if (new_span) { mbar_wait_parked(tmemfree, (mspan & 1) ^ 1); accL = 0; new_span = false; }
-                    if (tic == 0) { ++chain; set = chain & 1; mbar_wait_parked(&drained[set], ((chain >> 1) & 1) ^ 1); accH = 0; }
-                    tc_fence_after_sync();
-                    const uint32_t ahi = smem_u32(base + SM::off_A + s * STAGE_A);
-                    const uint32_t rhi = smem_u32(base + SM::off_R), rlo = smem_u32(base + SM::off_Rlo), alo = smem_u32(base + SM::off_Alo);
-#pragma unroll
-                    for (int pass = 0; pass < MODE; ++pass) {
-                        const uint32_t a0 = (pass == 1) ? alo : ahi;
-                        const uint32_t r0 = (pass == 2) ? rlo : rhi;
-                        const uint32_t dcol = tmem + (pass == 0 ? set * NN : ACCL);
-#pragma unroll
-                        for (int kk = 0; kk < TILE / 8; ++kk) {
-                            mma_tf32_ss(dcol, make_desc_mn_sw128_32b(a0 + kk * 1024, 8192, 512),
-                                        make_desc_mn_sw128_32b(r0 + kk * 1024, 8192, 512), idesc, pass == 0 ? accH : accL);
-                            if (pass == 0) accH = 1; else accL = 1;
-                        }
-                    }
-                    mma_commit(rfree);
-                    if (++tic == CHAIN) { mma_commit(&chain_done[set]); tic = 0; }
-                    if (last_of_pair) { if (tic > 0) mma_commit(&chain_done[set]); mma_commit(flushb); ++mspan; tic = 0; new_span = true; }
-                }
-                __syncwarp();
-            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(rready);
             if (awi == 0) TC6_TRACE(1, j, 5);
             if (last_of_pair) flush(sspan);
         }
     } else {
-        // ===================================================================== drainer warps: TMEM -> partial slots, fully asynchronous
-        setmaxnreg_dec<32>();
-        const int dq = warp - (W0 + GW + AW);                // TMEM lane quadrant (= warp % 4)
+        // ===================================================================== MMA warps: D = A^T R per tile, accumulated over the pair span
+        setmaxnreg_inc<136>();
+        const int mw = warp - (W0 + GW + AW), g = lane >> 2, t = lane & 3;
         const SlotLayout L{KR, C};
-        // The CTA's partial slot (<= 2 x 68 KB) is read-modify-written once per chain of CHAIN tiles.  Left to the default policy the streaming
-        // inputs push it out of L2 between two chains: ncu showed 1.3 GB of DRAM writes per launch (and as many reads) for a kernel that writes
-        // 20 MB of results.  evict-last keeps the 20 MB of slots of all CTAs resident.
-        const uint64_t pol_slot = l2_policy_evict_last();
-        auto drain_region = [&](float* slot, uint32_t col0, bool overwrite) {
-            const int row = dq * 32 + lane;
-            if (KBLK != 4 && dq * 32 >= KR) return;          // this lane quadrant holds no basis row (warp-uniform)
-            const uint32_t tq = tmem + ((uint32_t)(dq * 32) << 16) + col0;
-            float v[16];
+        // lm_reduce reads the lower block triangle of H_dd only (and mirrors it): m-block i (rows 16i .. 16i+15 of D) needs the n8 column
+        // blocks 0 .. 2i+1, plus the [v | t] block (columns KR .. KR+7).  With 8 m-blocks warp mw takes m-blocks mw and 7-mw: 20 n8 blocks
+        // for every warp.  K = 64 / 32: one m-block per warp.
+        constexpr int NMB = KR / 16, NQ = NMB == 8 ? 20 : 2 * NMB + 1;
+        const int mb0 = mw, mb1 = NMB == 8 ? 7 - mw : -1;
+        const int cnt0 = mw < NMB ? 2 * mb0 + 3 : 0;         // n8 blocks of m-block mb0; the rest of the NQ belong to mb1
+        auto col_of = [&](int q) {                           // first column of accumulator block q (warp-uniform)
+            const int lq = q < cnt0 ? q : q - cnt0, cq = q < cnt0 ? cnt0 : NQ - cnt0;
+            return lq == cq - 1 ? KR : 8 * lq;
+        };
+        float acc[NQ][4];
+#pragma unroll
+        for (int q = 0; q < NQ; ++q) acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.f;
+        const uint32_t rhi = smem_u32(base + SM::off_R), rlo = smem_u32(base + SM::off_Rlo), alo = smem_u32(base + SM::off_Alo);
+        int span = 0;
+        int rr = (ntiles > 0) ? (int)((unsigned)t_begin % (unsigned)prm.tiles_per_pair) : 0;
+        for (int j = 0; j < ntiles; ++j) {
+            const int s = j % NST;
+            mbar_wait_parked(rready, j & 1);
+            mbar_wait_parked(&fullB[s], (j / NST) & 1);      // orders the TMA writes of the stage before the fragment loads
+            const uint32_t ahi = smem_u32(base + SM::off_A + s * STAGE_A);
 #pragma unroll 1
-            for (int cb = 0; cb < KR / 16; ++cb) {
-                tmem_ld_32x16(tq + cb * 16, v);
-                float* dst = slot + (size_t)(cb * 16) * KR + row;
-                if (overwrite) {
+            for (int pass = 0; pass < MODE; ++pass) {        // hi x hi, then A_lo x R, then A x R_lo, into the same accumulators
+                const uint32_t a = pass == 1 ? alo : ahi, r = pass == 2 ? rlo : rhi;
+#pragma unroll 2
+                for (int kk = 0; kk < TILE / 8; ++kk) {
+                    uint32_t f0[4] = {0u, 0u, 0u, 0u}, f1[4] = {0u, 0u, 0u, 0u};
+                    if (cnt0 > 0) load_a_frag(f0, a, 16 * mb0, kk, lane);
+                    if (mb1 >= 0) load_a_frag(f1, a, 16 * mb1, kk, lane);
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) st_f32_hint(dst + (size_t)j * KR, v[j], pol_slot);
-                } else {
-#pragma unroll
-                    for (int hb = 0; hb < 16; hb += 8) {     // 8 columns at a time: the drainers live on 32 registers
-                        float o[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) o[j] = ld_f32_hint(dst + (size_t)(hb + j) * KR, pol_slot);
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) st_f32_hint(dst + (size_t)(hb + j) * KR, o[j] + v[hb + j], pol_slot);
+                    for (int q = 0; q < NQ; ++q) {
+                        if (q >= cnt0 && mb1 < 0) continue;
+                        const bool first = q < cnt0;
+                        const uint32_t af[4] = {first ? f0[0] : f1[0], first ? f0[1] : f1[1], first ? f0[2] : f1[2], first ? f0[3] : f1[3]};
+                        mma_step_rn(acc[q], af, r, col_of(q), kk, lane);
                     }
                 }
             }
-            tmem_ld_32x16(tq + KR, v);
-            float* dst = slot + L.off_ext() + row;
-#pragma unroll
-            for (int r = 0; r < 7; ++r) {
-                if (overwrite) st_f32_hint(dst + r * KR, v[r], pol_slot);
-                else st_f32_hint(dst + r * KR, ld_f32_hint(dst + r * KR, pol_slot) + v[r], pol_slot);
-            }
-        };
-        int chain = -1, tic = 0, span = 0, cur_b = -1;
-        bool first = true;
-        int b = (ntiles > 0) ? (int)((unsigned)t_begin / (unsigned)prm.tiles_per_pair) : 0;
-        int rr = (ntiles > 0) ? (int)((unsigned)t_begin - (unsigned)b * (unsigned)prm.tiles_per_pair) : 0;
-        auto drain_hi = [&]() {
-            const int set = chain & 1;
-            float* slot = prm.partials + ((size_t)blockIdx.x * prm.max_span + span) * prm.slot_floats;
-            mbar_wait_parked(&chain_done[set], (chain >> 1) & 1);
-            tc_fence_after_sync();
-            drain_region(slot, set * NN, first);
-            first = false;
-            tc_fence_before_sync();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&drained[set]);
-        };
-        auto end_span = [&]() {
-            if (tic > 0) drain_hi();
-            if constexpr (MODE >= 2) {
+            if (lane == 0) mbar_arrive(rfree);
+            const bool last_of_pair = (++rr == prm.tiles_per_pair) || (j == ntiles - 1);
+            if (rr == prm.tiles_per_pair) rr = 0;
+            if (last_of_pair) {                              // slot of the span: H_dd column-major (hdd_transposed), ext rows [v | t]
                 float* slot = prm.partials + ((size_t)blockIdx.x * prm.max_span + span) * prm.slot_floats;
-                mbar_wait_parked(flushb, span & 1);
-                tc_fence_after_sync();
-                drain_region(slot, ACCL, false);
-                tc_fence_before_sync();
+#pragma unroll
+                for (int q = 0; q < NQ; ++q) {
+                    if (q >= cnt0 && mb1 < 0) continue;
+                    const int i0 = 16 * (q < cnt0 ? mb0 : mb1) + g, n0 = col_of(q) + 2 * t;
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const int i = i0 + (e >> 1) * 8, n = n0 + (e & 1);
+                        if (n < KR) slot[(size_t)n * KR + i] = acc[q][e];
+                        else if (n - KR < 7) slot[L.off_ext() + (n - KR) * KR + i] = acc[q][e];
+                        acc[q][e] = 0.f;
+                    }
+                }
+                ++span;
             }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tmemfree);
-            ++span;
-        };
-        for (int it = 0; it < ntiles; ++it) {
-            if (b != cur_b) { if (cur_b >= 0) end_span(); cur_b = b; tic = 0; first = true; }
-            if (tic == 0) ++chain;
-            if (++tic == CHAIN) { drain_hi(); tic = 0; }
-            if (++rr == prm.tiles_per_pair) { rr = 0; ++b; }
         }
-        if (cur_b >= 0) end_span();
     }
-
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<TMEM_COLS>(tmem);
 }
 
 template <int NCH, bool FLY, int MODE, int KBLK = 4>

@@ -19,10 +19,13 @@
 //   division of labour (measured, profiles/r02b_*: with the taps on LDS the kernel turned instruction-issue / role-latency bound, so work moved to
 //                 where the warps are): the 16 gather warps also derive s_n = jd^T M jd and write the MMA operands of their pixel — the R row
 //                 rna(s_n b_n) and the precision mode's side of the basis tile (stochastic tf32 rounding in place, or A_lo) — which the 4
-//                 algebra warps did in generation 6; the geometry warps only form b.W and the warp; the per-channel arithmetic runs on packed
-//                 fp32 pairs (FFMA2 / FMUL2 / FADD2); conv1 arrives with the window (one 4-D TMA box {32 ch, 8, 8, pair} per chunk).
+//                 algebra warps did in generation 6; the geometry warps only form b.W and the warp; the per-channel arithmetic runs on fp32
+//                 channel pairs; conv1 arrives with the window (one 4-D TMA box {32 ch, 8, 8, pair} per chunk).
 //
-// Roles (896 threads, 1 CTA / SM) and barriers as generation 6, plus winfull[NWB] (TMA landed, count 1 + tx) / winfree[NWB] (count GW).
+// Roles (896 threads, 1 CTA / SM; setmaxnreg budgets 48 / 64 / 64 / 136 = 64 512 registers): 4 geometry, 16 gather, 4 algebra warps and
+// 4 MMA warps that contract each tile with mma.sync tf32 into register accumulators as in generation 6 (tc_utils.cuh: mma_step_rn).
+// Barriers as generation 6 (rready / rfree between the algebra, gather and MMA warps), plus winfull[NWB] (TMA landed, count 1 + tx) /
+// winfree[NWB] (count GW).
 #include "common.cuh"
 #include "lm_build.h"
 #include "tc_utils.cuh"
@@ -32,12 +35,10 @@
 namespace banet { namespace v7 {
 using namespace tc;
 
-constexpr int TILE = 64, W0 = 4, GW = 16, AW = 4, DW = 4;      // geometry | gather | algebra | drainer warps
-constexpr int THREADS = (W0 + GW + AW + DW) * 32;               // 896
-constexpr int NN = 160;
+constexpr int TILE = 64, W0 = 4, GW = 16, AW = 4, MW = 4;      // geometry | gather | algebra | MMA warps
+constexpr int THREADS = (W0 + GW + AW + MW) * 32;               // 896
 constexpr int STAGE_A = 4 * TILE * 128, STAGE_R = 5 * TILE * 128;
 constexpr int REC = 16;
-constexpr int CHAIN = 8, TMEM_COLS = 512, ACCL = 320;
 #ifndef BANET_TC7_WX
 #define BANET_TC7_WX 13
 #endif
@@ -76,7 +77,6 @@ template <int MODE, int NCH> struct Smem {
     static constexpr int off_win = off_Rlo;                            // [NWB] x ([WY][WX][32] floats F2 window chunk | [64][32] floats conv1 chunk)
     static constexpr int off_misc = off_win + NWB * WBUF;
     static constexpr int off_bar = off_misc;                           // 22 + 2*NWB mbarriers (<= 30)
-    static constexpr int off_tmem = off_bar + 30 * 8;
     static constexpr int off_tile = off_misc + 256;                    // [NREC][8] ints: pair, tx0, ty0, fx, fy (float bits), dither seed of the tile in record buffer s
     static constexpr int off_box = off_tile + 128;                     // [NREC][W0][4] ints: tap bounding box (xmin,xmax,ymin,ymax) per geometry warp
     static constexpr int off_pose = off_box + NREC * W0 * 16;          // [W0][16] floats (private to each geometry warp)
@@ -85,10 +85,10 @@ template <int MODE, int NCH> struct Smem {
     static constexpr int off_rbs = off_rec + NREC * TILE * REC * 4;    // [GW][128] floats: rbar hand-over gather -> algebra
     static constexpr int off_ccs = off_rbs + GW * 128 * 4;             // [AW][28] floats: H_cc / g_c / nvalid partials per algebra warp
     static constexpr int total = off_ccs + AW * 28 * 4;
-    static constexpr int slack = 512;
+    static constexpr int slack = 1024;                                 // stage bases 1024-B aligned (128B swizzle atoms)
     static constexpr int bytes = total + slack;
     static_assert(NWB >= 2 && NWB <= 4 && NST <= 4 && WIN_BYTES % 128 == 0, "ring sizes");
-    static_assert(bytes <= 232448, "shared memory budget of one sm_100 CTA");
+    static_assert(bytes <= 232448, "shared memory budget of one sm_90 CTA");
 };
 
 template <int NT> __device__ __forceinline__ void team_bar() { asm volatile("bar.sync 2, %0;" :: "n"(NT) : "memory"); }
@@ -99,13 +99,16 @@ __device__ __forceinline__ float4 lds4(uint32_t saddr) {
     asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "r"(saddr));
     return r;
 }
-// packed fp32 pairs (sm_100: FFMA2 / FMUL2 / FADD2, one issue slot for two lanes' worth of channels; a (w, w) pair is encoded as a scalar broadcast)
+// fp32 channel pairs: two lanes' worth of channels per value (a (w, w) pair is a scalar broadcast); Hopper has no packed fp32
+// instructions, so each operation is two scalar ones with the same rounding
 typedef unsigned long long u64;
 __device__ __forceinline__ u64 pk2(float a, float b) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b)); return r; }
 __device__ __forceinline__ float2 upk2(u64 v) { float2 r; asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v)); return r; }
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) { u64 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-__device__ __forceinline__ u64 mul2(u64 a, u64 b) { u64 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ u64 sub2(u64 a, u64 b) { u64 d; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
+__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) {
+    const float2 x = upk2(a), y = upk2(b), z = upk2(c); return pk2(__fmaf_rn(x.x, y.x, z.x), __fmaf_rn(x.y, y.y, z.y));
+}
+__device__ __forceinline__ u64 mul2(u64 a, u64 b) { const float2 x = upk2(a), y = upk2(b); return pk2(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y)); }
+__device__ __forceinline__ u64 sub2(u64 a, u64 b) { const float2 x = upk2(a), y = upk2(b); return pk2(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y)); }
 __device__ __forceinline__ ulonglong2 lds2x64(uint32_t saddr) {
     ulonglong2 r;
     asm volatile("ld.shared.v2.b64 {%0,%1}, [%2];" : "=l"(r.x), "=l"(r.y) : "r"(saddr));
@@ -162,17 +165,14 @@ lm_build_tc7_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_cons
 {
     using SM = Smem<MODE, NCH>;
     constexpr int NST = SM::NST, NREC = SM::NREC, NWB = SM::NWB;
-    constexpr int KR = 32 * KBLK, EXTB = KBLK, NMMA = KBLK == 4 ? NN : KR + 16;
+    constexpr int KR = 32 * KBLK, EXTB = KBLK;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     // align through the 32-bit shared address so that the compiler keeps every access in the shared state space (LDS/STS, not generic LD/ST)
-    unsigned char* base = smem_raw + ((512u - (smem_u32(smem_raw) & 511u)) & 511u);
+    unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint64_t* bars = reinterpret_cast<uint64_t*>(base + SM::off_bar);
     uint64_t* fullB = bars;            // [NST]  TMA landed
-    uint64_t* rfree = bars + 4;        //        MMAs of the tile completed
-    uint64_t* flushb = bars + 5;       //        every MMA of the span completed
-    uint64_t* tmemfree = bars + 6;     //        lo accumulator drained
-    uint64_t* chain_done = bars + 7;   // [2]
-    uint64_t* drained = bars + 9;      // [2]
+    uint64_t* rfree = bars + 4;        //        MMAs of the tile completed (count MW)
+    uint64_t* rready = bars + 5;       //        [v | t] block written: every MMA operand of the tile is in place (count AW)
     uint64_t* recs = bars + 11;        // [NREC] records of the tile in buffer s written (count W0)
     uint64_t* gath = bars + 14;        // [NREC] M,q of the tile in buffer s written (count GW)
     uint64_t* recfree = bars + 17;     // [NREC] records of the tile in buffer s consumed by the algebra warps (count AW)
@@ -180,7 +180,6 @@ lm_build_tc7_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_cons
     uint64_t* rbfree = bars + 21;      //        algebra warps consumed them (count AW)
     uint64_t* winfull = bars + 22;     // [NWB]  window chunk landed (count 1 + tx bytes; plain arrive for a direct-tap tile)
     uint64_t* winfree = bars + 26;     // [NWB]  window chunk consumed by the gather warps (count GW)
-    uint32_t* s_tmem = reinterpret_cast<uint32_t*>(base + SM::off_tmem);
     int* sTile = reinterpret_cast<int*>(base + SM::off_tile);
     int* sBox = reinterpret_cast<int*>(base + SM::off_box);
     float* sPose = reinterpret_cast<float*>(base + SM::off_pose);
@@ -201,22 +200,16 @@ lm_build_tc7_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_cons
         for (int i = 0; i < NST; ++i) mbar_init(&fullB[i], 1);
         for (int i = 0; i < NREC; ++i) { mbar_init(&recs[i], W0); mbar_init(&gath[i], GW); mbar_init(&recfree[i], AW); }
         for (int i = 0; i < NWB; ++i) { mbar_init(&winfull[i], 1); mbar_init(&winfree[i], GW); }
-        mbar_init(rfree, 1); mbar_init(flushb, 1); mbar_init(tmemfree, DW);
-        mbar_init(&chain_done[0], 1); mbar_init(&chain_done[1], 1); mbar_init(&drained[0], DW); mbar_init(&drained[1], DW);
+        mbar_init(rfree, MW); mbar_init(rready, AW);
         mbar_init(rbdump, GW); mbar_init(rbfree, AW);
         fence_barrier_init();
         prefetch_tmap(&tmapB); prefetch_tmap(&tmapF); prefetch_tmap(&tmapC);
     }
-    if (warp == 0) tmem_alloc<TMEM_COLS>(s_tmem);
     for (int i = tid; i < TILE * 8; i += THREADS) {       // pad chunks of R's 5th block stay zero
         const int r = i >> 3, c = i & 7;
-        *reinterpret_cast<float4*>(base + SM::off_R + EXTB * 8192 + sw128_32b_off(r, c)) = make_float4(0.f, 0.f, 0.f, 0.f);
+        *reinterpret_cast<float4*>(base + SM::off_R + EXTB * 8192 + sw128_off(r, c)) = make_float4(0.f, 0.f, 0.f, 0.f);
     }
-    fence_proxy_async_smem();
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem = *s_tmem;
 
     // lane -> (row r of the warp's 16, half hf of the 128 basis columns); 16-B chunk walk rotated by the row so that every
     // quarter-warp touches 8 distinct bank groups of the swizzled tile (used by the b.W and the R-row loops)
@@ -287,9 +280,9 @@ lm_build_tc7_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_cons
                 float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
                 for (int i = 0; i < 16; ++i) {
-                    const int blk = 2 * hf + (i >> 3), c = ((i & 7) + r16) & 7;
+                    const int blk = 2 * hf + (i >> 3), c = i & 7;
                     if (KBLK != 4 && blk >= KBLK) continue;
-                    const float4 bv = *reinterpret_cast<const float4*>(As + blk * 8192 + sw128_32b_off(nlr, c));
+                    const float4 bv = *reinterpret_cast<const float4*>(As + blk * 8192 + sw128_off(nlr, c));
                     const float4 w4 = *reinterpret_cast<const float4*>(myW + blk * 32 + c * 4);
                     acc.x = fmaf(bv.x, w4.x, acc.x); acc.y = fmaf(bv.y, w4.y, acc.y); acc.z = fmaf(bv.z, w4.z, acc.z); acc.w = fmaf(bv.w, w4.w, acc.w);
                 }
@@ -341,7 +334,7 @@ lm_build_tc7_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_cons
         }
     } else if (warp < W0 + GW) {
         // ===================================================================== gather warps: records -> staged taps (LDS) -> M, q
-        setmaxnreg_inc<88>();
+        setmaxnreg_dec<64>();
         const int g = warp - W0, pq = lane >> 3, ql = lane & 7;          // quarter-warp pq handles pixel g*4+pq; lane ql its channels 4*ql..+3 of a chunk
         constexpr int NCHK = C / CHK;
         const int nchunks = ntiles * NCHK;
@@ -522,7 +515,7 @@ lm_build_tc7_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_cons
                 mbar_wait_parked(&fullB[st], (j / NST) & 1);                  // long complete (the geometry warps needed it)
                 unsigned char* As = base + SM::off_A + st * STAGE_A;
                 unsigned char* Rs = base + SM::off_R;
-                const uint32_t rowo = sw128_32b_off(pxi, ql);
+                const uint32_t rowo = sw128_off(pxi, ql);
                 uint32_t hbase = 0;
                 if constexpr (MODE == 1) hbase = (uint32_t)sTile[s * 8 + 5] ^ ((uint32_t)__float_as_int(rgeo.w) * 0x9E3779B1u);
 #pragma unroll
@@ -546,13 +539,13 @@ lm_build_tc7_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_cons
                         *reinterpret_cast<float4*>(base + SM::off_Alo + off) = make_float4(bv.x - tf32_trunc(bv.x), bv.y - tf32_trunc(bv.y), bv.z - tf32_trunc(bv.z), bv.w - tf32_trunc(bv.w));
                 }
             }
-            fence_proxy_async_smem();                        // the MMA reads R / A / A_lo through the async proxy
+            if constexpr (MODE == 1) fence_proxy_async_smem();      // generic writes before the TMA refill of this stage
             __syncwarp();
             if (lane == 0) mbar_arrive(&gath[s]);
         }
         if (cur_b >= 0) dump_rb();
     } else if (warp < W0 + GW + AW) {
-        // ===================================================================== algebra warps: 2x7 algebra (H_cc, g_c, [v | t]), MMA + TMA issue
+        // ===================================================================== algebra warps: 2x7 algebra (H_cc, g_c, [v | t]), TMA issue
         setmaxnreg_dec<64>();
         const int awi = warp - (W0 + GW);                    // 0..3: pixels / rows 16*awi .. 16*awi+15
         const int atid = tid - (W0 + GW) * 32;
@@ -565,11 +558,6 @@ lm_build_tc7_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_cons
         int scale_b = -1, sspan = -1;
         float fx = 0.f, fy = 0.f;
         int rr = (ntiles > 0) ? (int)((unsigned)t_begin % (unsigned)prm.tiles_per_pair) : 0;
-        // issuer state (kept by every lane of warp 0, used by its lane 0)
-        constexpr uint32_t idesc = make_idesc_tf32_mn_mn(128, NMMA);
-        int chain = -1, tic = 0, set = 0, mspan = 0;
-        bool new_span = true;
-        uint32_t accH = 0, accL = 0;
 
         auto issue_tma = [&](int t) {                        // basis tile t -> stage t % NST (elected thread)
             const int st = t % NST;
@@ -661,120 +649,83 @@ lm_build_tc7_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_cons
             if (lane < 16) {                                 // R columns 128..134 = [v(6) | t], column 135 stays zero
                 const float4 e0 = make_float4(tf32_rna(ext[0]), tf32_rna(ext[1]), tf32_rna(ext[2]), tf32_rna(ext[3]));
                 const float4 e1 = make_float4(tf32_rna(ext[4]), tf32_rna(ext[5]), tf32_rna(ext[6]), 0.f);
-                *reinterpret_cast<float4*>(Rs + EXTB * 8192 + sw128_32b_off(nlr, 0)) = e0;
-                *reinterpret_cast<float4*>(Rs + EXTB * 8192 + sw128_32b_off(nlr, 1)) = e1;
+                *reinterpret_cast<float4*>(Rs + EXTB * 8192 + sw128_off(nlr, 0)) = e0;
+                *reinterpret_cast<float4*>(Rs + EXTB * 8192 + sw128_off(nlr, 1)) = e1;
                 if constexpr (MODE == 3) {
-                    *reinterpret_cast<float4*>(base + SM::off_Rlo + EXTB * 8192 + sw128_32b_off(nlr, 0)) = make_float4(ext[0] - e0.x, ext[1] - e0.y, ext[2] - e0.z, ext[3] - e0.w);
-                    *reinterpret_cast<float4*>(base + SM::off_Rlo + EXTB * 8192 + sw128_32b_off(nlr, 1)) = make_float4(ext[4] - e1.x, ext[5] - e1.y, ext[6] - e1.z, 0.f);
+                    *reinterpret_cast<float4*>(base + SM::off_Rlo + EXTB * 8192 + sw128_off(nlr, 0)) = make_float4(ext[0] - e0.x, ext[1] - e0.y, ext[2] - e0.z, ext[3] - e0.w);
+                    *reinterpret_cast<float4*>(base + SM::off_Rlo + EXTB * 8192 + sw128_off(nlr, 1)) = make_float4(ext[4] - e1.x, ext[5] - e1.y, ext[6] - e1.z, 0.f);
                 }
             }
             // (the R rows s_n * b_n were written by the gather warps' scaling pass; this team only adds the [v | t] block)
-            fence_proxy_async_smem();
-            team_bar<AW * 32>();                           // all 64 rows written
-            if (awi == 0) {
-                if (lane == 0) {                             // ---- tcgen05.mma issue for this tile
-                    if (new_span) { mbar_wait_parked(tmemfree, (mspan & 1) ^ 1); accL = 0; new_span = false; }
-                    if (tic == 0) { ++chain; set = chain & 1; mbar_wait_parked(&drained[set], ((chain >> 1) & 1) ^ 1); accH = 0; }
-                    tc_fence_after_sync();
-                    const uint32_t ahi = smem_u32(base + SM::off_A + s * STAGE_A);
-                    const uint32_t rhi = smem_u32(base + SM::off_R), rlo = smem_u32(base + SM::off_Rlo), alo = smem_u32(base + SM::off_Alo);
-#pragma unroll
-                    for (int pass = 0; pass < MODE; ++pass) {
-                        const uint32_t a0 = (pass == 1) ? alo : ahi;
-                        const uint32_t r0 = (pass == 2) ? rlo : rhi;
-                        const uint32_t dcol = tmem + (pass == 0 ? set * NN : ACCL);
-#pragma unroll
-                        for (int kk = 0; kk < TILE / 8; ++kk) {
-                            mma_tf32_ss(dcol, make_desc_mn_sw128_32b(a0 + kk * 1024, 8192, 512),
-                                        make_desc_mn_sw128_32b(r0 + kk * 1024, 8192, 512), idesc, pass == 0 ? accH : accL);
-                            if (pass == 0) accH = 1; else accL = 1;
-                        }
-                    }
-                    mma_commit(rfree);
-                    if (++tic == CHAIN) { mma_commit(&chain_done[set]); tic = 0; }
-                    if (last_of_pair) { if (tic > 0) mma_commit(&chain_done[set]); mma_commit(flushb); ++mspan; tic = 0; new_span = true; }
-                }
-                __syncwarp();
-            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(rready);
             if (last_of_pair) flush(sspan);
         }
     } else {
-        // ===================================================================== drainer warps: TMEM -> partial slots, fully asynchronous
-        setmaxnreg_dec<40>();
-        const int dq = warp - (W0 + GW + AW);                // TMEM lane quadrant (= warp % 4)
+        // ===================================================================== MMA warps: D = A^T R per tile, accumulated over the pair span
+        setmaxnreg_inc<136>();
+        const int mw = warp - (W0 + GW + AW), g = lane >> 2, t = lane & 3;
         const SlotLayout L{KR, C};
-        const uint64_t pol_slot = l2_policy_evict_last();    // keep the CTA's partial slot L2-resident between two chains (see lm_build_tc6.cu)
-        auto drain_region = [&](float* slot, uint32_t col0, bool overwrite) {
-            const int row = dq * 32 + lane;
-            if (KBLK != 4 && dq * 32 >= KR) return;          // this lane quadrant holds no basis row (warp-uniform)
-            const uint32_t tq = tmem + ((uint32_t)(dq * 32) << 16) + col0;
-            float v[16];
+        // lm_reduce reads the lower block triangle of H_dd only (and mirrors it): m-block i (rows 16i .. 16i+15 of D) needs the n8 column
+        // blocks 0 .. 2i+1, plus the [v | t] block (columns KR .. KR+7).  With 8 m-blocks warp mw takes m-blocks mw and 7-mw: 20 n8 blocks
+        // for every warp.  K = 64 / 32: one m-block per warp.
+        constexpr int NMB = KR / 16, NQ = NMB == 8 ? 20 : 2 * NMB + 1;
+        const int mb0 = mw, mb1 = NMB == 8 ? 7 - mw : -1;
+        const int cnt0 = mw < NMB ? 2 * mb0 + 3 : 0;         // n8 blocks of m-block mb0; the rest of the NQ belong to mb1
+        auto col_of = [&](int q) {                           // first column of accumulator block q (warp-uniform)
+            const int lq = q < cnt0 ? q : q - cnt0, cq = q < cnt0 ? cnt0 : NQ - cnt0;
+            return lq == cq - 1 ? KR : 8 * lq;
+        };
+        float acc[NQ][4];
+#pragma unroll
+        for (int q = 0; q < NQ; ++q) acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.f;
+        const uint32_t rhi = smem_u32(base + SM::off_R), rlo = smem_u32(base + SM::off_Rlo), alo = smem_u32(base + SM::off_Alo);
+        int span = 0;
+        int rr = (ntiles > 0) ? (int)((unsigned)t_begin % (unsigned)prm.tiles_per_pair) : 0;
+        for (int j = 0; j < ntiles; ++j) {
+            const int s = j % NST;
+            mbar_wait_parked(rready, j & 1);
+            mbar_wait_parked(&fullB[s], (j / NST) & 1);      // orders the TMA writes of the stage before the fragment loads
+            const uint32_t ahi = smem_u32(base + SM::off_A + s * STAGE_A);
 #pragma unroll 1
-            for (int cb = 0; cb < KR / 16; ++cb) {
-                tmem_ld_32x16(tq + cb * 16, v);
-                float* dst = slot + (size_t)(cb * 16) * KR + row;
-                if (overwrite) {
+            for (int pass = 0; pass < MODE; ++pass) {        // hi x hi, then A_lo x R, then A x R_lo, into the same accumulators
+                const uint32_t a = pass == 1 ? alo : ahi, r = pass == 2 ? rlo : rhi;
+#pragma unroll 2
+                for (int kk = 0; kk < TILE / 8; ++kk) {
+                    uint32_t f0[4] = {0u, 0u, 0u, 0u}, f1[4] = {0u, 0u, 0u, 0u};
+                    if (cnt0 > 0) load_a_frag(f0, a, 16 * mb0, kk, lane);
+                    if (mb1 >= 0) load_a_frag(f1, a, 16 * mb1, kk, lane);
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) st_f32_hint(dst + (size_t)j * KR, v[j], pol_slot);
-                } else {
-#pragma unroll
-                    for (int hb = 0; hb < 16; hb += 8) {
-                        float o[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) o[j] = ld_f32_hint(dst + (size_t)(hb + j) * KR, pol_slot);
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) st_f32_hint(dst + (size_t)(hb + j) * KR, o[j] + v[hb + j], pol_slot);
+                    for (int q = 0; q < NQ; ++q) {
+                        if (q >= cnt0 && mb1 < 0) continue;
+                        const bool first = q < cnt0;
+                        const uint32_t af[4] = {first ? f0[0] : f1[0], first ? f0[1] : f1[1], first ? f0[2] : f1[2], first ? f0[3] : f1[3]};
+                        mma_step_rn(acc[q], af, r, col_of(q), kk, lane);
                     }
                 }
             }
-            tmem_ld_32x16(tq + KR, v);
-            float* dst = slot + L.off_ext() + row;
-#pragma unroll
-            for (int r = 0; r < 7; ++r) {
-                if (overwrite) st_f32_hint(dst + r * KR, v[r], pol_slot);
-                else st_f32_hint(dst + r * KR, ld_f32_hint(dst + r * KR, pol_slot) + v[r], pol_slot);
-            }
-        };
-        int chain = -1, tic = 0, span = 0, cur_b = -1;
-        bool first = true;
-        int b = (ntiles > 0) ? (int)((unsigned)t_begin / (unsigned)prm.tiles_per_pair) : 0;
-        int rr = (ntiles > 0) ? (int)((unsigned)t_begin - (unsigned)b * (unsigned)prm.tiles_per_pair) : 0;
-        auto drain_hi = [&]() {
-            const int set = chain & 1;
-            float* slot = prm.partials + ((size_t)blockIdx.x * prm.max_span + span) * prm.slot_floats;
-            mbar_wait_parked(&chain_done[set], (chain >> 1) & 1);
-            tc_fence_after_sync();
-            drain_region(slot, set * NN, first);
-            first = false;
-            tc_fence_before_sync();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&drained[set]);
-        };
-        auto end_span = [&]() {
-            if (tic > 0) drain_hi();
-            if constexpr (MODE >= 2) {
+            if (lane == 0) mbar_arrive(rfree);
+            const bool last_of_pair = (++rr == prm.tiles_per_pair) || (j == ntiles - 1);
+            if (rr == prm.tiles_per_pair) rr = 0;
+            if (last_of_pair) {                              // slot of the span: H_dd column-major (hdd_transposed), ext rows [v | t]
                 float* slot = prm.partials + ((size_t)blockIdx.x * prm.max_span + span) * prm.slot_floats;
-                mbar_wait_parked(flushb, span & 1);
-                tc_fence_after_sync();
-                drain_region(slot, ACCL, false);
-                tc_fence_before_sync();
+#pragma unroll
+                for (int q = 0; q < NQ; ++q) {
+                    if (q >= cnt0 && mb1 < 0) continue;
+                    const int i0 = 16 * (q < cnt0 ? mb0 : mb1) + g, n0 = col_of(q) + 2 * t;
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        const int i = i0 + (e >> 1) * 8, n = n0 + (e & 1);
+                        if (n < KR) slot[(size_t)n * KR + i] = acc[q][e];
+                        else if (n - KR < 7) slot[L.off_ext() + (n - KR) * KR + i] = acc[q][e];
+                        acc[q][e] = 0.f;
+                    }
+                }
+                ++span;
             }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tmemfree);
-            ++span;
-        };
-        for (int it = 0; it < ntiles; ++it) {
-            if (b != cur_b) { if (cur_b >= 0) end_span(); cur_b = b; tic = 0; first = true; }
-            if (tic == 0) ++chain;
-            if (++tic == CHAIN) { drain_hi(); tic = 0; }
-            if (++rr == prm.tiles_per_pair) { rr = 0; ++b; }
         }
-        if (cur_b >= 0) end_span();
     }
-
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<TMEM_COLS>(tmem);
 }
 
 

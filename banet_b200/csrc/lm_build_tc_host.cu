@@ -1,12 +1,12 @@
-// Host side of the tensor-core build path (sm_100a: TMA + tcgen05 + TMEM): support check, launch plan, tensor maps, dispatch to
-// the kernel generations.
+// Host side of the tensor-core build path (sm_90a: TMA + mbarrier pipelines + warp-level tf32 MMA): support check, launch plan,
+// tensor map, dispatch.
 //
 // Maths and partial-slot contract are those of lm_build.cu (reference bundlenet.py:206-263 + utils.cu:219-417); the basis contraction
-// runs on the 5th-gen tensor cores:
+// runs on the tensor cores:
 //
-//     D[128 x 160] += Bt^T R          per 64-pixel tile, kind::tf32, fp32 accumulate in TMEM
-//        Bt [64 px x 128]  the basis tile exactly as it lies in HBM (TMA, 128B/32B-atom swizzle) = MN-major "A"
-//        R  [64 px x 160]  row n = [ s_n * b_n (128) | v_n (6) | t_n | 0 ... ]  built by the algebra warps = MN-major "B"
+//     D[128 x 136] += Bt^T R          per 64-pixel tile, tf32 mma.sync, fp32 accumulate in registers
+//        Bt [64 px x 128]  the basis tile exactly as it lies in HBM (TMA, 128B/32B-atom swizzle)
+//        R  [64 px x 160]  row n = [ s_n * b_n (128) | v_n (6) | t_n | 0 ... ]  built by the algebra warps, same layout
 //     => D[i][j<128] = H_dd[i][j],  D[i][128+r] = H_cd[r][i] (r<6),  D[i][134] = g_d[i]
 //
 // Precision modes (tf32 keeps 10 mantissa bits; products are exact, accumulation is fp32):
@@ -20,8 +20,8 @@
 // Kernel generations:
 //   7 (lm_build_tc7.cu)  F2-only conv2 + dense grid: the tile's F2 footprint is staged into shared memory by TMA (channel chunks),
 //                        the 12 gradient/bilinear taps of every pixel come from LDS; per-tile fallback to global taps when the
-//                        footprint of a tile does not fit the staged window.  MODE 1 (where it is the default) and 2.
-//   6 (lm_build_tc6.cu)  everything else (the reference's [F2|gx|gy] layout, unstructured point lists, MODE 3): taps by ld.global.
+//                        footprint of a tile does not fit the staged window.  MODE 1 and 2.
+//   6 (lm_build_tc6.cu)  everything (both conv2 layouts, dense grids and point lists, every mode): taps by ld.global.
 #include "common.cuh"
 #include "lm_build.h"
 #include "tc_utils.cuh"
@@ -41,6 +41,17 @@ static banet_tuning_t g_tuning = {0, 0, 4, 0, 0, 0};
 void set_tuning(const banet_tuning_t& t) { g_tuning = t; }
 const banet_tuning_t& tuning() { return g_tuning; }
 
+// Generation 7 applies to the F2-only layout on a dense grid (tap coordinates are packed in 16 bits), modes 1 and 2.  The default
+// (tc_generation = 0) is generation 6 everywhere: in interleaved A/B runs on an H100 80GB HBM3 (400 W power limit, 32 pairs, F2-only
+// layout) generation 7 took 25.5 vs 21.5 ms at 640x480 and 5.8 vs 5.4 ms at 320x240 in TF32X1, and 2.3x as long in TF32X2 (its
+// gather warps run on 64 registers and spill, see DESIGN.md §4).  banet_set_tuning(tc_generation = 7) forces it where it applies.
+static bool use_gen7(const banet_level_t* lv, int mode, int kblk)
+{
+    const bool wanted = g_tuning.tc_generation == 7;
+    return wanted && lv->conv2_channels == lv->C && lv->grid_w > 0 && lv->h < 65536 && lv->w < 65536 &&
+           lm_build_tc7_supported(mode, lv->C / 64, kblk);
+}
+
 bool tc_supported(const banet_level_t* lv)
 {
     const bool k_ok = lv->K == 128 || lv->K == 64 || lv->K == 32;
@@ -48,17 +59,6 @@ bool tc_supported(const banet_level_t* lv)
            ((reinterpret_cast<uintptr_t>(lv->conv1) | reinterpret_cast<uintptr_t>(lv->conv2) | reinterpret_cast<uintptr_t>(lv->B)) % 16 == 0) &&
            (long long)lv->nb * lv->N < (1LL << 31) && (long long)lv->nb * ((lv->N + 63) / 64 + 80) < (1LL << 31) &&
            (long long)lv->h * lv->w * lv->conv2_channels < (1LL << 31);
-}
-
-// Generation 7 applies to the F2-only layout on a dense grid (tap coordinates are packed in 16 bits).  Default choice (tc_generation = 0),
-// from interleaved A/B runs at the board's steady power state (profiles/r02d_gen6_vs_gen7_f2layout.txt): in the single-pass mode (TF32X1)
-// generation 7 is 9 % (640x480) to 15 % (320x240) faster than generation 6 on this layout; in the two- and three-pass modes its gather
-// warps also carry the operand splitting and generation 6 is faster.  banet_set_tuning forces either (6 / 7).
-static bool use_gen7(const banet_level_t* lv, int mode, int kblk)
-{
-    const bool wanted = g_tuning.tc_generation == 7 || (g_tuning.tc_generation == 0 && mode == 1);
-    return wanted && lv->conv2_channels == lv->C && lv->grid_w > 0 && lv->h < 65536 && lv->w < 65536 &&
-           lm_build_tc7_supported(mode, lv->C / 64, kblk);
 }
 
 int build_plan_tc(const banet_level_t* lv, int num_sms, BuildPlan* plan)
@@ -88,8 +88,8 @@ int lm_build_tc(const banet_level_t* lv, const BuildPlan& plan, int mode, const 
     if (kblk != 4 && mode == 1) mode = 2;          // K = 64 / 32: the single-pass mode is not instantiated
     CUtensorMap tm;
     int rc;
-    if (lv->grid_w > 0) rc = make_tmap_f32_3d_sw128_32b(&tm, lv->B, (uint64_t)lv->nb * lv->grid_h, lv->grid_w, lv->K, 8, 8, 32);
-    else rc = make_tmap_f32_2d_sw128_32b(&tm, lv->B, (uint64_t)lv->nb * lv->N, lv->K, TC_TILE, 32);
+    if (lv->grid_w > 0) rc = make_tmap_f32_3d_sw128(&tm, lv->B, (uint64_t)lv->nb * lv->grid_h, lv->grid_w, lv->K, 8, 8, 32);
+    else rc = make_tmap_f32_2d_sw128(&tm, lv->B, (uint64_t)lv->nb * lv->N, lv->K, TC_TILE, 32);
     if (rc) return rc;
     const bool fly = lv->conv2_channels == lv->C;
     BuildParams prm;
@@ -103,9 +103,9 @@ int lm_build_tc(const banet_level_t* lv, const BuildPlan& plan, int mode, const 
     prm.tiles_x = lv->grid_w > 0 ? (lv->grid_w + 7) / 8 : 0; prm.tiles_y = lv->grid_h > 0 ? (lv->grid_h + 7) / 8 : 0;
     prm.band_rows = 1; prm.l2_hints = 0; prm.tap_prefetch = 0; prm.kq_i = 0; prm.kq_j = 0;
     prm.hdd_transposed = 1;
-    prm.force_direct = g_tuning.tc7_force_direct;
     prm.trace = nullptr;
     const int nch = lv->C / 64;
+    prm.force_direct = g_tuning.tc7_force_direct;
     if (use_gen7(lv, mode, kblk)) {
         int band = g_tuning.tc7_band_rows; if (band < 1) band = 1; if (band > prm.tiles_y) band = prm.tiles_y;
         prm.band_rows = band;
@@ -118,7 +118,7 @@ int lm_build_tc(const banet_level_t* lv, const BuildPlan& plan, int mode, const 
         if (rc) return rc;
         rc = lm_build_tc7_launch(mode, nch, kblk, tm, tmF, tmC, prm, plan.grid, st);
     } else {
-        // dense grid: band walk + L2 policy (defaults picked from the B200 measurements in profiles/r02c_*)
+        // dense grid: band walk + L2 policy (diagnostic knobs, off by default)
         int band = g_tuning.tc6_band_rows > 0 ? g_tuning.tc6_band_rows : kTc6DefaultBandRows;
         if (band > prm.tiles_y) band = prm.tiles_y;
         prm.band_rows = lv->grid_w > 0 && band > 1 ? band : 1;

@@ -1,5 +1,5 @@
-// sm_100a primitives used by the tensor-core build path: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (TMEM alloc / mma / commit / ld), shared-memory matrix descriptors and the 128B swizzle.
+// sm_90a primitives used by the tensor-core build path: mbarrier, TMA (cp.async.bulk.tensor), the 128B swizzle and
+// warp-level tf32 MMAs that read their fragments from the swizzled tiles.
 // Inline PTX only; no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
@@ -50,7 +50,7 @@ __device__ __forceinline__ bool mbar_wait_bounded(uint64_t* bar, uint32_t parity
 template <int NREG> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(NREG)); }
 template <int NREG> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(NREG)); }
 
-// generic-proxy writes (st.shared) -> visible to the async proxy (TMA / tcgen05.mma operand reads)
+// generic-proxy writes (st.shared) -> visible to the async proxy (TMA)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------------------------------------------------------- TMA
@@ -86,12 +86,6 @@ __device__ __forceinline__ float4 ld_stream_f4_hint(const float* p, uint64_t pol
                  : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p), "l"(pol));
     return r;
 }
-__device__ __forceinline__ float ld_f32_hint(const float* p, uint64_t pol) {
-    float r; asm volatile("ld.global.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(r) : "l"(p), "l"(pol) : "memory"); return r;
-}
-__device__ __forceinline__ void st_f32_hint(float* p, float v, uint64_t pol) {
-    asm volatile("st.global.L2::cache_hint.f32 [%0], %1, %2;" :: "l"(p), "f"(v), "l"(pol) : "memory");
-}
 __device__ __forceinline__ float4 ldg4_hint(const float* p, uint64_t pol) {
     float4 r;
     asm("ld.global.nc.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%4], %5;" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p), "l"(pol));
@@ -113,77 +107,49 @@ __device__ __forceinline__ void prefetch_l2_tensor_4d(const CUtensorMap* m, int 
                  :: "l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-template <int COLS> __device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {      // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(dst_smem)), "n"(COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- warp-level tf32 MMA on the swizzled tiles
+// Both operands of the contraction D[i][n] = sum_px A[px][i] * R[px][n] lie pixel-major in shared memory (A as TMA lands the basis
+// tile from HBM): they are MN-major.  Hopper's wgmma takes tf32 operands K-major only, so the fragments are read from the swizzled
+// tiles by LDS and fed to mma.sync m16n8k8 (fp32 accumulate in registers).  Every fragment is truncated to tf32 explicitly (low 13
+// bits cleared): the operand splitting of the precision modes (A_lo = b - trunc(b), R = rna(s*b) by +0x1000) relies on it.
+__device__ __forceinline__ void mma_tf32_m16n8k8(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-template <int COLS> __device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {        // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(taddr), "n"(COLS) : "memory");
+__device__ __forceinline__ uint32_t lds_tf32(uint32_t saddr) {
+    uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(saddr)); return v & 0xFFFFE000u;
 }
-__device__ __forceinline__ void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after_sync()  { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::tf32, issued by ONE thread.
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                 :: "r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+// Byte offset, inside a tile of [64 px] x [32-column blocks of 128 B] (block stride 8192 B, 128B swizzle), of column `col` in
+// pixel row 8*kk + r (r in 0..7; add kk * 1024).
+__device__ __forceinline__ uint32_t frag_off(int col, int r) {
+    return (uint32_t)((col >> 5) * 8192 + r * 128 + ((((col & 31) >> 2) ^ r) << 4) + (col & 3) * 4);
 }
-// arrive on `bar` once every previously issued tcgen05.mma of this thread has completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(smem_u32(bar)) : "memory");
+// A fragment (rows i0 .. i0+15 of A^T, pixels 8*kk .. 8*kk+7) from the tile at shared address `a`
+__device__ __forceinline__ void load_a_frag(uint32_t (&f)[4], uint32_t a, int i0, int kk, int lane) {
+    const int g = lane >> 2, t = lane & 3;
+    a += kk * 1024;
+    f[0] = lds_tf32(a + frag_off(i0 + g, t));     f[1] = lds_tf32(a + frag_off(i0 + g + 8, t));
+    f[2] = lds_tf32(a + frag_off(i0 + g, t + 4)); f[3] = lds_tf32(a + frag_off(i0 + g + 8, t + 4));
 }
-// 32 lanes x 32 columns of 32-bit: thread i of the warp gets TMEM lane (lane_base + i), columns col..col+31
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float* out) {
-    uint32_t r[32];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                   "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                   "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) out[i] = __uint_as_float(r[i]);
+// d += A^T[i0 .. i0+15][8 px] x R[8 px][n0 .. n0+7]
+__device__ __forceinline__ void mma_step(float (&d)[4], const uint32_t (&af)[4], uint32_t r, int n0, int kk, int lane) {
+    const int n = n0 + (lane >> 2), t = lane & 3;
+    r += kk * 1024;
+    mma_tf32_m16n8k8(d, af, lds_tf32(r + frag_off(n, t)), lds_tf32(r + frag_off(n, t + 4)));
 }
-
-// 32 lanes x 16 columns
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float* out) {
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr) : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) out[i] = __uint_as_float(r[i]);
+// The same step for long sums: the tensor core forms the 8-pixel product from zero and it is added to d in round-to-nearest fp32.
+// The tensor core's own fp32 accumulation truncates (biased toward zero, see tests/test_gpu_tensorcore.py), which over the
+// thousands of steps of a pair span would bias H_dd.
+__device__ __forceinline__ void mma_step_rn(float (&d)[4], const uint32_t (&af)[4], uint32_t r, int n0, int kk, int lane) {
+    float p[4] = {0.f, 0.f, 0.f, 0.f};
+    mma_step(p, af, r, n0, kk, lane);
+    d[0] += p[0]; d[1] += p[1]; d[2] += p[2]; d[3] += p[3];
 }
 
-// ---------------------------------------------------------------- descriptors
-// Shared-memory matrix descriptor for an MN-major 32-bit (tf32) operand.  The only canonical layout the
-// tensor core accepts for MN-major tf32 is SWIZZLE_128B with 32-byte atomicity (LayoutType 1,
-// "128B_BASE32B"; TMA: CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B):
-//   Swizzle<2,5,2> o ((T,8,m),(4,k)) : ((1,T,LBO),(8T,SBO))   (T = 4 fp32)
-// i.e. atoms of 4 k-rows x 128 B (32 MN-elements), row pitch 128 B, 32-byte chunk index ^= (row & 3);
-// next 32 MN-elements at +LBO bytes, next 4 k-rows at +SBO bytes.  Atom bases 512-B aligned.
-__device__ __forceinline__ uint64_t make_desc_mn_sw128_32b(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFFu);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;                      // descriptor version 1 (sm_100)
-    d |= (uint64_t)1 << 61;                      // LayoutType::SWIZZLE_128B_BASE32B
-    return d;
-}
-// Instruction descriptor: kind::tf32, fp32 accumulate, A and B both MN-major, M x N.
-__host__ __device__ constexpr uint32_t make_idesc_tf32_mn_mn(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// Byte offset of (row r, 16-byte chunk c in 0..7) inside one [rows][128 B] block in the 128B / 32B-atom swizzle
-// (block base 512-B aligned): the 32-byte chunk index (c >> 1) is XORed with (r & 3).
-__device__ __forceinline__ uint32_t sw128_32b_off(int r, int c) { return (uint32_t)(r * 128 + ((((c >> 1) ^ (r & 3)) << 5) | ((c & 1) << 4))); }
+// Byte offset of (row r, 16-byte chunk c in 0..7) inside one [rows][128 B] block in the 128B swizzle as TMA writes it
+// (CU_TENSOR_MAP_SWIZZLE_128B, block base 1024-B aligned): the chunk index is XORed with (r & 7).
+__device__ __forceinline__ uint32_t sw128_off(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
 
 __device__ __forceinline__ float tf32_rna(float x) {          // round to nearest tf32 (10-bit mantissa), ties away
     uint32_t u;

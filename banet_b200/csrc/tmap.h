@@ -24,9 +24,9 @@ inline PFN_encodeTiled get_encode_tiled()
     return fn;
 }
 
-// fp32 matrix [rows, cols] row-major (cols contiguous); box = box_cols x box_rows, 128B swizzle with 32-byte atoms
-// (the layout tcgen05 kind::tf32 needs for MN-major operands); box_cols*4 must be 128.
-inline int make_tmap_f32_2d_sw128_32b(CUtensorMap* out, const float* base, uint64_t rows, uint64_t cols, uint32_t box_rows, uint32_t box_cols)
+// fp32 matrix [rows, cols] row-major (cols contiguous); box = box_cols x box_rows, 128B swizzle (16-byte chunk index XOR row & 7,
+// tc_utils.cuh: sw128_off); box_cols*4 must be 128.
+inline int make_tmap_f32_2d_sw128(CUtensorMap* out, const float* base, uint64_t rows, uint64_t cols, uint32_t box_rows, uint32_t box_cols)
 {
     PFN_encodeTiled enc = get_encode_tiled();
     BANET_REQUIRE(enc, BANET_ERR_CUDA, "cuTensorMapEncodeTiled driver entry point not available");
@@ -35,7 +35,7 @@ inline int make_tmap_f32_2d_sw128_32b(CUtensorMap* out, const float* base, uint6
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     BANET_REQUIRE(r == CUDA_SUCCESS, BANET_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) rows=%llu cols=%llu", (int)r,
                   (unsigned long long)rows, (unsigned long long)cols);
@@ -44,7 +44,7 @@ inline int make_tmap_f32_2d_sw128_32b(CUtensorMap* out, const float* base, uint6
 
 // fp32 tensor [planes, rows, cols] (cols contiguous, dense): box = box_cols x box_rows x box_planes, same swizzle.
 // Used for the basis of a dense pixel grid: cols = K, rows = grid_w (x), planes = nb*grid_h (y); an 8x8 pixel tile is one box.
-inline int make_tmap_f32_3d_sw128_32b(CUtensorMap* out, const float* base, uint64_t planes, uint64_t rows, uint64_t cols,
+inline int make_tmap_f32_3d_sw128(CUtensorMap* out, const float* base, uint64_t planes, uint64_t rows, uint64_t cols,
                                       uint32_t box_planes, uint32_t box_rows, uint32_t box_cols)
 {
     PFN_encodeTiled enc = get_encode_tiled();
@@ -54,7 +54,7 @@ inline int make_tmap_f32_3d_sw128_32b(CUtensorMap* out, const float* base, uint6
     cuuint32_t box[3] = {box_cols, box_rows, box_planes};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     BANET_REQUIRE(r == CUDA_SUCCESS, BANET_ERR_CUDA, "cuTensorMapEncodeTiled(3d) failed (%d)", (int)r);
     return BANET_OK;

@@ -1,5 +1,5 @@
 """Thin torch-facing wrappers over the C-ABI (include/banet_abi.h).  torch is plumbing only: it owns
-device memory and streams; all arithmetic happens in libbanet_sm100.so.  No fallbacks: CPU tensors or a
+device memory and streams; all arithmetic happens in libbanet.so.  No fallbacks: CPU tensors or a
 missing library raise.
 """
 from __future__ import annotations

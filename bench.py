@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — LM iterations/sec of the BA layer's inner loop (BASELINE.json metric) on N B200s.
+"""bench.py — LM iterations/sec of the BA layer's inner loop (BASELINE.json metric) on N H100s.
 
 A "step" is one whole coarse-to-fine solve of BASELINE config 2 on every rank's shard:
 nb=32 frame-pairs per GPU, dense levels 80x60 -> 640x480 (ΣN = 408 000 points/pair), C=128 feature
@@ -37,8 +37,8 @@ LEVEL_IDS = (0, 1, 2, 3)
 H_FULL, W_FULL = 480, 640
 
 
-DTYPE_NAME = {"auto": "tf32 level-wise (tcgen05 kind::tf32 x3 below 65536 points/pair, x1 above; f32 accumulate; everything else f32)",
-              "levelwise": "tf32 level-wise (tcgen05 kind::tf32 x3 below 65536 points/pair, x1 above; f32 accumulate; everything else f32)",
+DTYPE_NAME = {"auto": "tf32 level-wise (mma.sync tf32 x3 below 65536 points/pair, x1 above; f32 accumulate; everything else f32)",
+              "levelwise": "tf32 level-wise (mma.sync tf32 x3 below 65536 points/pair, x1 above; f32 accumulate; everything else f32)",
               "fp32": "f32", "tf32x1": "tf32x1 (f32 accumulate)", "tf32x2": "tf32x2 split-A (f32 accumulate)", "tf32x3": "tf32x3 split-A/R (f32-grade)"}
 
 
@@ -70,7 +70,9 @@ def parse():
                          "pyramid, half-resolution basis / depth and intrinsics in; conv1, conv2, p, D, B derived on the device (ResizeHostSolver); "
                          "'features' = per-level tensors with F2 only ([F2|gx|gy] derived on the device); 'concat' = per-level tensors incl. the 3C tensor")
     ap.add_argument("--precision", default="auto", choices=["auto", "fp32", "tf32x1", "tf32x2", "tf32x3", "levelwise"],
-                    help="contraction path of the build kernel: auto = tensor cores (tcgen05 tf32 split-A) when K=128, else fp32 SIMT")
+                    help="contraction path of the build kernel: auto = tensor cores (tf32 split-A) when K=128, else fp32 SIMT")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the solve's outputs of the last step (R, T, W) to DIR/<name>.npy in float32")
     return ap.parse_args()
 
 
@@ -85,7 +87,19 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "fallback (H100 SXM data sheet)"
+
+
+def gpu_identity(index=0):
+    """Card name and power limit: a time or a rate means little without them."""
+    out = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                           capture_output=True, text=True, timeout=30)
+        out["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        pass
+    return out
 
 
 class ClockSampler:
@@ -286,7 +300,7 @@ def run_cfg4(args):
 
 def run_cfg5(args):
     """BASELINE configs[4]: depth-basis sweep K in {32,64,128,256} at 640x480 (one level), nb=64, 5 LM iterations: H_dd on tensor cores
-    (tcgen05 kind::tf32, AUTO policy) vs the fp32 SIMT register-tiled path."""
+    (tf32 tensor cores, AUTO policy) vs the fp32 SIMT register-tiled path."""
     from banet_b200 import ops, synth, _lib
     _lib.require_device()
     dev = torch.device("cuda", 0)
@@ -324,6 +338,8 @@ def run_cfg5(args):
 
 def main():
     args = parse()
+    if args.dump_outputs and (args.impl == "reference" or args.config != "cfg2"):
+        sys.exit("bench.py: --dump-outputs writes the outputs of the cfg2 solve; it is not available with --impl reference or --config cfg4|cfg5")
     if args.impl == "reference":
         run_reference(args)
         return
@@ -414,6 +430,11 @@ def main():
     barrier()
     ms = ev0.elapsed_time(ev1)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in zip(("R", "T", "W"), out):
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.detach().float().cpu().numpy())
     if world > 1:
         tms = torch.tensor([ms], device=dev, dtype=torch.float64)
         td.all_reduce(tms, op=td.ReduceOp.MAX)
@@ -481,9 +502,9 @@ def main():
                            "nvalid_fraction_finest_level": nvalid_frac, "planted_motion": "4 deg / 8 cm" if args.motion == "large" else "1 deg / 2 cm",
                            "conv2_layout": "[F2|gx|gy] (3C channels, the reference's BundleIteration boundary)" if args.layout == "concat"
                                            else "F2 only (C channels); the kernel recomputes gx, gy on the fly (reference grad_fixed, bundlenet.py:92-100)",
-                           "l2": "inputs (~33 GB/GPU) far exceed the 126 MB L2; no flush needed",
+                           "l2": "inputs (~33 GB/GPU) far exceed the 50 MB L2; no flush needed",
                            "parallelism": f"pairs sharded over {world} GPU(s), one all-gather of (R,T,W) per step"},
-                "clocks": clocks, "e2e": e2e, "gpu_launches": args.steps * (1 + total_iters * 3), "precision_check": precision_check,
+                "gpu": gpu_identity(local), "clocks": clocks, "e2e": e2e, "gpu_launches": args.steps * (1 + total_iters * 3), "precision_check": precision_check,
                 "roofline": roofline, "cpu_baseline": cpu_baseline}
         print(json.dumps(line))
     if world > 1:

@@ -1,5 +1,5 @@
 /*
- * banet_abi.h — C-ABI of libbanet_sm100.so: the B200 (sm_100a) drop-in for the BA layer's inner
+ * banet_abi.h — C-ABI of libbanet.so: the H100 (sm_90a) drop-in for the BA layer's inner
  * Levenberg–Marquardt loop of frobelbest/BANet.  Plain pointers and sizes only; no torch / TF types.
  *
  * Conventions
@@ -37,14 +37,14 @@ typedef void* banet_stream_t;            /* cudaStream_t */
 
 int         banet_abi_version(void);
 const char* banet_last_error(void);
-/* 0 if the current CUDA device can run this library (compute capability 10.x), else an error. */
+/* 0 if the current CUDA device can run this library (compute capability 9.0), else an error. */
 int         banet_device_check(void);
 int         banet_num_sms(void);
 
 /* Diagnostic / test knobs (process-wide; defaults = production).  Results never depend on them beyond
  * fp32 summation order. */
 typedef struct banet_tuning {
-    int tc_generation;      /* 0: default (generation 7 = TMA-staged F2 windows for F2-only layout + dense grid + single-pass TF32X1, generation 6 = ld.global taps otherwise); 6 / 7: force one wherever it applies */
+    int tc_generation;      /* 0: default (generation 6 everywhere; lm_build_tc_host.cu has the measurement); 6 / 7: force one wherever it applies (7: F2-only layout + dense grid, TF32X1 / X2) */
     int tc7_force_direct;   /* 1: generation 7 takes its per-tile global-tap fallback for every tile (tests the fallback) */
     int tc7_band_rows;      /* generation 7 walks the 8x8 tiles of a pair in bands of this many tile rows (L2 reuse of the window halos); default 4 */
     int tc6_band_rows;      /* generation 6, dense grid: same walk (tap rows shared by vertically adjacent tiles are re-read from L2, not HBM); 0 = default, 1 = row-major */

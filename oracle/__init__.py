@@ -18,7 +18,7 @@ installed here — but the reference's own code does run, two ways, and the orac
      Third-party restatement is confined to the shim (resampler, LU / QR solves, selu, l2_normalize, REFLECT pad) and listed there.
   2. its CUDA: `oracle/Makefile` compiles /root/reference/utils.cu UNMODIFIED (EquationConstruction + EquationConstructionGrad: real
      cuBLAS batched GEMMs + the reference's own reduction / tiling kernels) against stand-in TensorFlow headers (oracle/tf_stub) into
-     oracle/_ref/libbanet_ref_eqc.so.  On the GPU, tests/test_gpu_reference_pin.py compares the B200 kernels AND the oracle with it;
+     oracle/_ref/libbanet_ref_eqc.so.  On the GPU, tests/test_gpu_reference_pin.py compares the kernels AND the oracle with it (through stored outputs, tests/golden/ref_eqc_pin.npz);
      tests/golden/ref_eqc.npz (written by that compiled kernel on a B200) pins the oracle and the cuBLAS-chain replay
      (oracle/gemm_chain.py) on the CPU (tests/test_oracle_pinned_eqc.py).
 Further self-consistency checks (tests/test_oracle_consistency.py): materialised reference form == structured block form == chunked

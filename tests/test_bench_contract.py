@@ -1,4 +1,4 @@
-"""The bench line contract (task statement, section 4) checked on the committed round-2 measurement, plus bench.py's CLI."""
+"""The bench line contract checked on the committed H100 measurement (profiles/h100_bench_1gpu.json), plus bench.py's CLI."""
 import json
 import os
 import subprocess
@@ -8,7 +8,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_committed_bench_line_has_every_contract_key():
-    d = json.load(open(os.path.join(ROOT, "profiles", "r02_bench_1gpu.json")))
+    d = json.load(open(os.path.join(ROOT, "profiles", "h100_bench_1gpu.json")))
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline", "dtype",
               "data", "config", "clocks", "e2e", "gpu_launches", "roofline", "cpu_baseline"):
         assert k in d, k

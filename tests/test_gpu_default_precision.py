@@ -1,10 +1,8 @@
 """GPU: the SHIPPED default precision policy, whole solves, against the float64 oracle at the north-star tolerance.
 
-cfg2-shaped case, sized so that the float64 oracle finishes in about a minute of host time on the GPU box (the full-resolution nb = 2 run of
-BASELINE.json configs[1] -- 4 levels up to 640x480, 400 s of oracle time -- is recorded in profiles/r02a_precision_vs_oracle_cfg2shape.txt):
+cfg2-shaped case, sized so that the float64 oracle finishes in about a minute of host time:
 nb = 1, 4 dense levels 40x30 .. 320x240 (the finest level is above the 65536-point threshold of the level-wise policy, so both TF32X3 and TF32X1 run),
-C = K = 128, lambda-MLP in the loop, 5 LM iterations per level; both conv2 layouts (the reference's [F2|gx|gy] -> generation-6 kernel,
-F2-only -> generation 7).  Asserted at 1e-4 rel-fro on R, T, W and the depth output D + B.W (bundlenet.py:397) for AUTO (what
+C = K = 128, lambda-MLP in the loop, 5 LM iterations per level; both conv2 layouts (the reference's [F2|gx|gy] and F2-only).  Asserted at 1e-4 rel-fro on R, T, W and the depth output D + B.W (bundlenet.py:397) for AUTO (what
 bench.py times) and for the fp32-grade modes; the other modes are printed."""
 import pytest
 import torch

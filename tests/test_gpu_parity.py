@@ -1,4 +1,4 @@
-"""GPU parity tests (run with `-m gpu` on a B200): every C-ABI entry point against the CPU oracle on the
+"""GPU parity tests (run with `-m gpu` on an H100): every C-ABI entry point against the CPU oracle on the
 same seeded inputs, and against the committed golden fixtures.  All arithmetic on the path is fp32;
 tolerances are relative Frobenius errors against the float64 oracle, written beside each assert.
 The headline bar (BASELINE.json north_star) is 1e-4 rel-fro on pose/depth outputs."""

@@ -52,7 +52,7 @@ def test_tc7_matches_oracle(prec, C):
 
 @pytest.mark.parametrize("band", [1, 3, 4, 30])
 def test_tc7_band_order_and_generation6_agree(band):
-    """240x320, 2 pairs = 2400 tiles over 148 CTAs (ring wrap, several TMEM chains, two pair spans per CTA): every band order gives
+    """240x320, 2 pairs = 2400 tiles over 132 CTAs (ring wrap, two pair spans per CTA): every band order gives
     the generation-6 result up to fp32 summation order, run-to-run bit reproducible."""
     from banet_b200 import ops, _lib
     sc = _scene(2, 240, 320, 128, seed=17)
@@ -93,7 +93,7 @@ def test_tc7_large_motion_fallback(force):
 
 def test_tc7_whole_solve_under_the_default_policy():
     """A 2-level solve through banet_lm_run under the AUTO (level-wise) policy: 120x160 -> TF32X3 (generation 6), 240x320 -> TF32X1 on the
-    generation-7 kernel; against the FP32 SIMT path (held to the oracle in test_gpu_parity.py) at the north-star tolerance."""
+    generation-6 or (forced) generation-7 kernel; against the FP32 SIMT path (held to the oracle in test_gpu_parity.py) at the north-star tolerance."""
     from banet_b200 import ops, _lib, synth
     sc = synth.make_scene(nb=2, H=240, W=320, C=128, K=128, level_ids=(2, 3), seed=31, device="cuda", dtype=torch.float32)
     levels = [_f2_level(ops, l) for l in sc.levels]

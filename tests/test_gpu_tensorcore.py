@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 / TMA building blocks (SWIZZLE_128B MN-major operands, kind::tf32) against fp64 matmul."""
+"""GPU tests of the TMA / tf32-MMA building blocks (SWIZZLE_128B pixel-major tiles, mma.sync tf32 fragments read from them) against fp64 matmul."""
 import pytest
 import torch
 
@@ -50,9 +50,9 @@ def test_tcgen05_precision_modes(mode, use_rna, tol):
 
 
 def test_tcgen05_accumulator_rounding():
-    """Accumulate the same (tf32-exact, positive) tile T times: the exact answer is T * D1.  Documents how the TMEM fp32
-    accumulator rounds (printed).  Measured on B200: every accumulation step TRUNCATES (mean -5e-8 relative per step),
-    which is why lm_build_tc keeps TMEM chains short and adds them up round-to-nearest outside the tensor core."""
+    """Accumulate the same (tf32-exact, positive) tile T times through the MMA's own fp32 accumulator: the exact answer is
+    T * D1.  Documents how the tensor core's accumulator rounds (printed): every accumulation step TRUNCATES, which is why the
+    build kernel forms each 8-pixel step from zero and adds it round-to-nearest outside the tensor core (tc_utils.cuh: mma_step_rn)."""
     g = torch.Generator().manual_seed(3)
     A = _tf32_exact(torch.rand(64, 128, generator=g) + 0.5).cuda(); R = _tf32_exact(torch.rand(64, 160, generator=g) + 0.5).cuda()
     ref1 = A.double().t() @ R.double()
@@ -137,8 +137,8 @@ def test_lm_run_tensorcore_vs_oracle_outputs():
 @pytest.mark.parametrize("fly,grid", [(False, True), (True, True), (False, False)])
 @pytest.mark.parametrize("prec", [1, 2, 3])
 def test_lm_build_tensorcore_long_tile_runs(prec, fly, grid):
-    """Many tiles per CTA (ring wrap of the TMA stages and record buffers, several TMEM chains and two pair spans per CTA):
-    240x320, 2 pairs = 2400 tiles over 148 CTAs.  Checked against the FP32 SIMT path (itself pinned to the oracle above),
+    """Many tiles per CTA (ring wrap of the TMA stages and record buffers, two pair spans per CTA):
+    240x320, 2 pairs = 2400 tiles over 132 CTAs.  Checked against the FP32 SIMT path (itself pinned to the oracle above),
     plus run-to-run bit reproducibility."""
     from banet_b200 import ops, synth
     sc = synth.make_scene(nb=2, H=240, W=320, C=128, K=128, level_ids=(3,), seed=17, device="cuda", dtype=torch.float32)
@@ -191,8 +191,7 @@ def test_cfg4_window_sparse_points_solve():
 def test_small_basis_counts_on_the_tensor_cores(K):
     """K = 64 / 32 (BASELINE.json configs[4], the K sweep): the generation-6 kernel with KBLK = K / 32 basis blocks against the float64
     oracle, with and without the dense-grid hint, in the two- and three-pass modes (the single-pass mode is instantiated for K = 128 only, so
-    AUTO resolves to TF32X2 here) and against the FP32 SIMT path.  First measured in round 2 (profiles/r02a_small_k_check.txt: relH 1.0e-7 /
-    2.6e-8 / 2.4e-8 for X2 / X3 / FP32)."""
+    AUTO resolves to TF32X2 here) and against the FP32 SIMT path."""
     from banet_b200 import ops, synth, _lib
     sc = synth.make_scene(nb=3, H=96, W=128, C=64, K=K, level_ids=(3,), seed=50 + K, device="cpu", dtype=torch.float32)
     lv = sc.levels[0]
