@@ -78,6 +78,12 @@ SIGNATURES = {
     "banet_lm_window_run": (C.c_int, [C.POINTER(BanetLevel), C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_float, C.c_float,
                                       C.POINTER(BanetSolveOpts), C.c_int] + [c_float_p] * 3 + [C.c_void_p]
                             + [C.c_void_p, C.c_size_t, c_stream]),
+    "banet_lm_window_solve_update_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "banet_lm_window_solve_update": (C.c_int, [c_float_p] * 3 + [C.c_int, C.c_int, C.POINTER(BanetSolveOpts)] + [c_float_p] * 3
+                                     + [c_float_p] * 4 + [C.c_void_p] + [C.c_void_p, C.c_size_t, c_stream]),
+    "banet_lm_window_solve_update_bwd_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "banet_lm_window_solve_update_bwd": (C.c_int, [c_float_p] * 4 + [C.c_int, C.c_int, C.POINTER(BanetSolveOpts)] + [c_float_p] * 5
+                                         + [c_float_p] * 6 + [C.c_void_p, C.c_size_t, c_stream]),
     "banet_depth_compose": (C.c_int, [c_float_p] * 3 + [C.c_int] * 3 + [c_float_p, c_stream]),
     "banet_lm_step": (C.c_int, [c_float_p] * 3 + [C.c_int] * 4 + [c_float_p, C.c_float, c_float_p, C.POINTER(BanetSolveOpts)] + [c_float_p] * 3
                       + [c_float_p] * 3 + [c_float_p, c_float_p, C.c_void_p, c_stream]),

@@ -6,6 +6,7 @@ Two training paths:
     (J, G, d, the tiled upstream gradients of utils.cu:613-617) is materialised, so it runs at any N and K <= 256.  The lambda-MLP
     (5 dense layers on a [nb,C] vector, bundlenet.py:244-248) stays stock torch in between.  Gradient signature = the reference's:
     conv1, conv2, D, B, R, T, W and the lambda-MLP parameters (TF autodiff + the registered op gradient, bundlenet.py:79-82).
+    `window_iteration_fused` is the same for the joint keyframe window (banet_lm_window_solve_update / _bwd after the per-pair build).
   * `iteration` (the reference's own split of labour, kept as the A/B baseline and for op-level drop-in use):
 
     reference:  TF graph ops (warp, resampler, Jacobians, damping, solve, update; TF autodiff)  +  native op
@@ -186,6 +187,29 @@ class _LMSolveUpdateFn(torch.autograd.Function):
         return dH, dg.reshape(g.shape), dlam.reshape(lam.shape), dR, dT, dW, None, None
 
 
+class _WindowSolveUpdateFn(torch.autograd.Function):
+    """(R' [nf,3,3], T' [nf,3,1], W' [K,1]) = banet_lm_window_solve_update(H, g, lambda [1], R, T, W); backward =
+    banet_lm_window_solve_update_bwd.  Saves H, g, lambda, the joint solution, R, T: nothing per-pixel."""
+
+    @staticmethod
+    def forward(ctx, H, g, lam, R, T, W, damping_eps):
+        Rn, Tn, Wn, delta, status = ops.lm_window_solve_update(H, g, lam, R, T, W, damping_eps=damping_eps)
+        ctx.save_for_backward(H, g, lam, delta, R, T)
+        ctx.eps = float(damping_eps)
+        ctx.mark_non_differentiable(status)
+        return Rn, Tn, Wn, status
+
+    @staticmethod
+    def backward(ctx, dRn, dTn, dWn, _dstatus):
+        H, g, lam, delta, R, T = ctx.saved_tensors
+        K = H.shape[1] - 6
+        dRn = dRn if dRn is not None else torch.zeros_like(R)
+        dTn = dTn if dTn is not None else torch.zeros_like(T)
+        dWn = dWn if dWn is not None else torch.zeros(K, 1, device=H.device)
+        dH, dg, dlam, dR, dT, dW = ops.lm_window_solve_update_bwd(H, g, lam, delta, R, T, dRn.contiguous(), dTn.contiguous(), dWn.contiguous(), ctx.eps)
+        return dH, dg.reshape(g.shape), dlam.reshape(lam.shape), dR, dT, dW, None
+
+
 class _GradFixedConcatFn(torch.autograd.Function):
     """[F | grad_fixed(F)] (+ the half swap of bundlenet.py:386), differentiable (banet_grad_fixed_concat / _bwd)."""
 
@@ -260,6 +284,34 @@ def iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regular
         Rn, Tn, Wn, status = out
     else:
         (Rn, Tn, status), Wn = out, None
+    if return_status:
+        return Rn, Tn, Wn, status
+    return Rn, Tn, Wn
+
+
+def window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base: Optional[float],
+                           damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None,
+                           precision: int = 0, grid=None, return_status: bool = False):
+    """One differentiable LM iteration of a keyframe window (the joint solve of ops.lm_window_run) on the fused kernels: nf pairs
+    (keyframe -> frame f) share W [K,1]; R [nf,3,3], T [nf,3,1] and conv2 [nf,h,w,3C] are per frame.  The keyframe tensors conv1, p, D, B
+    (and intr) may be given once ([1,...]): they are broadcast to the frames and their gradients summed over them.  lambda: from the mean
+    |residual| over all points of all frames through the MLP (times l2_regularizer_base), or lambda_override [1].
+    Returns (R', T', W' [K,1]) (, status [nf])."""
+    nf = R.shape[0]
+    K = B.shape[-1]
+    frames = lambda t: t.expand(nf, *t.shape[1:]).contiguous() if t.shape[0] == 1 and nf > 1 else t
+    conv1, intr, p, D, B = frames(conv1), frames(intr), frames(p), frames(D), frames(B)
+    N = conv1.shape[1]
+    Wf = W.reshape(1, K, 1).expand(nf, K, 1).contiguous()                       # every pair builds with the shared W; dW sums over them
+    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, Wf, intr.detach(), p.detach(), precision, exact_sym, grid)
+    if lambda_override is not None:
+        lam = lambda_override.reshape(1)
+    else:
+        avg = (rbar_sum.sum(0) / float(nf * N)).reshape(1, 1, -1)               # mean |residual| over all nf * N points
+        lam = torch.pow(torch.linalg.norm(avg, dim=-1, keepdim=True), 2.0 + lambda_mlp(avg, mlp_params)).reshape(1)
+        if l2_regularizer_base is not None:
+            lam = l2_regularizer_base * lam
+    Rn, Tn, Wn, status = _WindowSolveUpdateFn.apply(H, g, lam, R, T, W.reshape(K, 1), damping_eps)
     if return_status:
         return Rn, Tn, Wn, status
     return Rn, Tn, Wn

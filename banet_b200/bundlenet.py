@@ -146,6 +146,30 @@ class BundleNet(torch.nn.Module):
         Rn, Tn, Wn, _ = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, B, R, T, W, base, level)
         return Rn, Tn, Wn
 
+    def WindowIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, l2_regularizer_base=None, level=None):
+        """One joint LM iteration of a keyframe window (an extension; the reference's layer is 2-view): the nf pairs (keyframe -> frame f)
+        share the keyframe depth D + B.W.  Arguments as BundleIteration with R [nf,3,3], T [nf,3,1], conv2 [nf,h,w,3C] per frame and
+        W [K,1] shared; the keyframe tensors conv1, p, D, B may be given once ([1,...]) or per frame.  -> (updatedR, updatedT, updatedW [K,1]).
+        Differentiable (banet_lm_window_solve_update_bwd) whenever gradients are being recorded; there is no reference_split twin."""
+        base = 1.0 if l2_regularizer_base is None else float(l2_regularizer_base)
+        if self.vmatrix_batch_scramble:
+            raise RuntimeError("vmatrix_batch_scramble=True is a 2-view quirk (bundlenet.py:45); the window solve has per-frame VMatrix only")
+        nf = R.shape[0]
+        intr = _intr_from_tiled(fx, fy, ox, oy)
+        if self._wants_grad(conv1, conv2, D, B, R, T, W):
+            if self.training_path == "reference_split":
+                raise RuntimeError("training_path='reference_split' has no torch-graph twin of the window solve; use training_path='fused'")
+            Rn, Tn, Wn, status = _ag.window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base,
+                                                            exact_sym=self.exact_sym_grad, precision=self.precision, return_status=True)
+            self._check_status(status)
+            return Rn, Tn, Wn
+        frames = lambda t: t.expand(nf, *t.shape[1:]) if t.shape[0] == 1 else t
+        lv = ops.Level(frames(conv1), conv2, frames(intr), frames(p), frames(D), frames(B))
+        Rn, Tn, Wn, status = ops.lm_window_run([lv], 1, R, T, W, mlp_packed=[self.mlp_packed(str(level))], l2_regularizer_base=base,
+                                               precision=self.precision)
+        self._check_status(status)
+        return Rn, Tn, Wn
+
     # ---- level schedulers ----------------------------------------------------------------------
     def _prepare(self, intrisic: Tensor, points: Tensor):
         geo = self.geo

@@ -362,12 +362,57 @@ extern "C" int banet_lm_window_run(const banet_level_t* levels, int nlevels, int
             rc = build_dispatch(lv, res, plan, R, T, W, H, g, rbar, nvalid, base + c.build, st);
             if (rc) return rc;
             rc = lm_window_step(H, g, rbar, nf, lv->N, lv->C, K, use_mlp ? mlp_weights[l] : nullptr, l2_regularizer_base, use_mlp ? nullptr : lam,
-                                *opts, R, T, W, wsw, nullptr, status, st);
+                                *opts, R, T, W, nf, R, T, W, nullptr, wsw, nullptr, status, 1, st);
             if (rc) return rc;
         }
     }
     BANET_CUDA_LAUNCH_CHECK("lm_window_run");
     return BANET_OK;
+}
+
+extern "C" size_t banet_lm_window_solve_update_workspace_bytes(int nf, int K)
+{
+    if (nf <= 0 || K <= 0) return 0;
+    return align_up(lm_window_step_workspace_floats(nf, K, 0) * sizeof(float), 256);
+}
+
+extern "C" int banet_lm_window_solve_update(const float* H, const float* g, const float* lambda, int nf, int K, const banet_solve_opts_t* opts,
+                                            const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
+                                            float* delta, int32_t* status, void* ws, size_t ws_bytes, banet_stream_t stream)
+{
+    BANET_REQUIRE(H && g && lambda && opts && R && T && W && R_out && T_out && W_out && delta && status, BANET_ERR_BAD_ARG,
+                  "lm_window_solve_update: null pointer");
+    BANET_REQUIRE(nf > 0 && K > 0 && !opts->vmatrix_batch_scramble, BANET_ERR_BAD_ARG,
+                  "lm_window_solve_update: needs nf > 0, a depth basis (K > 0) and vmatrix_batch_scramble = 0 (nf=%d K=%d)", nf, K);
+    BANET_REQUIRE(lm_window_supported(nf, K, 1), BANET_ERR_UNSUPPORTED, "lm_window_solve_update: 6*%d+%d unknowns do not fit the solve kernel", nf, K);
+    const size_t need = banet_lm_window_solve_update_workspace_bytes(nf, K);
+    BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_window_solve_update: workspace %zu < %zu bytes", ws_bytes, need);
+    return lm_window_step(H, g, nullptr, nf, 1, 0, K, nullptr, 1.f, lambda, *opts, R, T, W, 1, R_out, T_out, W_out, delta,
+                          reinterpret_cast<float*>(ws), nullptr, status, 0, (cudaStream_t)stream);
+}
+
+extern "C" size_t banet_lm_window_solve_update_bwd_workspace_bytes(int nf, int K)
+{
+    if (nf <= 0 || K <= 0) return 0;
+    return align_up(lm_window_step_bwd_workspace_floats(nf, K) * sizeof(float), 256);
+}
+
+extern "C" int banet_lm_window_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nf, int K,
+                                                const banet_solve_opts_t* opts, const float* R, const float* T,
+                                                const float* dR_out, const float* dT_out, const float* dW_out,
+                                                float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW,
+                                                void* ws, size_t ws_bytes, banet_stream_t stream)
+{
+    BANET_REQUIRE(H && g && lambda && delta && opts && R && T && dR_out && dT_out && dW_out && dH && dg && dlambda && dR && dT && dW, BANET_ERR_BAD_ARG,
+                  "lm_window_solve_update_bwd: null pointer");
+    BANET_REQUIRE(nf > 0 && K > 0 && !opts->vmatrix_batch_scramble, BANET_ERR_BAD_ARG,
+                  "lm_window_solve_update_bwd: needs nf > 0, a depth basis (K > 0) and vmatrix_batch_scramble = 0 (nf=%d K=%d)", nf, K);
+    BANET_REQUIRE(lm_window_supported(nf, K, 1) && solve_bwd_supported(6 * nf + K), BANET_ERR_UNSUPPORTED,
+                  "lm_window_solve_update_bwd: 6*%d+%d unknowns do not fit the solve kernels", nf, K);
+    const size_t need = banet_lm_window_solve_update_bwd_workspace_bytes(nf, K);
+    BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_window_solve_update_bwd: workspace %zu < %zu bytes", ws_bytes, need);
+    return lm_window_step_bwd(H, g, lambda, delta, nf, K, *opts, R, T, dR_out, dT_out, dW_out, dH, dg, dlambda, dR, dT, dW,
+                              reinterpret_cast<float*>(ws), (cudaStream_t)stream);
 }
 
 extern "C" size_t banet_lm_track_legacy_workspace_bytes(const banet_level_t* levels, int nlevels)

@@ -71,8 +71,14 @@ bool lm_window_supported(int nf, int K, int C);
 size_t lm_window_step_workspace_floats(int nf, int K, int C);
 int lm_window_broadcast_w(float* W, int nf, int K, cudaStream_t st);
 int lm_window_step(const float* H, const float* g, const float* rbar_sum, int nf, int N, int C, int K, const float* mlp, float base,
-                   const float* lambda_in, const banet_solve_opts_t& opts, float* R, float* T, float* W, float* ws, float* lambda_out,
-                   int32_t* status, cudaStream_t st);
+                   const float* lambda_in, const banet_solve_opts_t& opts, const float* R, const float* T, const float* W, int w_rows,
+                   float* R_out, float* T_out, float* W_out, float* delta_j, float* ws, float* lambda_out, int32_t* status, int status_accumulate,
+                   cudaStream_t st);
+// its backward (lambda given); ws: lm_window_step_bwd_workspace_floats floats
+size_t lm_window_step_bwd_workspace_floats(int nf, int K);
+int lm_window_step_bwd(const float* H, const float* g, const float* lambda, const float* delta_j, int nf, int K, const banet_solve_opts_t& opts,
+                       const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
+                       float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, float* ws, cudaStream_t st);
 
 // legacy pose-only tracker loop with device-side accept / reject and early termination (lm_legacy.cu)
 size_t lm_track_legacy_workspace_bytes(const banet_level_t* levels, int nlevels);
@@ -85,5 +91,12 @@ int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const 
 int lm_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int K, const banet_solve_opts_t& opts,
                         const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
                         float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, cudaStream_t st);
+// its two stages: the SE(3) update backward (ddelta[0:6] of pair b -> ddelta + b * P), and u = Ht^-1 [ddelta[0:npose] | dW'] with dH, dg = u,
+// dlambda, dW = dW' (pairs of P unknowns, the first npose of them poses)
+int launch_pose_update_bwd(const float* delta, int nb, int P, const float* R, const float* T, const float* gRn, const float* gTn,
+                           float* ddelta, float* dR, float* dT, cudaStream_t st);
+bool solve_bwd_supported(int P);
+int launch_solve_bwd(const float* H, const float* lambda, const float* delta, int nb, int P, int npose, const banet_solve_opts_t& opts,
+                     const float* gWn, float* dH, float* dg, float* dlambda, float* dW, cudaStream_t st);
 
 }  // namespace banet

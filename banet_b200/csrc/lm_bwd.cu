@@ -385,10 +385,11 @@ __global__ void pose_update_bwd_kernel(const float* __restrict__ delta, int nb, 
 constexpr int SB_THREADS = 1024;
 __host__ __device__ __forceinline__ int tri2(int i, int k) { return i * (i + 1) / 2 + k; }
 
-// u = Ht^-1 ddelta with the same Cholesky as lm_solve_kernel; dg (in: ddelta[0:6] from pose_update_bwd_kernel, out: u)
+// u = Ht^-1 ddelta with the same Cholesky as lm_solve_kernel; dg (in: ddelta[0:npose] from pose_update_bwd_kernel, out: u).  npose = 6 for the
+// pairs of the 2-view iteration, 6 nf for the one system of a keyframe window; the remaining P - npose entries of ddelta are dW'.
 template <typename S>
 __global__ void __launch_bounds__(SB_THREADS)
-lm_solve_bwd_kernel(const float* __restrict__ H, const float* __restrict__ lambda, const float* __restrict__ delta, int P, float eps, int ndamped,
+lm_solve_bwd_kernel(const float* __restrict__ H, const float* __restrict__ lambda, const float* __restrict__ delta, int P, int npose, float eps, int ndamped,
                     const float* __restrict__ gWn, float* __restrict__ dH, float* __restrict__ dg, float* __restrict__ dlambda, float* __restrict__ dW)
 {
     extern __shared__ __align__(16) unsigned char smraw[];
@@ -397,11 +398,11 @@ lm_solve_bwd_kernel(const float* __restrict__ H, const float* __restrict__ lambd
     S* uu = r + P;                                      // ddelta -> u
     S* dgq = uu + P;                                    // sqrt of the pivots
     __shared__ int s_flag;
-    __shared__ double s_dl;
-    const int b = blockIdx.x, tid = threadIdx.x, K = P - 6;
+    __shared__ double s_dl[SB_THREADS / 32];            // per-warp partial sums of dlambda, added in a fixed order: bit-reproducible
+    const int b = blockIdx.x, tid = threadIdx.x, K = P - npose;
     const float* Hb = H + (size_t)b * P * P;
     const float lam = lambda[b];
-    if (tid == 0) { s_flag = 0; s_dl = 0.0; }
+    if (tid == 0) s_flag = 0;
     __syncthreads();
     int bad = 0;
     for (int i = tid / 32; i < P; i += SB_THREADS / 32)
@@ -414,8 +415,8 @@ lm_solve_bwd_kernel(const float* __restrict__ H, const float* __restrict__ lambd
         }
     for (int i = tid; i < P; i += SB_THREADS) {
         r[i] = (S)delta[(size_t)b * P + i];
-        if (i < 6) uu[i] = (S)dg[(size_t)b * P + i];
-        else { const float v = gWn[(size_t)b * K + i - 6]; uu[i] = (S)v; dW[(size_t)b * K + i - 6] = v; }       // W' = W + delta_d
+        if (i < npose) uu[i] = (S)dg[(size_t)b * P + i];
+        else { const float v = gWn[(size_t)b * K + i - npose]; uu[i] = (S)v; dW[(size_t)b * K + i - npose] = v; }       // W' = W + delta_d
     }
     if (!isfinite(lam)) bad = 1;
     if (bad) atomicOr(&s_flag, 2);
@@ -470,9 +471,47 @@ lm_solve_bwd_kernel(const float* __restrict__ H, const float* __restrict__ lambd
     for (int i = tid; i < P; i += SB_THREADS) dg[(size_t)b * P + i] = flag ? 0.f : (float)uu[i];
     part += __shfl_xor_sync(0xffffffffu, part, 16); part += __shfl_xor_sync(0xffffffffu, part, 8); part += __shfl_xor_sync(0xffffffffu, part, 4);
     part += __shfl_xor_sync(0xffffffffu, part, 2); part += __shfl_xor_sync(0xffffffffu, part, 1);
-    if ((tid & 31) == 0 && part != 0.0) atomicAdd(&s_dl, part);
+    if ((tid & 31) == 0) s_dl[tid >> 5] = part;
     __syncthreads();
-    if (tid == 0) dlambda[b] = flag ? 0.f : (float)s_dl;
+    if (tid == 0) {
+        double dl = 0.0;
+        for (int wq = 0; wq < SB_THREADS / 32; ++wq) dl += s_dl[wq];
+        dlambda[b] = flag ? 0.f : (float)dl;
+    }
+}
+
+int launch_pose_update_bwd(const float* delta, int nb, int P, const float* R, const float* T, const float* gRn, const float* gTn,
+                           float* ddelta, float* dR, float* dT, cudaStream_t st)
+{
+    pose_update_bwd_kernel<<<(nb + 63) / 64, 64, 0, st>>>(delta, nb, P, R, T, gRn, gTn, ddelta, dR, dT);
+    BANET_CUDA_LAUNCH_CHECK("pose_update_bwd_kernel launch");
+    return BANET_OK;
+}
+
+// packed lower triangle + 3 vectors in shared memory: double up to 200 KB (P <= 220), float beyond
+static size_t solve_bwd_floats(int P) { return (size_t)P * (P + 1) / 2 + 3 * (size_t)P; }
+static bool solve_bwd_double(int P) { return solve_bwd_floats(P) * sizeof(double) <= 200 * 1024; }
+bool solve_bwd_supported(int P) { return solve_bwd_double(P) || solve_bwd_floats(P) * sizeof(float) <= 220 * 1024; }
+
+int launch_solve_bwd(const float* H, const float* lambda, const float* delta, int nb, int P, int npose, const banet_solve_opts_t& opts,
+                     const float* gWn, float* dH, float* dg, float* dlambda, float* dW, cudaStream_t st)
+{
+    const int ndamped = opts.undamped_last ? P - 1 : P;
+    const bool use_double = solve_bwd_double(P);
+    const size_t smem = solve_bwd_floats(P) * (use_double ? sizeof(double) : sizeof(float));
+    BANET_REQUIRE(solve_bwd_supported(P), BANET_ERR_UNSUPPORTED, "lm_solve_bwd: P=%d does not fit shared memory", P);
+    cudaError_t e;
+    if (use_double) {
+        e = cudaFuncSetAttribute(lm_solve_bwd_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) { set_error("lm_solve_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
+        lm_solve_bwd_kernel<double><<<nb, SB_THREADS, smem, st>>>(H, lambda, delta, P, npose, opts.damping_eps, ndamped, gWn, dH, dg, dlambda, dW);
+    } else {
+        e = cudaFuncSetAttribute(lm_solve_bwd_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) { set_error("lm_solve_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
+        lm_solve_bwd_kernel<float><<<nb, SB_THREADS, smem, st>>>(H, lambda, delta, P, npose, opts.damping_eps, ndamped, gWn, dH, dg, dlambda, dW);
+    }
+    BANET_CUDA_LAUNCH_CHECK("lm_solve_bwd_kernel launch");
+    return BANET_OK;
 }
 
 int lm_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int K, const banet_solve_opts_t& opts,
@@ -483,25 +522,10 @@ int lm_solve_update_bwd(const float* H, const float* g, const float* lambda, con
     BANET_REQUIRE(!opts.vmatrix_batch_scramble, BANET_ERR_UNSUPPORTED,
                   "lm_solve_update_bwd: the batch-interleaved VMatrix of bundlenet.py:45 is not differentiated (use vmatrix_batch_scramble=0)");
     const int P = 6 + K;
-    const int ndamped = opts.undamped_last ? P - 1 : P;
-    const size_t ntri = (size_t)P * (P + 1) / 2 + 3 * (size_t)P;
-    const bool use_double = ntri * sizeof(double) <= 200 * 1024;
-    const size_t smem = ntri * (use_double ? sizeof(double) : sizeof(float));
-    BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_solve_update_bwd: P=%d does not fit shared memory", P);
-    pose_update_bwd_kernel<<<(nb + 63) / 64, 64, 0, st>>>(delta, nb, P, R, T, gRn, gTn, dg, dR, dT);       // ddelta[0:6] parked in dg
-    BANET_CUDA_LAUNCH_CHECK("pose_update_bwd_kernel launch");
-    cudaError_t e;
-    if (use_double) {
-        e = cudaFuncSetAttribute(lm_solve_bwd_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { set_error("lm_solve_update_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
-        lm_solve_bwd_kernel<double><<<nb, SB_THREADS, smem, st>>>(H, lambda, delta, P, opts.damping_eps, ndamped, gWn, dH, dg, dlambda, dW);
-    } else {
-        e = cudaFuncSetAttribute(lm_solve_bwd_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { set_error("lm_solve_update_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
-        lm_solve_bwd_kernel<float><<<nb, SB_THREADS, smem, st>>>(H, lambda, delta, P, opts.damping_eps, ndamped, gWn, dH, dg, dlambda, dW);
-    }
-    BANET_CUDA_LAUNCH_CHECK("lm_solve_bwd_kernel launch");
-    return BANET_OK;
+    BANET_REQUIRE(solve_bwd_supported(P), BANET_ERR_UNSUPPORTED, "lm_solve_update_bwd: P=%d does not fit shared memory", P);
+    int rc = launch_pose_update_bwd(delta, nb, P, R, T, gRn, gTn, dg, dR, dT, st);       // ddelta[0:6] parked in dg
+    if (rc) return rc;
+    return launch_solve_bwd(H, lambda, delta, nb, P, 6, opts, gWn, dH, dg, dlambda, dW, st);
 }
 
 }  // namespace banet

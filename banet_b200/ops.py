@@ -323,6 +323,25 @@ def lm_window_run(levels: Sequence[Level], iters_per_level: int, R: Tensor, T: T
     return R, T, Wt[0].clone(), status
 
 
+def lm_window_solve_update(H: Tensor, g: Tensor, lam: Tensor, R: Tensor, T: Tensor, W: Tensor, damping_eps: float = 1e-5, undamped_last: bool = True):
+    """One iteration of a keyframe window after the build (banet_lm_window_solve_update): H [nf,P,P], g [nf,P] from lm_build with nb = nf,
+    lam [1], R [nf,3,3], T [nf,3,1], W [K,1] shared -> R', T', W' [K,1], delta [6 nf + K] (the joint solution), status [nf] (int32)."""
+    lib = load()
+    Hc = _chk(H, "H"); nf, P, _ = Hc.shape
+    K = P - 6
+    gc = _chk(g.reshape(nf, P), "g", (nf, P)); lc = _chk(lam.reshape(1), "lambda", (1,))
+    R = _chk(R, "R", (nf, 3, 3)); T = _chk(T, "T", (nf, 3, 1)); Wt = _chk(W.reshape(K, 1), "W", (K, 1))
+    dev = Hc.device
+    Ro = torch.empty_like(R); To = torch.empty_like(T); Wo = torch.empty_like(Wt)
+    delta = torch.empty(6 * nf + K, device=dev); status = torch.empty(nf, device=dev, dtype=torch.int32)
+    opts = BanetSolveOpts(float(damping_eps), int(undamped_last), 0)
+    ws = _ws(lib.banet_lm_window_solve_update_workspace_bytes(nf, K), dev)
+    check(lib.banet_lm_window_solve_update(Hc.data_ptr(), gc.data_ptr(), lc.data_ptr(), nf, K, C.byref(opts), R.data_ptr(), T.data_ptr(), Wt.data_ptr(),
+                                           Ro.data_ptr(), To.data_ptr(), Wo.data_ptr(), delta.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(),
+                                           _stream()), "banet_lm_window_solve_update")
+    return Ro, To, Wo, delta, status
+
+
 class LMRunGraph:
     """`banet_lm_run` captured ONCE into a CUDA graph and replayed: the library call allocates nothing and never synchronises, so the whole
     coarse-to-fine loop (3 launches per LM iteration) is capturable as it is.  For small or sparse problems (the reference's 4096-point
@@ -409,6 +428,26 @@ def lm_solve_update_bwd(H: Tensor, g: Tensor, lam: Tensor, delta: Tensor, R: Ten
     check(lib.banet_lm_solve_update_bwd(Hc.data_ptr(), gc.data_ptr(), lc.data_ptr(), dl.data_ptr(), nb, K, C.byref(opts), R.data_ptr(), T.data_ptr(),
                                         gR.data_ptr(), gT.data_ptr(), _ptr(gW), dH.data_ptr(), dg.data_ptr(), dlam.data_ptr(), dR.data_ptr(),
                                         dT.data_ptr(), _ptr(dW), _stream()), "banet_lm_solve_update_bwd")
+    return dH, dg, dlam, dR, dT, dW
+
+
+def lm_window_solve_update_bwd(H: Tensor, g: Tensor, lam: Tensor, delta: Tensor, R: Tensor, T: Tensor, dRn: Tensor, dTn: Tensor, dWn: Tensor,
+                               damping_eps: float = 1e-5, undamped_last: bool = True):
+    """Backward of lm_window_solve_update (banet_lm_window_solve_update_bwd) -> dH [nf,P,P], dg [nf,P], dlambda [1], dR, dT, dW [K,1]."""
+    lib = load()
+    Hc = _chk(H, "H"); nf, P, _ = Hc.shape
+    K = P - 6
+    gc = _chk(g.reshape(nf, P), "g", (nf, P)); lc = _chk(lam.reshape(1), "lambda", (1,)); dl = _chk(delta, "delta", (6 * nf + K,))
+    R = _chk(R, "R", (nf, 3, 3)); T = _chk(T, "T", (nf, 3, 1))
+    gR = _chk(dRn, "dR_out", (nf, 3, 3)); gT = _chk(dTn, "dT_out", (nf, 3, 1)); gW = _chk(dWn.reshape(K, 1), "dW_out", (K, 1))
+    dev = Hc.device
+    dH = torch.empty(nf, P, P, device=dev); dg = torch.empty(nf, P, device=dev); dlam = torch.empty(1, device=dev)
+    dR = torch.empty(nf, 3, 3, device=dev); dT = torch.empty(nf, 3, 1, device=dev); dW = torch.empty(K, 1, device=dev)
+    opts = BanetSolveOpts(float(damping_eps), int(undamped_last), 0)
+    ws = _ws(lib.banet_lm_window_solve_update_bwd_workspace_bytes(nf, K), dev)
+    check(lib.banet_lm_window_solve_update_bwd(Hc.data_ptr(), gc.data_ptr(), lc.data_ptr(), dl.data_ptr(), nf, K, C.byref(opts), R.data_ptr(), T.data_ptr(),
+                                               gR.data_ptr(), gT.data_ptr(), gW.data_ptr(), dH.data_ptr(), dg.data_ptr(), dlam.data_ptr(), dR.data_ptr(),
+                                               dT.data_ptr(), dW.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "banet_lm_window_solve_update_bwd")
     return dH, dg, dlam, dR, dT, dW
 
 

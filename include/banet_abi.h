@@ -230,6 +230,29 @@ int    banet_lm_window_run(const banet_level_t* levels, int nlevels, int iters_p
                            float* R, float* T, float* W, int32_t* status,
                            void* ws, size_t ws_bytes, banet_stream_t stream);
 
+/* One window iteration after the build, with the damping given (the training path of the window; SURVEY.md section 8f-4, DESIGN.md §7 item 6):
+ * the step banet_lm_window_run takes per iteration with lambda_fixed -- assembly of the block-arrow system, damping (:264-266), one solve,
+ * per-frame SE(3) update (:269-275), shared W update (:276) -- and the same bits for the same lambda.
+ *   H [nf,P,P], g [nf,P]: banet_lm_build with nb = nf (P = 6 + K); lambda [1]; R [nf,3,3], T [nf,3,1], W [K,1] (shared)
+ *   -> R_out, T_out, W_out [K,1] (may alias the inputs), delta [6 nf + K] (the joint solution: frame f's pose step at 6f, the depth step at
+ *   6 nf; the backward needs it), status [nf] (the window's status for every frame; a skipped step skips every frame: delta = 0).
+ * 6 nf + K must fit the fused solve (<= ~220, as banet_lm_window_run). */
+size_t banet_lm_window_solve_update_workspace_bytes(int nf, int K);
+int    banet_lm_window_solve_update(const float* H, const float* g, const float* lambda, int nf, int K, const banet_solve_opts_t* opts,
+                                    const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
+                                    float* delta, int32_t* status, void* ws, size_t ws_bytes, banet_stream_t stream);
+/* Its backward: gradients of (R',T',W') [dR_out [nf,3,3], dT_out [nf,3,1], dW_out [K,1]] -> dH [nf,P,P] (not symmetric, as
+ * banet_lm_build_bwd takes it), dg [nf,P], dlambda [1], dR, dT, dW [K,1]; every output is overwritten.  dW = dW_out: the build's share of
+ * dW comes from banet_lm_build_bwd.  A skipped step (status != 0, delta = 0) gets zero dH, dg, dlambda and passes dR_out, dT_out, dW_out
+ * through, as banet_lm_solve_update_bwd does.  The backward factors the damped system in fp64 up to 6 nf + K = 220; the forward's fused
+ * solve switches to fp32 above about 200 unknowns. */
+size_t banet_lm_window_solve_update_bwd_workspace_bytes(int nf, int K);
+int    banet_lm_window_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nf, int K,
+                                        const banet_solve_opts_t* opts, const float* R, const float* T,
+                                        const float* dR_out, const float* dT_out, const float* dW_out,
+                                        float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW,
+                                        void* ws, size_t ws_bytes, banet_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * (4) The legacy pose-only keyframe tracker loop: legacy/ba.py:83-145 (`Tracker.trackTF`) with CameraIteration (:147-214) or, with
  *     early termination, CameraIteration2 (:226-345: lambda-MLP step, residual re-evaluated at the updated pose, step kept only if it
