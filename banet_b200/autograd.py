@@ -6,7 +6,8 @@ Two training paths:
     (J, G, d, the tiled upstream gradients of utils.cu:613-617) is materialised, so it runs at any N and K <= 256.  The lambda-MLP
     (5 dense layers on a [nb,C] vector, bundlenet.py:244-248) stays stock torch in between.  Gradient signature = the reference's:
     conv1, conv2, D, B, R, T, W and the lambda-MLP parameters (TF autodiff + the registered op gradient, bundlenet.py:79-82).
-    `window_iteration_fused` is the same for the joint keyframe window (banet_lm_window_solve_update / _bwd after the per-pair build).
+    `window_iteration_fused` is the same for the joint keyframe window (banet_lm_window_solve_update / _bwd after the per-pair build),
+    `window_batch_iteration_fused` for a batch of windows (banet_lm_window_batch_solve_update / _bwd).
   * `iteration` (the reference's own split of labour, kept as the A/B baseline and for op-level drop-in use):
 
     reference:  TF graph ops (warp, resampler, Jacobians, damping, solve, update; TF autodiff)  +  native op
@@ -210,6 +211,30 @@ class _WindowSolveUpdateFn(torch.autograd.Function):
         return dH, dg.reshape(g.shape), dlam.reshape(lam.shape), dR, dT, dW, None
 
 
+class _WindowBatchSolveUpdateFn(torch.autograd.Function):
+    """(R' [nw*nf,3,3], T' [nw*nf,3,1], W' [nw,K,1]) = banet_lm_window_batch_solve_update(H, g, lambda [nw], R, T, W); backward =
+    banet_lm_window_batch_solve_update_bwd.  Saves H, g, lambda, the windows' solutions, R, T: nothing per-pixel."""
+
+    @staticmethod
+    def forward(ctx, H, g, lam, R, T, W, damping_eps):
+        Rn, Tn, Wn, delta, status = ops.lm_window_batch_solve_update(H, g, lam, R, T, W, damping_eps=damping_eps)
+        ctx.save_for_backward(H, g, lam, delta, R, T)
+        ctx.eps = float(damping_eps)
+        ctx.mark_non_differentiable(status)
+        return Rn, Tn, Wn, status
+
+    @staticmethod
+    def backward(ctx, dRn, dTn, dWn, _dstatus):
+        H, g, lam, delta, R, T = ctx.saved_tensors
+        nw, K = lam.numel(), H.shape[1] - 6
+        dRn = dRn if dRn is not None else torch.zeros_like(R)
+        dTn = dTn if dTn is not None else torch.zeros_like(T)
+        dWn = dWn if dWn is not None else torch.zeros(nw, K, 1, device=H.device)
+        dH, dg, dlam, dR, dT, dW = ops.lm_window_batch_solve_update_bwd(H, g, lam, delta, R, T, dRn.contiguous(), dTn.contiguous(), dWn.contiguous(),
+                                                                        ctx.eps)
+        return dH, dg.reshape(g.shape), dlam.reshape(lam.shape), dR, dT, dW, None
+
+
 class _GradFixedConcatFn(torch.autograd.Function):
     """[F | grad_fixed(F)] (+ the half swap of bundlenet.py:386), differentiable (banet_grad_fixed_concat / _bwd)."""
 
@@ -312,6 +337,37 @@ def window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_
         if l2_regularizer_base is not None:
             lam = l2_regularizer_base * lam
     Rn, Tn, Wn, status = _WindowSolveUpdateFn.apply(H, g, lam, R, T, W.reshape(K, 1), damping_eps)
+    if return_status:
+        return Rn, Tn, Wn, status
+    return Rn, Tn, Wn
+
+
+def window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base: Optional[float],
+                                 damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None,
+                                 precision: int = 0, grid=None, return_status: bool = False):
+    """One differentiable LM iteration of a batch of nw keyframe windows of nf frames (window_iteration_fused per window, one launch each
+    for the build, the step and their backwards).  R [nw,nf,3,3], T [nw,nf,3,1], conv2 [nw,nf,h,w,3C] per frame, W [nw,K,1] per window; the
+    keyframe tensors conv1, p, D, B (and intr) are [nw,nf,...] or [nw,1,...] (broadcast to the frames, their gradients summed over them).
+    lambda per window: from the mean |residual| over its nf * N points through the MLP (times l2_regularizer_base), or lambda_override [nw].
+    Returns (R' [nw,nf,3,3], T' [nw,nf,3,1], W' [nw,K,1]) (, status [nw,nf])."""
+    nw, nf = R.shape[0], R.shape[1]
+    K = B.shape[-1]
+    nb = nw * nf
+    pairs = lambda t: (t.expand(nw, nf, *t.shape[2:]) if t.shape[1] == 1 and nf > 1 else t).reshape(nb, *t.shape[2:]).contiguous()
+    conv1, conv2, intr, p, D, B = pairs(conv1), pairs(conv2), pairs(intr), pairs(p), pairs(D), pairs(B)
+    N, C = conv1.shape[1], conv1.shape[2]
+    Wf = W.reshape(nw, 1, K, 1).expand(nw, nf, K, 1).reshape(nb, K, 1).contiguous()   # every pair builds with its window's W
+    Rf, Tf = R.reshape(nb, 3, 3), T.reshape(nb, 3, 1)
+    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, Rf, Tf, Wf, intr.detach(), p.detach(), precision, exact_sym, grid)
+    if lambda_override is not None:
+        lam = lambda_override.reshape(nw)
+    else:
+        avg = (rbar_sum.reshape(nw, nf, C).sum(1) / float(nf * N)).unsqueeze(1)         # mean |residual| over each window's nf * N points
+        lam = torch.pow(torch.linalg.norm(avg, dim=-1, keepdim=True), 2.0 + lambda_mlp(avg, mlp_params)).reshape(nw)
+        if l2_regularizer_base is not None:
+            lam = l2_regularizer_base * lam
+    Rn, Tn, Wn, status = _WindowBatchSolveUpdateFn.apply(H, g, lam, Rf, Tf, W.reshape(nw, K, 1), damping_eps)
+    Rn, Tn, status = Rn.reshape(nw, nf, 3, 3), Tn.reshape(nw, nf, 3, 1), status.reshape(nw, nf)
     if return_status:
         return Rn, Tn, Wn, status
     return Rn, Tn, Wn

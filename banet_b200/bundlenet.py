@@ -150,10 +150,14 @@ class BundleNet(torch.nn.Module):
         """One joint LM iteration of a keyframe window (an extension; the reference's layer is 2-view): the nf pairs (keyframe -> frame f)
         share the keyframe depth D + B.W.  Arguments as BundleIteration with R [nf,3,3], T [nf,3,1], conv2 [nf,h,w,3C] per frame and
         W [K,1] shared; the keyframe tensors conv1, p, D, B may be given once ([1,...]) or per frame.  -> (updatedR, updatedT, updatedW [K,1]).
-        Differentiable (banet_lm_window_solve_update_bwd) whenever gradients are being recorded; there is no reference_split twin."""
+        Differentiable (banet_lm_window_solve_update_bwd) whenever gradients are being recorded; there is no reference_split twin.
+        A batch of nw windows: R [nw,nf,3,3], T [nw,nf,3,1], conv2 [nw,nf,h,w,3C], W [nw,K,1], keyframe tensors and fx, fy, ox, oy
+        [nw,1,...] or [nw,nf,...] -> ([nw,nf,3,3], [nw,nf,3,1], [nw,K,1]), last_status [nw,nf] (banet_lm_window_batch_*)."""
         base = 1.0 if l2_regularizer_base is None else float(l2_regularizer_base)
         if self.vmatrix_batch_scramble:
             raise RuntimeError("vmatrix_batch_scramble=True is a 2-view quirk (bundlenet.py:45); the window solve has per-frame VMatrix only")
+        if R.dim() == 4:
+            return self._window_batch_iteration(conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, base, level)
         nf = R.shape[0]
         intr = _intr_from_tiled(fx, fy, ox, oy)
         if self._wants_grad(conv1, conv2, D, B, R, T, W):
@@ -169,6 +173,25 @@ class BundleNet(torch.nn.Module):
                                                precision=self.precision)
         self._check_status(status)
         return Rn, Tn, Wn
+
+    def _window_batch_iteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, base, level):
+        """WindowIteration on a batch of nw windows (R [nw,nf,3,3]): the fused path when gradients are recorded, else one iteration of
+        ops.lm_window_batch_run."""
+        nw, nf = R.shape[0], R.shape[1]
+        intr = torch.stack([t.reshape(t.shape[0], t.shape[1], -1)[..., 0] for t in (fx, fy, ox, oy)], dim=-1).to(torch.float32)   # [nw,1|nf,4]
+        if self._wants_grad(conv1, conv2, D, B, R, T, W):
+            if self.training_path == "reference_split":
+                raise RuntimeError("training_path='reference_split' has no torch-graph twin of the window solve; use training_path='fused'")
+            Rn, Tn, Wn, status = _ag.window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base,
+                                                                  exact_sym=self.exact_sym_grad, precision=self.precision, return_status=True)
+            self._check_status(status)
+            return Rn, Tn, Wn
+        pairs = lambda t: (t.expand(nw, nf, *t.shape[2:]) if t.shape[1] == 1 else t).reshape(nw * nf, *t.shape[2:])
+        lv = ops.Level(pairs(conv1), pairs(conv2), pairs(intr), pairs(p), pairs(D), pairs(B))
+        Rn, Tn, Wn, status = ops.lm_window_batch_run([lv], nw, 1, R.reshape(nw * nf, 3, 3), T.reshape(nw * nf, 3, 1), W,
+                                                     mlp_packed=[self.mlp_packed(str(level))], l2_regularizer_base=base, precision=self.precision)
+        self._check_status(status.reshape(nw, nf))
+        return Rn.reshape(nw, nf, 3, 3), Tn.reshape(nw, nf, 3, 1), Wn
 
     # ---- level schedulers ----------------------------------------------------------------------
     def _prepare(self, intrisic: Tensor, points: Tensor):

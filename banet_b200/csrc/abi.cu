@@ -415,6 +415,126 @@ extern "C" int banet_lm_window_solve_update_bwd(const float* H, const float* g, 
                               reinterpret_cast<float*>(ws), (cudaStream_t)stream);
 }
 
+// ---- batches of keyframe windows (section 3d): nb = nw nf pairs, pair w nf + f = (keyframe of window w -> frame f) -----------------------
+namespace {
+size_t batch_run_extra(int nw, int nf, int K)                     // per-pair copies of W for the build + the step's per-frame factors
+{
+    return align_up((size_t)nw * nf * K * sizeof(float), 256) + lm_window_batch_ws_bytes(nw, nf);
+}
+}  // namespace
+
+extern "C" size_t banet_lm_window_batch_run_workspace_bytes(const banet_level_t* levels, int nlevels, int nw, int precision)
+{
+    if (!levels || nlevels <= 0 || nw <= 0 || levels[0].K <= 0 || levels[0].nb % nw != 0) return 0;
+    RunCarve c;
+    if (carve(levels, nlevels, precision, &c) != BANET_OK) return 0;
+    return c.total + batch_run_extra(nw, levels[0].nb / nw, levels[0].K);
+}
+
+extern "C" int banet_lm_window_batch_run(const banet_level_t* levels, int nlevels, int nw, int iters_per_level,
+                                         const float* const* mlp_weights, float l2_regularizer_base, float lambda_fixed,
+                                         const banet_solve_opts_t* opts, int precision,
+                                         float* R, float* T, float* W, int32_t* status, void* ws, size_t ws_bytes, banet_stream_t stream)
+{
+    BANET_REQUIRE(levels && opts && R && T && W && status, BANET_ERR_BAD_ARG, "lm_window_batch_run: null pointer");
+    BANET_REQUIRE(nlevels > 0 && iters_per_level > 0 && nw > 0, BANET_ERR_BAD_ARG, "lm_window_batch_run: bad argument nlevels=%d iters=%d nw=%d",
+                  nlevels, iters_per_level, nw);
+    const int nb = levels[0].nb, K = levels[0].K;
+    BANET_REQUIRE(K > 0 && !opts->vmatrix_batch_scramble, BANET_ERR_BAD_ARG, "lm_window_batch_run: needs a depth basis (K > 0) and vmatrix_batch_scramble = 0");
+    BANET_REQUIRE(nb > 0 && nb % nw == 0, BANET_ERR_BAD_ARG, "lm_window_batch_run: nb=%d is not nw * nf with nw=%d", nb, nw);
+    const int nf = nb / nw;
+    for (int l = 0; l < nlevels; ++l) {
+        int rc = check_level(&levels[l], "lm_window_batch_run");
+        if (rc) return rc;
+        BANET_REQUIRE(levels[l].nb == nb && levels[l].K == K, BANET_ERR_BAD_ARG, "lm_window_batch_run: nb/K must agree across levels");
+        BANET_REQUIRE((mlp_weights && mlp_weights[l]) || lambda_fixed >= 0.f, BANET_ERR_BAD_ARG,
+                      "lm_window_batch_run: level %d has no lambda-MLP weights and lambda_fixed < 0", l);
+        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
+        BANET_REQUIRE(lm_window_batch_supported(K, use_mlp ? levels[l].C : 0), BANET_ERR_UNSUPPORTED,
+                      "lm_window_batch_run: K=%d (C=%d) does not fit the window step (K <= 256)", K, levels[l].C);
+    }
+    RunCarve c;
+    int rc = carve(levels, nlevels, precision, &c);
+    if (rc) return rc;
+    const size_t need = c.total + batch_run_extra(nw, nf, K);
+    BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_window_batch_run: workspace %zu < %zu bytes", ws_bytes, need);
+    cudaStream_t st = (cudaStream_t)stream;
+    char* base = reinterpret_cast<char*>(ws);
+    float* H = reinterpret_cast<float*>(base + c.H);
+    float* g = reinterpret_cast<float*>(base + c.g);
+    float* rbar = reinterpret_cast<float*>(base + c.rbar);
+    float* nvalid = reinterpret_cast<float*>(base + c.nvalid);
+    float* lam = reinterpret_cast<float*>(base + c.lambda);            // [nw]
+    float* delta = reinterpret_cast<float*>(base + c.delta);          // [nw, 6 nf + K] <= [nb, 6 + K]
+    float* Wp = reinterpret_cast<float*>(base + c.total);             // [nb, K] per-pair copies of the windows' W
+    void* fws = base + c.total + align_up((size_t)nb * K * sizeof(float), 256);
+    zero_status_kernel<<<(nb + 255) / 256, 256, 0, st>>>(status, nb);
+    rc = lm_window_batch_broadcast_w(W, nw, nf, K, Wp, st);
+    if (rc) return rc;
+    for (int l = 0; l < nlevels; ++l) {
+        const banet_level_t* lv = &levels[l];
+        BuildPlan plan;
+        const int res = resolve_precision(lv, precision);
+        if (res < 0) return res;
+        rc = plan_for(lv, res, &plan);
+        if (rc) return rc;
+        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
+        if (!use_mlp) fill_kernel<<<(nw + 255) / 256, 256, 0, st>>>(lam, nw, lambda_fixed);
+        for (int it = 0; it < iters_per_level; ++it) {                // one build launch and one step launch per iteration
+            rc = build_dispatch(lv, res, plan, R, T, Wp, H, g, rbar, nvalid, base + c.build, st);
+            if (rc) return rc;
+            rc = lm_window_batch_step(H, g, rbar, nw, nf, lv->N, lv->C, K, use_mlp ? mlp_weights[l] : nullptr, l2_regularizer_base,
+                                      use_mlp ? nullptr : lam, *opts, R, T, W, R, T, W, Wp, delta, use_mlp ? lam : nullptr, status, 1, fws, st);
+            if (rc) return rc;
+        }
+    }
+    BANET_CUDA_LAUNCH_CHECK("lm_window_batch_run");
+    return BANET_OK;
+}
+
+extern "C" size_t banet_lm_window_batch_solve_update_workspace_bytes(int nw, int nf, int K)
+{
+    if (nw <= 0 || nf <= 0 || K <= 0) return 0;
+    return lm_window_batch_ws_bytes(nw, nf);
+}
+
+extern "C" int banet_lm_window_batch_solve_update(const float* H, const float* g, const float* lambda, int nw, int nf, int K, const banet_solve_opts_t* opts,
+                                                  const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
+                                                  float* delta, int32_t* status, void* ws, size_t ws_bytes, banet_stream_t stream)
+{
+    BANET_REQUIRE(H && g && lambda && opts && R && T && W && R_out && T_out && W_out && delta && status, BANET_ERR_BAD_ARG,
+                  "lm_window_batch_solve_update: null pointer");
+    BANET_REQUIRE(nw > 0 && nf > 0 && K > 0 && !opts->vmatrix_batch_scramble, BANET_ERR_BAD_ARG,
+                  "lm_window_batch_solve_update: needs nw, nf > 0, a depth basis (K > 0) and vmatrix_batch_scramble = 0 (nw=%d nf=%d K=%d)", nw, nf, K);
+    BANET_REQUIRE(lm_window_batch_supported(K, 0), BANET_ERR_UNSUPPORTED, "lm_window_batch_solve_update: K=%d does not fit the window step (K <= 256)", K);
+    const size_t need = banet_lm_window_batch_solve_update_workspace_bytes(nw, nf, K);
+    BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_window_batch_solve_update: workspace %zu < %zu bytes", ws_bytes, need);
+    return lm_window_batch_step(H, g, nullptr, nw, nf, 1, 0, K, nullptr, 1.f, lambda, *opts, R, T, W, R_out, T_out, W_out, nullptr, delta,
+                                nullptr, status, 0, ws, (cudaStream_t)stream);
+}
+
+extern "C" size_t banet_lm_window_batch_solve_update_bwd_workspace_bytes(int nw, int nf, int K)
+{
+    if (nw <= 0 || nf <= 0 || K <= 0) return 0;
+    return lm_window_batch_ws_bytes(nw, nf);
+}
+
+extern "C" int banet_lm_window_batch_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nw, int nf, int K,
+                                                      const banet_solve_opts_t* opts, const float* R, const float* T,
+                                                      const float* dR_out, const float* dT_out, const float* dW_out,
+                                                      float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW,
+                                                      void* ws, size_t ws_bytes, banet_stream_t stream)
+{
+    BANET_REQUIRE(H && g && lambda && delta && opts && R && T && dR_out && dT_out && dW_out && dH && dg && dlambda && dR && dT && dW, BANET_ERR_BAD_ARG,
+                  "lm_window_batch_solve_update_bwd: null pointer");
+    BANET_REQUIRE(nw > 0 && nf > 0 && K > 0 && !opts->vmatrix_batch_scramble, BANET_ERR_BAD_ARG,
+                  "lm_window_batch_solve_update_bwd: needs nw, nf > 0, a depth basis (K > 0) and vmatrix_batch_scramble = 0 (nw=%d nf=%d K=%d)", nw, nf, K);
+    BANET_REQUIRE(lm_window_batch_supported(K, 0), BANET_ERR_UNSUPPORTED, "lm_window_batch_solve_update_bwd: K=%d does not fit the window step (K <= 256)", K);
+    const size_t need = banet_lm_window_batch_solve_update_bwd_workspace_bytes(nw, nf, K);
+    BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_window_batch_solve_update_bwd: workspace %zu < %zu bytes", ws_bytes, need);
+    return lm_window_batch_step_bwd(H, g, lambda, delta, nw, nf, K, *opts, R, T, dR_out, dT_out, dW_out, dH, dg, dlambda, dR, dT, dW, ws, (cudaStream_t)stream);
+}
+
 extern "C" size_t banet_lm_track_legacy_workspace_bytes(const banet_level_t* levels, int nlevels)
 {
     if (!levels || nlevels <= 0) return 0;

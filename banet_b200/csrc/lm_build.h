@@ -80,6 +80,20 @@ int lm_window_step_bwd(const float* H, const float* g, const float* lambda, cons
                        const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
                        float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, float* ws, cudaStream_t st);
 
+// a batch of keyframe windows (nw windows of nf frames, pair w nf + f), each stepped by eliminating its pose blocks (lm_window_batch.cu); ws:
+// lm_window_batch_ws_bytes.  W [nw,K] -> W_out; W_pairs [nw nf,K] (optional) receives W' per pair for the next build.  delta [nw, 6 nf + K].
+bool lm_window_batch_supported(int K, int C);
+size_t lm_window_batch_ws_bytes(int nw, int nf);
+int lm_window_batch_broadcast_w(const float* W, int nw, int nf, int K, float* W_pairs, cudaStream_t st);
+int lm_window_batch_step(const float* H, const float* g, const float* rbar_sum, int nw, int nf, int N, int C, int K, const float* mlp, float base,
+                         const float* lambda_in, const banet_solve_opts_t& opts, const float* R, const float* T, const float* W,
+                         float* R_out, float* T_out, float* W_out, float* W_pairs, float* delta, float* lambda_out, int32_t* status,
+                         int status_accumulate, void* ws, cudaStream_t st);
+// its backward (lambda given): dH [nw nf,P,P], dg [nw nf,P], dlambda [nw], dR, dT [nw nf,...], dW [nw,K]
+int lm_window_batch_step_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nw, int nf, int K, const banet_solve_opts_t& opts,
+                             const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
+                             float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, void* ws, cudaStream_t st);
+
 // legacy pose-only tracker loop with device-side accept / reject and early termination (lm_legacy.cu)
 size_t lm_track_legacy_workspace_bytes(const banet_level_t* levels, int nlevels);
 int lm_track_legacy(const banet_level_t* levels, int nlevels, const int* level_iters, const float* const* mlp_weights, const banet_legacy_opts_t& o,

@@ -342,6 +342,53 @@ def lm_window_solve_update(H: Tensor, g: Tensor, lam: Tensor, R: Tensor, T: Tens
     return Ro, To, Wo, delta, status
 
 
+def lm_window_batch_run(levels: Sequence[Level], nw: int, iters_per_level: int, R: Tensor, T: Tensor, W: Tensor,
+                        mlp_packed: Optional[Sequence[Optional[Tensor]]] = None, l2_regularizer_base: Optional[float] = None,
+                        lambda_fixed: float = -1.0, damping_eps: float = 1e-5, undamped_last: bool = True,
+                        precision: int = _lib.PREC_AUTO, workspace: Optional[Tensor] = None):
+    """Joint coarse-to-fine solve of a batch of nw keyframe windows (banet_lm_window_batch_run): every level holds nb = nw * nf pairs, pair
+    w * nf + f = (keyframe of window w -> frame f).  R [nb,3,3], T [nb,3,1] per frame, W [nw,K,1] per window.  Returns new
+    (R, T, W [nw,K,1], status [nb])."""
+    lib = load()
+    arr, nlev, nb, K, mlp_ptrs, base, opts, _, _keep = _prepare_run(levels, mlp_packed, l2_regularizer_base, damping_eps, undamped_last,
+                                                                   False, precision)
+    nbytes = lib.banet_lm_window_batch_run_workspace_bytes(arr, nlev, int(nw), precision)
+    if nbytes == 0:
+        check(-4 if nw > 0 and nb % nw == 0 else -1, "banet_lm_window_batch_run_workspace_bytes")
+    R = _chk(R, "R", (nb, 3, 3)).clone(); T = _chk(T, "T", (nb, 3, 1)).clone()
+    Wt = _chk(W.reshape(nw, K, 1), "W", (nw, K, 1)).clone()
+    ws = workspace if workspace is not None and workspace.numel() >= nbytes else _ws(nbytes, R.device)
+    status = torch.empty(nb, device=R.device, dtype=torch.int32)
+    check(lib.banet_lm_window_batch_run(arr, nlev, int(nw), int(iters_per_level), mlp_ptrs, base, float(lambda_fixed), C.byref(opts), precision,
+                                        R.data_ptr(), T.data_ptr(), Wt.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(), _stream()),
+          "banet_lm_window_batch_run")
+    return R, T, Wt, status
+
+
+def lm_window_batch_solve_update(H: Tensor, g: Tensor, lam: Tensor, R: Tensor, T: Tensor, W: Tensor, damping_eps: float = 1e-5,
+                                 undamped_last: bool = True):
+    """One iteration of nw keyframe windows after the build (banet_lm_window_batch_solve_update): H [nw*nf,P,P], g [nw*nf,P] from lm_build,
+    lam [nw], R [nw*nf,3,3], T [nw*nf,3,1], W [nw,K,1] -> R', T', W' [nw,K,1], delta [nw, 6 nf + K], status [nw*nf] (int32)."""
+    lib = load()
+    Hc = _chk(H, "H"); nb, P, _ = Hc.shape
+    K = P - 6
+    nw = lam.numel()
+    if nw == 0 or nb % nw:
+        raise _lib.BanetError(f"lambda has {nw} windows, which does not divide the {nb} pairs")
+    nf = nb // nw
+    gc = _chk(g.reshape(nb, P), "g", (nb, P)); lc = _chk(lam.reshape(nw), "lambda", (nw,))
+    R = _chk(R, "R", (nb, 3, 3)); T = _chk(T, "T", (nb, 3, 1)); Wt = _chk(W.reshape(nw, K, 1), "W", (nw, K, 1))
+    dev = Hc.device
+    Ro = torch.empty_like(R); To = torch.empty_like(T); Wo = torch.empty_like(Wt)
+    delta = torch.empty(nw, 6 * nf + K, device=dev); status = torch.empty(nb, device=dev, dtype=torch.int32)
+    opts = BanetSolveOpts(float(damping_eps), int(undamped_last), 0)
+    ws = _ws(lib.banet_lm_window_batch_solve_update_workspace_bytes(nw, nf, K), dev)
+    check(lib.banet_lm_window_batch_solve_update(Hc.data_ptr(), gc.data_ptr(), lc.data_ptr(), nw, nf, K, C.byref(opts), R.data_ptr(), T.data_ptr(),
+                                                 Wt.data_ptr(), Ro.data_ptr(), To.data_ptr(), Wo.data_ptr(), delta.data_ptr(), status.data_ptr(),
+                                                 ws.data_ptr(), ws.numel(), _stream()), "banet_lm_window_batch_solve_update")
+    return Ro, To, Wo, delta, status
+
+
 class LMRunGraph:
     """`banet_lm_run` captured ONCE into a CUDA graph and replayed: the library call allocates nothing and never synchronises, so the whole
     coarse-to-fine loop (3 launches per LM iteration) is capturable as it is.  For small or sparse problems (the reference's 4096-point
@@ -448,6 +495,32 @@ def lm_window_solve_update_bwd(H: Tensor, g: Tensor, lam: Tensor, delta: Tensor,
     check(lib.banet_lm_window_solve_update_bwd(Hc.data_ptr(), gc.data_ptr(), lc.data_ptr(), dl.data_ptr(), nf, K, C.byref(opts), R.data_ptr(), T.data_ptr(),
                                                gR.data_ptr(), gT.data_ptr(), gW.data_ptr(), dH.data_ptr(), dg.data_ptr(), dlam.data_ptr(), dR.data_ptr(),
                                                dT.data_ptr(), dW.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "banet_lm_window_solve_update_bwd")
+    return dH, dg, dlam, dR, dT, dW
+
+
+def lm_window_batch_solve_update_bwd(H: Tensor, g: Tensor, lam: Tensor, delta: Tensor, R: Tensor, T: Tensor, dRn: Tensor, dTn: Tensor, dWn: Tensor,
+                                     damping_eps: float = 1e-5, undamped_last: bool = True):
+    """Backward of lm_window_batch_solve_update (banet_lm_window_batch_solve_update_bwd) -> dH [nw*nf,P,P], dg [nw*nf,P], dlambda [nw],
+    dR, dT, dW [nw,K,1]."""
+    lib = load()
+    Hc = _chk(H, "H"); nb, P, _ = Hc.shape
+    K = P - 6
+    nw = lam.numel()
+    if nw == 0 or nb % nw:
+        raise _lib.BanetError(f"lambda has {nw} windows, which does not divide the {nb} pairs")
+    nf = nb // nw
+    gc = _chk(g.reshape(nb, P), "g", (nb, P)); lc = _chk(lam.reshape(nw), "lambda", (nw,)); dl = _chk(delta, "delta", (nw, 6 * nf + K))
+    R = _chk(R, "R", (nb, 3, 3)); T = _chk(T, "T", (nb, 3, 1))
+    gR = _chk(dRn, "dR_out", (nb, 3, 3)); gT = _chk(dTn, "dT_out", (nb, 3, 1)); gW = _chk(dWn.reshape(nw, K, 1), "dW_out", (nw, K, 1))
+    dev = Hc.device
+    dH = torch.empty(nb, P, P, device=dev); dg = torch.empty(nb, P, device=dev); dlam = torch.empty(nw, device=dev)
+    dR = torch.empty(nb, 3, 3, device=dev); dT = torch.empty(nb, 3, 1, device=dev); dW = torch.empty(nw, K, 1, device=dev)
+    opts = BanetSolveOpts(float(damping_eps), int(undamped_last), 0)
+    ws = _ws(lib.banet_lm_window_batch_solve_update_bwd_workspace_bytes(nw, nf, K), dev)
+    check(lib.banet_lm_window_batch_solve_update_bwd(Hc.data_ptr(), gc.data_ptr(), lc.data_ptr(), dl.data_ptr(), nw, nf, K, C.byref(opts), R.data_ptr(),
+                                                     T.data_ptr(), gR.data_ptr(), gT.data_ptr(), gW.data_ptr(), dH.data_ptr(), dg.data_ptr(),
+                                                     dlam.data_ptr(), dR.data_ptr(), dT.data_ptr(), dW.data_ptr(), ws.data_ptr(), ws.numel(), _stream()),
+          "banet_lm_window_batch_solve_update_bwd")
     return dH, dg, dlam, dR, dT, dW
 
 

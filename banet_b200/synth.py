@@ -112,12 +112,14 @@ class Scene:
 def make_scene(nb: int, H: int, W: int, C: int, K: int, level_ids=(0, 1, 2, 3), seed: int = 1234,
                device="cpu", dtype=torch.float32, n_points: Optional[int] = None,
                rot_deg: float = 1.0, trans_m: float = 0.02, w_std: float = 0.02,
-               start_trans_noise_m: float = 0.01, pair_chunk: int = 4, shared_depth: bool = False) -> Scene:
+               start_trans_noise_m: float = 0.01, pair_chunk: int = 4, shared_depth: bool = False,
+               window_frames: Optional[int] = None) -> Scene:
     """Build a planted-solution scene.  (H,W) is the finest (level-3) resolution; level l has
     (H,W)/2**(3-l).  K == 0 -> pose-only scene (B None).  n_points: if given, use that many random
     sub-pixel points per level instead of the dense grid (the reference's sparse mode,
     legacy/seq_example.py:12,72-82).  shared_depth: the nb pairs are (keyframe -> frame f) of one window: same D, B and planted W for
-    every pair, own pose and own frame features (the joint window solve, ops.lm_window_run)."""
+    every pair, own pose and own frame features (the joint window solve, ops.lm_window_run).  window_frames = nf (with shared_depth): nb / nf
+    independent windows (ops.lm_window_batch_run), pairs w nf .. w nf + nf - 1 share window w's depth, basis and planted W; None: one window."""
     g = torch.Generator(device="cpu").manual_seed(seed)
     dev = torch.device(device)
 
@@ -131,8 +133,12 @@ def make_scene(nb: int, H: int, W: int, C: int, K: int, level_ids=(0, 1, 2, 3), 
     R_true = rodrigues(w_true)
     T_true = (randn(nb, 3) * trans_m).unsqueeze(-1)
     W_true = (randn(nb, K) * w_std).unsqueeze(-1) if K > 0 else None
+    gf = nb if window_frames is None else int(window_frames)         # pairs per window
+    if shared_depth and nb % gf:
+        raise ValueError(f"window_frames={gf} does not divide nb={nb}")
+    ng = nb // gf
     if shared_depth and K > 0:
-        W_true = W_true[:1].repeat(nb, 1, 1)
+        W_true = W_true[::gf].repeat_interleave(gf, 0)
     R0 = torch.eye(3, device=dev, dtype=dtype).repeat(nb, 1, 1)
     T0 = T_true + randn(nb, 3, 1) * start_trans_noise_m
     W0 = torch.zeros(nb, K, 1, device=dev, dtype=dtype) if K > 0 else None
@@ -159,8 +165,8 @@ def make_scene(nb: int, H: int, W: int, C: int, K: int, level_ids=(0, 1, 2, 3), 
         D = torch.empty(nb, N, 1, device=dev, dtype=dtype)
         Bm = torch.empty(nb, N, K, device=dev, dtype=dtype) if K > 0 else None
         sig_b = max(1.0, 8.0 / scale)
-        shared_dmap = gaussian_blur_nchw(1.0 + 2.0 * rand(1, 1, h, w), sig_b).permute(0, 2, 3, 1) if shared_depth else None
-        shared_bm = gaussian_blur_nchw(randn(1, K, h, w), sig_b) if shared_depth and K > 0 else None
+        shared_dmap = gaussian_blur_nchw(1.0 + 2.0 * rand(ng, 1, h, w), sig_b).permute(0, 2, 3, 1) if shared_depth else None
+        shared_bm = gaussian_blur_nchw(randn(ng, K, h, w), sig_b) if shared_depth and K > 0 else None
         for b0 in range(0, nb, pair_chunk):                 # chunked so cfg2-sized scenes fit comfortably
             b1 = min(nb, b0 + pair_chunk)
             n = b1 - b0
@@ -168,7 +174,8 @@ def make_scene(nb: int, H: int, W: int, C: int, K: int, level_ids=(0, 1, 2, 3), 
             f2 = f2 / f2.flatten(2).std(dim=2).clamp_min(1e-6).view(n, C, 1, 1)
             f2 = f2.permute(0, 2, 3, 1).contiguous()
             conv2[b0:b1] = grad_fixed_nhwc(f2)
-            dmap = shared_dmap.expand(n, -1, -1, -1) if shared_depth else gaussian_blur_nchw(1.0 + 2.0 * rand(n, 1, h, w), sig_b).permute(0, 2, 3, 1)
+            grp = torch.arange(b0, b1, device=dev) // gf                                   # the window of each pair
+            dmap = shared_dmap[grp] if shared_depth else gaussian_blur_nchw(1.0 + 2.0 * rand(n, 1, h, w), sig_b).permute(0, 2, 3, 1)
             # rescale the blurred map back to span ~[1,3] m
             dmin = dmap.flatten(1).min(1).values.view(n, 1, 1, 1); dmax = dmap.flatten(1).max(1).values.view(n, 1, 1, 1)
             dmap = 1.0 + 2.0 * (dmap - dmin) / (dmax - dmin).clamp_min(1e-6)
@@ -176,7 +183,7 @@ def make_scene(nb: int, H: int, W: int, C: int, K: int, level_ids=(0, 1, 2, 3), 
             D[b0:b1] = bilinear_zero_pad(dmap.contiguous(), xs, ys)
             Dt = D[b0:b1]
             if K > 0:
-                bm = shared_bm.expand(n, -1, -1, -1) if shared_depth else gaussian_blur_nchw(randn(n, K, h, w), sig_b)
+                bm = shared_bm[grp] if shared_depth else gaussian_blur_nchw(randn(n, K, h, w), sig_b)
                 bm = bm * torch.rsqrt(bm.flatten(2).var(dim=2) + 1e-3).view(n, K, 1, 1)
                 Bm[b0:b1] = bilinear_zero_pad(bm.permute(0, 2, 3, 1).contiguous(), xs, ys)
                 Dt = Dt + Bm[b0:b1] @ W_true[b0:b1]

@@ -222,7 +222,9 @@ int    banet_lm_run(const banet_level_t* levels, int nlevels, int iters_per_leve
  *      reference's damping (:264-266, last depth coefficient undamped), ONE solve, per-frame SE(3) update (:269-275), shared W update.
  *      Same arguments as banet_lm_run.  conv1, p, D, B of a level hold the keyframe's tensors once per frame (the [nb,...] layout).
  *      W [nf,K,1]: frame 0's row is the window's W on entry (it is broadcast), every row holds the shared result on exit.
- *      status [nf]: the window's status (a skipped step skips every frame).  6 nf + K must fit the fused solve (<= ~220). */
+ *      status [nf]: the window's status (a skipped step skips every frame).  6 nf + K must fit the fused dense solve: it factors in fp64 up to
+ *      218 unknowns and in fp32 up to 325 (at C = 128; 220 and 329 with lambda_fixed), and rejects larger windows with BANET_ERR_UNSUPPORTED
+ *      (nf <= 15 in fp64 and nf <= 32 at all at K = 128).  Section (3d) has no such limit. */
 size_t banet_lm_window_run_workspace_bytes(const banet_level_t* levels, int nlevels, int precision);
 int    banet_lm_window_run(const banet_level_t* levels, int nlevels, int iters_per_level,
                            const float* const* mlp_weights, float l2_regularizer_base, float lambda_fixed,
@@ -236,7 +238,7 @@ int    banet_lm_window_run(const banet_level_t* levels, int nlevels, int iters_p
  *   H [nf,P,P], g [nf,P]: banet_lm_build with nb = nf (P = 6 + K); lambda [1]; R [nf,3,3], T [nf,3,1], W [K,1] (shared)
  *   -> R_out, T_out, W_out [K,1] (may alias the inputs), delta [6 nf + K] (the joint solution: frame f's pose step at 6f, the depth step at
  *   6 nf; the backward needs it), status [nf] (the window's status for every frame; a skipped step skips every frame: delta = 0).
- * 6 nf + K must fit the fused solve (<= ~220, as banet_lm_window_run). */
+ * 6 nf + K must fit the fused dense solve: fp64 up to 220 unknowns, fp32 up to 329, BANET_ERR_UNSUPPORTED beyond. */
 size_t banet_lm_window_solve_update_workspace_bytes(int nf, int K);
 int    banet_lm_window_solve_update(const float* H, const float* g, const float* lambda, int nf, int K, const banet_solve_opts_t* opts,
                                     const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
@@ -244,14 +246,58 @@ int    banet_lm_window_solve_update(const float* H, const float* g, const float*
 /* Its backward: gradients of (R',T',W') [dR_out [nf,3,3], dT_out [nf,3,1], dW_out [K,1]] -> dH [nf,P,P] (not symmetric, as
  * banet_lm_build_bwd takes it), dg [nf,P], dlambda [1], dR, dT, dW [K,1]; every output is overwritten.  dW = dW_out: the build's share of
  * dW comes from banet_lm_build_bwd.  A skipped step (status != 0, delta = 0) gets zero dH, dg, dlambda and passes dR_out, dT_out, dW_out
- * through, as banet_lm_solve_update_bwd does.  The backward factors the damped system in fp64 up to 6 nf + K = 220; the forward's fused
- * solve switches to fp32 above about 200 unknowns. */
+ * through, as banet_lm_solve_update_bwd does.  The backward factors the damped system in fp64 up to 6 nf + K = 222 and in fp32 up to 332;
+ * the forward's fused solve switches to fp32 above 220 unknowns and rejects more than 329. */
 size_t banet_lm_window_solve_update_bwd_workspace_bytes(int nf, int K);
 int    banet_lm_window_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nf, int K,
                                         const banet_solve_opts_t* opts, const float* R, const float* T,
                                         const float* dR_out, const float* dT_out, const float* dW_out,
                                         float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW,
                                         void* ws, size_t ws_bytes, banet_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * (3d) Batches of keyframe windows — the same extension as (3c), nw windows per call, each solved through its block-arrow structure:
+ *      the per-frame 6x6 pose blocks are eliminated (Schur complement) and only the K x K depth system is factored, so nf is limited by
+ *      the workspace only.  The maths is (3c)'s: lambda from the window's mean |residual| over its nf N points through the MLP
+ *      (bundlenet.py:241-253), damping of every diagonal entry but the last depth coefficient (:264-266), per-frame SE(3) update (:269-275),
+ *      shared W update (:276); results agree with (3c) to fp32 rounding, not bit for bit (a different factorisation).
+ *      Conventions: pair w*nf + f is (keyframe of window w -> frame f); H, g, R, T, conv1 ... of a level are per pair ([nw*nf,...]: the
+ *      keyframe's tensors once per frame), W [nw,K,1] and lambda [nw] per window, status [nw*nf] (a window's status for each of its frames:
+ *      0 ok, 1 non-positive pivot in a frame's 6x6 block or in the depth system, 2 non-finite input; a skipped window has delta = 0 and
+ *      keeps its R, T, W; other windows are not affected).  delta [nw, 6 nf + K]: frame f's pose step at 6f, the depth step at 6 nf.
+ *      The depth system is factored in fp64 while it fits shared memory (K <= 211 at C = 128, K <= 215 with lambda given), else in fp32;
+ *      K <= 256 (the build's range).  Every sum is taken in a fixed order: bit-reproducible, independent of the workspace's contents.
+ *      Argument errors (null pointers, nw, nf, K <= 0, vmatrix_batch_scramble != 0, nb != nw*nf: BANET_ERR_BAD_ARG; K out of range:
+ *      BANET_ERR_UNSUPPORTED; workspace too small: BANET_ERR_WORKSPACE) are reported before any CUDA call.
+ * ---------------------------------------------------------------------------------------------- */
+/* Whole coarse-to-fine solve of nw windows: banet_lm_window_run's arguments plus nw; levels[l].nb == nw*nf.  Each iteration is one build
+ * launch (all nw*nf pairs) and one step launch (all nw windows).  R [nw*nf,3,3], T [nw*nf,3,1], W [nw,K,1] are updated in place; status
+ * [nw*nf] accumulates (bitwise or).  The per-pair copies of W the build reads live in the workspace. */
+size_t banet_lm_window_batch_run_workspace_bytes(const banet_level_t* levels, int nlevels, int nw, int precision);
+int    banet_lm_window_batch_run(const banet_level_t* levels, int nlevels, int nw, int iters_per_level,
+                                 const float* const* mlp_weights, float l2_regularizer_base, float lambda_fixed,
+                                 const banet_solve_opts_t* opts, int precision,
+                                 float* R, float* T, float* W, int32_t* status,
+                                 void* ws, size_t ws_bytes, banet_stream_t stream);
+
+/* One iteration of nw windows after the build, with the damping given (the training path; banet_lm_window_solve_update per window):
+ *   H [nw*nf,P,P], g [nw*nf,P] (banet_lm_build with nb = nw*nf, P = 6 + K), lambda [nw], R [nw*nf,3,3], T [nw*nf,3,1], W [nw,K,1]
+ *   -> R_out, T_out, W_out (may alias the inputs), delta [nw, 6 nf + K] (the backward needs it), status [nw*nf]. */
+size_t banet_lm_window_batch_solve_update_workspace_bytes(int nw, int nf, int K);
+int    banet_lm_window_batch_solve_update(const float* H, const float* g, const float* lambda, int nw, int nf, int K, const banet_solve_opts_t* opts,
+                                          const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
+                                          float* delta, int32_t* status, void* ws, size_t ws_bytes, banet_stream_t stream);
+/* Its backward: gradients of (R',T',W') [dR_out [nw*nf,3,3], dT_out [nw*nf,3,1], dW_out [nw,K,1]] -> dH [nw*nf,P,P] (not symmetric, as
+ * banet_lm_build_bwd takes it), dg [nw*nf,P], dlambda [nw], dR, dT, dW [nw,K,1]; every output is overwritten.  Per window these are
+ * banet_lm_window_solve_update_bwd's values: the solve backward (the (1 + lambda) factor on the damped diagonal) composed with the
+ * assembly's adjoint, the depth block's gradient given to every frame, written per pair.  dW = dW_out.  A skipped window (the forward's
+ * status, re-derived from H, g, lambda) gets zero dH, dg, dlambda and passes dR_out, dT_out, dW_out through. */
+size_t banet_lm_window_batch_solve_update_bwd_workspace_bytes(int nw, int nf, int K);
+int    banet_lm_window_batch_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nw, int nf, int K,
+                                              const banet_solve_opts_t* opts, const float* R, const float* T,
+                                              const float* dR_out, const float* dT_out, const float* dW_out,
+                                              float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW,
+                                              void* ws, size_t ws_bytes, banet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * (4) The legacy pose-only keyframe tracker loop: legacy/ba.py:83-145 (`Tracker.trackTF`) with CameraIteration (:147-214) or, with
