@@ -27,6 +27,14 @@ class BanetLevel(C.Structure):
                 ("grid_w", C.c_int), ("grid_h", C.c_int)]
 
 
+class BanetKeyframeLevel(C.Structure):
+    """struct banet_keyframe_level (include/banet_abi.h): the keyframe tensors once per window, the frame tensors per pair."""
+    _fields_ = [("nw", C.c_int), ("nf", C.c_int), ("N", C.c_int), ("C", C.c_int), ("K", C.c_int),
+                ("h", C.c_int), ("w", C.c_int), ("conv2_channels", C.c_int),
+                ("conv1", C.c_void_p), ("p", C.c_void_p), ("D", C.c_void_p), ("B", C.c_void_p),
+                ("conv2", C.c_void_p), ("intr", C.c_void_p)]
+
+
 class BanetSolveOpts(C.Structure):
     """struct banet_solve_opts (include/banet_abi.h)."""
     _fields_ = [("damping_eps", C.c_float), ("undamped_last", C.c_int), ("vmatrix_batch_scramble", C.c_int)]
@@ -94,6 +102,13 @@ SIGNATURES = {
     "banet_lm_window_batch_solve_update_bwd_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
     "banet_lm_window_batch_solve_update_bwd": (C.c_int, [c_float_p] * 4 + [C.c_int] * 3 + [C.POINTER(BanetSolveOpts)] + [c_float_p] * 5
                                                + [c_float_p] * 6 + [C.c_void_p, C.c_size_t, c_stream]),
+    "banet_lm_keyframe_build_workspace_bytes": (C.c_size_t, [C.POINTER(BanetKeyframeLevel)]),
+    "banet_lm_keyframe_build": (C.c_int, [C.POINTER(BanetKeyframeLevel)] + [c_float_p] * 3 + [c_float_p] * 4 + [C.c_void_p, C.c_size_t, c_stream]),
+    "banet_lm_keyframe_build_bwd": (C.c_int, [C.POINTER(BanetKeyframeLevel)] + [c_float_p] * 6 + [C.c_int] + [c_float_p] * 7 + [c_stream]),
+    "banet_lm_keyframe_run_workspace_bytes": (C.c_size_t, [C.POINTER(BanetKeyframeLevel), C.c_int, C.c_int]),
+    "banet_lm_keyframe_run": (C.c_int, [C.POINTER(BanetKeyframeLevel), C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_float, C.c_float,
+                                        C.POINTER(BanetSolveOpts), C.c_int] + [c_float_p] * 3 + [C.c_void_p]
+                              + [C.c_void_p, C.c_size_t, c_stream]),
     "banet_depth_compose": (C.c_int, [c_float_p] * 3 + [C.c_int] * 3 + [c_float_p, c_stream]),
     "banet_lm_step": (C.c_int, [c_float_p] * 3 + [C.c_int] * 4 + [c_float_p, C.c_float, c_float_p, C.POINTER(BanetSolveOpts)] + [c_float_p] * 3
                       + [c_float_p] * 3 + [c_float_p, c_float_p, C.c_void_p, c_stream]),

@@ -161,6 +161,32 @@ class _LMBuildFn(torch.autograd.Function):
         return dconv1, dconv2, dD, dB, dR, dT, dW, None, None, None, None, None
 
 
+class _KeyframeBuildFn(torch.autograd.Function):
+    """(H, g, rbar_sum) = banet_lm_keyframe_build(...) (the window-reduced per-pair system); backward = banet_lm_keyframe_build_bwd.
+    conv1 [nw,N,C], D, B, p once per window; conv2, intr, R, T per pair; W [nw,K,1].  Saves the inputs only: no per-frame copy of the
+    keyframe."""
+
+    @staticmethod
+    def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, exact_sym):
+        lv = ops.KeyframeLevel(conv1, conv2, intr, p, D, B)
+        H, g, rbar, nvalid = ops.lm_keyframe_build(lv, R, T, W)
+        ctx.save_for_backward(conv1, conv2, D, B, R, T, W, intr, p)
+        ctx.exact_sym = bool(exact_sym)
+        ctx.mark_non_differentiable(nvalid)
+        return H, g, rbar, nvalid
+
+    @staticmethod
+    def backward(ctx, dH, dg, drbar, _dnvalid):
+        conv1, conv2, D, B, R, T, W, intr, p = ctx.saved_tensors
+        lv = ops.KeyframeLevel(conv1, conv2, intr, p, D, B)
+        nb, P = R.shape[0], 6 + B.shape[2]
+        dH = dH.contiguous() if dH is not None else torch.zeros(nb, P, P, device=conv1.device)
+        dg = dg if dg is not None else torch.zeros(nb, P, device=conv1.device)
+        drbar = drbar if drbar is not None else torch.zeros(nb, conv1.shape[2], device=conv1.device)
+        dconv1, dconv2, dD, dB, dR, dT, dW = ops.lm_keyframe_build_bwd(lv, R, T, W, dH, dg.contiguous(), drbar.contiguous(), ctx.exact_sym)
+        return dconv1, dconv2, dD, dB, dR, dT, dW.reshape(W.shape), None, None, None
+
+
 class _LMSolveUpdateFn(torch.autograd.Function):
     """(R', T', W') = banet_lm_solve_update(H, g, lambda, R, T, W); backward = banet_lm_solve_update_bwd."""
 
@@ -349,7 +375,13 @@ def window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_param
     for the build, the step and their backwards).  R [nw,nf,3,3], T [nw,nf,3,1], conv2 [nw,nf,h,w,3C] per frame, W [nw,K,1] per window; the
     keyframe tensors conv1, p, D, B (and intr) are [nw,nf,...] or [nw,1,...] (broadcast to the frames, their gradients summed over them).
     lambda per window: from the mean |residual| over its nf * N points through the MLP (times l2_regularizer_base), or lambda_override [nw].
+    Given WITHOUT a frame axis (conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K]; intr [nw,nf|1,4]), the keyframe tensors take the keyframe
+    build (banet_lm_keyframe_build / _bwd): nothing is copied per frame and their gradients come back as [nw,...]; precision must be AUTO or
+    FP32_SIMT there.
     Returns (R' [nw,nf,3,3], T' [nw,nf,3,1], W' [nw,K,1]) (, status [nw,nf])."""
+    if conv1.dim() == 3:
+        return _keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base, damping_eps, exact_sym,
+                                         lambda_override, precision, return_status)
     nw, nf = R.shape[0], R.shape[1]
     K = B.shape[-1]
     nb = nw * nf
@@ -359,6 +391,39 @@ def window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_param
     Wf = W.reshape(nw, 1, K, 1).expand(nw, nf, K, 1).reshape(nb, K, 1).contiguous()   # every pair builds with its window's W
     Rf, Tf = R.reshape(nb, 3, 3), T.reshape(nb, 3, 1)
     H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, Rf, Tf, Wf, intr.detach(), p.detach(), precision, exact_sym, grid)
+    if lambda_override is not None:
+        lam = lambda_override.reshape(nw)
+    else:
+        avg = (rbar_sum.reshape(nw, nf, C).sum(1) / float(nf * N)).unsqueeze(1)         # mean |residual| over each window's nf * N points
+        lam = torch.pow(torch.linalg.norm(avg, dim=-1, keepdim=True), 2.0 + lambda_mlp(avg, mlp_params)).reshape(nw)
+        if l2_regularizer_base is not None:
+            lam = l2_regularizer_base * lam
+    Rn, Tn, Wn, status = _WindowBatchSolveUpdateFn.apply(H, g, lam, Rf, Tf, W.reshape(nw, K, 1), damping_eps)
+    Rn, Tn, status = Rn.reshape(nw, nf, 3, 3), Tn.reshape(nw, nf, 3, 1), status.reshape(nw, nf)
+    if return_status:
+        return Rn, Tn, Wn, status
+    return Rn, Tn, Wn
+
+
+def _keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base, damping_eps, exact_sym, lambda_override,
+                              precision, return_status):
+    """window_batch_iteration_fused with the keyframe tensors once per window (conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K]): the
+    keyframe build (banet_lm_keyframe_build / _bwd) gives the window-reduced per-pair system, which the window step takes as it is.  Nothing
+    of the keyframe is copied per frame; its gradients come back as [nw,...]."""
+    from . import _lib
+    if precision not in (_lib.PREC_AUTO, _lib.PREC_FP32_SIMT):
+        raise _lib.BanetError(f"precision {precision}: the keyframe build is fp32 SIMT only (AUTO or FP32_SIMT)")
+    nw, nf = R.shape[0], R.shape[1]
+    K = B.shape[-1]
+    nb = nw * nf
+    for name, t, rank in (("p", p, 3), ("D", D, 3), ("B", B, 3)):
+        if t.dim() != rank or t.shape[0] != nw:
+            raise _lib.BanetError(f"{name}: the keyframe form takes [nw,...] tensors like conv1 [nw,N,C]; got {tuple(t.shape)}")
+    N, C = conv1.shape[1], conv1.shape[2]
+    intr = intr.expand(nw, nf, 4).reshape(nb, 4).contiguous()
+    conv2 = conv2.reshape(nb, *conv2.shape[2:])
+    Rf, Tf = R.reshape(nb, 3, 3), T.reshape(nb, 3, 1)
+    H, g, rbar_sum, _nvalid = _KeyframeBuildFn.apply(conv1, conv2, D, B, Rf, Tf, W.reshape(nw, K, 1), intr.detach(), p.detach(), exact_sym)
     if lambda_override is not None:
         lam = lambda_override.reshape(nw)
     else:

@@ -20,6 +20,7 @@ import torch
 
 from . import ops
 from . import autograd as _ag
+from . import _lib
 from ._lib import PREC_AUTO
 
 Tensor = torch.Tensor
@@ -179,6 +180,11 @@ class BundleNet(torch.nn.Module):
         ops.lm_window_batch_run."""
         nw, nf = R.shape[0], R.shape[1]
         intr = torch.stack([t.reshape(t.shape[0], t.shape[1], -1)[..., 0] for t in (fx, fy, ox, oy)], dim=-1).to(torch.float32)   # [nw,1|nf,4]
+        ranks = {t.dim() for t in (conv1, p, D, B)}
+        if len(ranks) != 1:
+            raise RuntimeError("WindowIteration: conv1, p, D, B must all carry a frame axis ([nw,1|nf,...]) or all come without one ([nw,...])")
+        if conv1.dim() == 3:
+            return self._keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, base, level)
         if self._wants_grad(conv1, conv2, D, B, R, T, W):
             if self.training_path == "reference_split":
                 raise RuntimeError("training_path='reference_split' has no torch-graph twin of the window solve; use training_path='fused'")
@@ -190,6 +196,26 @@ class BundleNet(torch.nn.Module):
         lv = ops.Level(pairs(conv1), pairs(conv2), pairs(intr), pairs(p), pairs(D), pairs(B))
         Rn, Tn, Wn, status = ops.lm_window_batch_run([lv], nw, 1, R.reshape(nw * nf, 3, 3), T.reshape(nw * nf, 3, 1), W,
                                                      mlp_packed=[self.mlp_packed(str(level))], l2_regularizer_base=base, precision=self.precision)
+        self._check_status(status.reshape(nw, nf))
+        return Rn.reshape(nw, nf, 3, 3), Tn.reshape(nw, nf, 3, 1), Wn
+
+    def _keyframe_batch_iteration(self, conv1, conv2, intr, p, D, B, R, T, W, base, level):
+        """WindowIteration on nw windows with the keyframe tensors once per window (conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K]):
+        the keyframe build (banet_lm_keyframe_*), fused autograd path when gradients are recorded, else one iteration of
+        ops.lm_keyframe_run.  fp32 SIMT only: a TF32 precision raises."""
+        if self.precision not in (_lib.PREC_AUTO, _lib.PREC_FP32_SIMT):
+            raise RuntimeError(f"precision {self.precision}: the keyframe form of WindowIteration has no tensor-core build; use AUTO or FP32_SIMT")
+        nw, nf = R.shape[0], R.shape[1]
+        if self._wants_grad(conv1, conv2, D, B, R, T, W):
+            if self.training_path == "reference_split":
+                raise RuntimeError("training_path='reference_split' has no torch-graph twin of the window solve; use training_path='fused'")
+            Rn, Tn, Wn, status = _ag.window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base,
+                                                                  exact_sym=self.exact_sym_grad, precision=self.precision, return_status=True)
+            self._check_status(status)
+            return Rn, Tn, Wn
+        lv = ops.KeyframeLevel(conv1, conv2.reshape(nw * nf, *conv2.shape[2:]), intr.expand(nw, nf, 4).reshape(nw * nf, 4), p, D, B)
+        Rn, Tn, Wn, status = ops.lm_keyframe_run([lv], 1, R.reshape(nw * nf, 3, 3), T.reshape(nw * nf, 3, 1), W,
+                                                 mlp_packed=[self.mlp_packed(str(level))], l2_regularizer_base=base, precision=self.precision)
         self._check_status(status.reshape(nw, nf))
         return Rn.reshape(nw, nf, 3, 3), Tn.reshape(nw, nf, 3, 1), Wn
 

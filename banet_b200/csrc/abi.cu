@@ -535,6 +535,161 @@ extern "C" int banet_lm_window_batch_solve_update_bwd(const float* H, const floa
     return lm_window_batch_step_bwd(H, g, lambda, delta, nw, nf, K, *opts, R, T, dR_out, dT_out, dW_out, dH, dg, dlambda, dR, dT, dW, ws, (cudaStream_t)stream);
 }
 
+// ---- keyframe-layout window batches (section 3e): the keyframe tensors once per window ------------------------------------------------
+namespace {
+int check_keyframe_level(const banet_keyframe_level_t* lv, const char* who)
+{
+    BANET_REQUIRE(lv, BANET_ERR_BAD_ARG, "%s: null level", who);
+    BANET_REQUIRE(lv->nw > 0 && lv->nf > 0 && lv->N > 0 && lv->C > 0 && lv->K > 0 && lv->h >= 2 && lv->w >= 2, BANET_ERR_BAD_ARG,
+                  "%s: bad shape nw=%d nf=%d N=%d C=%d K=%d h=%d w=%d", who, lv->nw, lv->nf, lv->N, lv->C, lv->K, lv->h, lv->w);
+    BANET_REQUIRE(lv->conv2_channels == 3 * lv->C || lv->conv2_channels == lv->C, BANET_ERR_BAD_ARG,
+                  "%s: conv2_channels=%d must be 3*C (reference layout) or C (F2 only)", who, lv->conv2_channels);
+    BANET_REQUIRE(lv->conv1 && lv->p && lv->D && lv->B && lv->conv2 && lv->intr, BANET_ERR_BAD_ARG, "%s: null tensor", who);
+    BANET_REQUIRE((long long)lv->h * lv->w * lv->conv2_channels < (1LL << 40), BANET_ERR_BAD_ARG, "%s: map too large", who);
+    BANET_REQUIRE(lv->K <= 256, BANET_ERR_UNSUPPORTED, "%s: K=%d > 256 not supported", who, lv->K);
+    BANET_REQUIRE(lv->C <= 2048, BANET_ERR_UNSUPPORTED, "%s: C=%d > 2048 not supported", who, lv->C);
+    return BANET_OK;
+}
+
+// The keyframe build is fp32 SIMT only: AUTO resolves to it (as AUTO does wherever the tensor cores do not apply); the TF32 modes have no
+// keyframe kernel.
+int check_keyframe_precision(int precision, const char* who)
+{
+    BANET_REQUIRE(precision == BANET_PREC_AUTO || precision == BANET_PREC_FP32_SIMT || precision == BANET_PREC_TF32X1 || precision == BANET_PREC_TF32X2 ||
+                  precision == BANET_PREC_TF32X3 || precision == BANET_PREC_TF32_LEVELWISE, BANET_ERR_BAD_ARG, "%s: unknown precision mode %d", who, precision);
+    BANET_REQUIRE(precision == BANET_PREC_AUTO || precision == BANET_PREC_FP32_SIMT, BANET_ERR_UNSUPPORTED,
+                  "%s: precision mode %d (tensor cores) has no keyframe build; use AUTO or FP32_SIMT", who, precision);
+    return BANET_OK;
+}
+
+struct KeyCarve { size_t build, H, g, rbar, nvalid, lambda, delta, step, total; };
+int key_carve(const banet_keyframe_level_t* levels, int nlevels, KeyCarve* c)
+{
+    size_t build = 0; int maxC = 0;
+    const int nw = levels[0].nw, nf = levels[0].nf, K = levels[0].K, P = 6 + K;
+    const size_t nb = (size_t)nw * nf;
+    for (int l = 0; l < nlevels; ++l) {
+        KeyframePlan plan;
+        int rc = keyframe_plan(&levels[l], num_sms(), &plan);
+        if (rc) return rc;
+        if (plan.ws_bytes > build) build = plan.ws_bytes;
+        if (levels[l].C > maxC) maxC = levels[l].C;
+    }
+    size_t off = 0;
+    c->build = off;  off += align_up(build, 256);
+    c->H = off;      off += align_up(nb * P * P * 4, 256);
+    c->g = off;      off += align_up(nb * P * 4, 256);
+    c->rbar = off;   off += align_up(nb * maxC * 4, 256);
+    c->nvalid = off; off += align_up(nb * 4, 256);
+    c->lambda = off; off += align_up((size_t)nw * 4, 256);
+    c->delta = off;  off += align_up((size_t)nw * (6 * nf + K) * 4, 256);
+    c->step = off;   off += lm_window_batch_ws_bytes(nw, nf);
+    c->total = off;
+    return BANET_OK;
+}
+}  // namespace
+
+extern "C" size_t banet_lm_keyframe_build_workspace_bytes(const banet_keyframe_level_t* lv)
+{
+    if (check_keyframe_level(lv, "lm_keyframe_build")) return 0;
+    KeyframePlan plan;
+    if (keyframe_plan(lv, num_sms(), &plan) != BANET_OK) return 0;
+    return plan.ws_bytes;
+}
+
+extern "C" int banet_lm_keyframe_build(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W,
+                                       float* H, float* g, float* rbar_sum, float* nvalid, void* ws, size_t ws_bytes, banet_stream_t stream)
+{
+    int rc = check_keyframe_level(lv, "lm_keyframe_build");
+    if (rc) return rc;
+    BANET_REQUIRE(R && T && W && H && g && rbar_sum && nvalid, BANET_ERR_BAD_ARG, "lm_keyframe_build: null pointer");
+    KeyframePlan plan;
+    rc = keyframe_plan(lv, num_sms(), &plan);
+    if (rc) return rc;
+    BANET_REQUIRE(ws && ws_bytes >= plan.ws_bytes, BANET_ERR_WORKSPACE, "lm_keyframe_build: workspace %zu < %zu bytes", ws_bytes, plan.ws_bytes);
+    return keyframe_build(lv, plan, R, T, W, H, g, rbar_sum, nvalid, ws, (cudaStream_t)stream);
+}
+
+extern "C" int banet_lm_keyframe_build_bwd(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W,
+                                           const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
+                                           float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, banet_stream_t stream)
+{
+    int rc = check_keyframe_level(lv, "lm_keyframe_build_bwd");
+    if (rc) return rc;
+    BANET_REQUIRE(R && T && W && dH && dg && drbar_sum && dconv1 && dconv2 && dD && dB && dR && dT && dW, BANET_ERR_BAD_ARG,
+                  "lm_keyframe_build_bwd: null pointer");
+    BANET_REQUIRE(lv->conv2_channels == 3 * lv->C, BANET_ERR_UNSUPPORTED, "lm_keyframe_build_bwd: conv2 must be the [F2|gx|gy] (3C) layout");
+    BANET_REQUIRE(keyframe_build_bwd_supported(lv->nf, lv->K, lv->C), BANET_ERR_UNSUPPORTED,
+                  "lm_keyframe_build_bwd: K=%d, C=%d do not fit shared memory", lv->K, lv->C);
+    return keyframe_build_bwd(lv, R, T, W, dH, dg, drbar_sum, exact_sym, dconv1, dconv2, dD, dB, dR, dT, dW, (cudaStream_t)stream);
+}
+
+extern "C" size_t banet_lm_keyframe_run_workspace_bytes(const banet_keyframe_level_t* levels, int nlevels, int precision)
+{
+    if (!levels || nlevels <= 0 || check_keyframe_precision(precision, "lm_keyframe_run")) return 0;
+    for (int l = 0; l < nlevels; ++l)
+        if (check_keyframe_level(&levels[l], "lm_keyframe_run") || levels[l].nw != levels[0].nw || levels[l].nf != levels[0].nf ||
+            levels[l].K != levels[0].K) return 0;
+    KeyCarve c;
+    if (key_carve(levels, nlevels, &c) != BANET_OK) return 0;
+    return c.total;
+}
+
+extern "C" int banet_lm_keyframe_run(const banet_keyframe_level_t* levels, int nlevels, int iters_per_level,
+                                     const float* const* mlp_weights, float l2_regularizer_base, float lambda_fixed,
+                                     const banet_solve_opts_t* opts, int precision,
+                                     float* R, float* T, float* W, int32_t* status, void* ws, size_t ws_bytes, banet_stream_t stream)
+{
+    BANET_REQUIRE(levels && opts && R && T && W && status, BANET_ERR_BAD_ARG, "lm_keyframe_run: null pointer");
+    BANET_REQUIRE(nlevels > 0 && iters_per_level > 0, BANET_ERR_BAD_ARG, "lm_keyframe_run: bad argument nlevels=%d iters=%d", nlevels, iters_per_level);
+    BANET_REQUIRE(!opts->vmatrix_batch_scramble, BANET_ERR_BAD_ARG, "lm_keyframe_run: needs vmatrix_batch_scramble = 0");
+    const int nw = levels[0].nw, nf = levels[0].nf, K = levels[0].K;
+    for (int l = 0; l < nlevels; ++l) {
+        int rc = check_keyframe_level(&levels[l], "lm_keyframe_run");
+        if (rc) return rc;
+        BANET_REQUIRE(levels[l].nw == nw && levels[l].nf == nf && levels[l].K == K, BANET_ERR_BAD_ARG, "lm_keyframe_run: nw/nf/K must agree across levels");
+        BANET_REQUIRE((mlp_weights && mlp_weights[l]) || lambda_fixed >= 0.f, BANET_ERR_BAD_ARG,
+                      "lm_keyframe_run: level %d has no lambda-MLP weights and lambda_fixed < 0", l);
+        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
+        BANET_REQUIRE(lm_window_batch_supported(K, use_mlp ? levels[l].C : 0), BANET_ERR_UNSUPPORTED,
+                      "lm_keyframe_run: K=%d (C=%d) does not fit the window step", K, levels[l].C);
+    }
+    int rc = check_keyframe_precision(precision, "lm_keyframe_run");
+    if (rc) return rc;
+    KeyCarve c;
+    rc = key_carve(levels, nlevels, &c);
+    if (rc) return rc;
+    BANET_REQUIRE(ws && ws_bytes >= c.total, BANET_ERR_WORKSPACE, "lm_keyframe_run: workspace %zu < %zu bytes", ws_bytes, c.total);
+    cudaStream_t st = (cudaStream_t)stream;
+    char* base = reinterpret_cast<char*>(ws);
+    float* H = reinterpret_cast<float*>(base + c.H);
+    float* g = reinterpret_cast<float*>(base + c.g);
+    float* rbar = reinterpret_cast<float*>(base + c.rbar);
+    float* nvalid = reinterpret_cast<float*>(base + c.nvalid);
+    float* lam = reinterpret_cast<float*>(base + c.lambda);
+    float* delta = reinterpret_cast<float*>(base + c.delta);
+    const int nb = nw * nf;
+    zero_status_kernel<<<(nb + 255) / 256, 256, 0, st>>>(status, nb);
+    for (int l = 0; l < nlevels; ++l) {
+        const banet_keyframe_level_t* lv = &levels[l];
+        KeyframePlan plan;
+        rc = keyframe_plan(lv, num_sms(), &plan);
+        if (rc) return rc;
+        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
+        if (!use_mlp) fill_kernel<<<(nw + 255) / 256, 256, 0, st>>>(lam, nw, lambda_fixed);
+        for (int it = 0; it < iters_per_level; ++it) {                // one build launch and one step launch per iteration
+            rc = keyframe_build(lv, plan, R, T, W, H, g, rbar, nvalid, base + c.build, st);
+            if (rc) return rc;
+            rc = lm_window_batch_step(H, g, rbar, nw, nf, lv->N, lv->C, K, use_mlp ? mlp_weights[l] : nullptr, l2_regularizer_base,
+                                      use_mlp ? nullptr : lam, *opts, R, T, W, R, T, W, nullptr, delta, use_mlp ? lam : nullptr, status, 1,
+                                      base + c.step, st);
+            if (rc) return rc;
+        }
+    }
+    BANET_CUDA_LAUNCH_CHECK("lm_keyframe_run");
+    return BANET_OK;
+}
+
 extern "C" size_t banet_lm_track_legacy_workspace_bytes(const banet_level_t* levels, int nlevels)
 {
     if (!levels || nlevels <= 0) return 0;

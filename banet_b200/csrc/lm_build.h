@@ -94,6 +94,21 @@ int lm_window_batch_step_bwd(const float* H, const float* g, const float* lambda
                              const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
                              float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, void* ws, cudaStream_t st);
 
+// keyframe-layout window batches (lm_window_key.cu): the keyframe tensors once per window, the window-reduced per-pair system (ABI 3e)
+struct KeyframePlan {
+    int KP, grid, max_span, tiles_per_win;
+    size_t slot_floats;
+    long long total_tiles;
+    size_t ws_bytes;
+};
+int keyframe_plan(const banet_keyframe_level_t* lv, int num_sms, KeyframePlan* plan);
+int keyframe_build(const banet_keyframe_level_t* lv, const KeyframePlan& plan, const float* R, const float* T, const float* W,
+                   float* H, float* g, float* rbar_sum, float* nvalid, void* ws, cudaStream_t st);
+bool keyframe_build_bwd_supported(int nf, int K, int C);
+int keyframe_build_bwd(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W, const float* dH, const float* dg,
+                       const float* drbar, int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
+                       cudaStream_t st);
+
 // legacy pose-only tracker loop with device-side accept / reject and early termination (lm_legacy.cu)
 size_t lm_track_legacy_workspace_bytes(const banet_level_t* levels, int nlevels);
 int lm_track_legacy(const banet_level_t* levels, int nlevels, const int* level_iters, const float* const* mlp_weights, const banet_legacy_opts_t& o,

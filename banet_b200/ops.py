@@ -389,6 +389,102 @@ def lm_window_batch_solve_update(H: Tensor, g: Tensor, lam: Tensor, R: Tensor, T
     return Ro, To, Wo, delta, status
 
 
+@dataclass
+class KeyframeLevel:
+    """One pyramid level of nw keyframe windows with the keyframe tensors given once per window (banet_keyframe_level in
+    include/banet_abi.h).  Pair w * nf + f is (keyframe of window w -> frame f)."""
+    conv1: Tensor             # [nw,N,C]
+    conv2: Tensor             # [nw*nf,h,w,3C]  ([nw*nf,h,w,C]: F2 only, forward only)
+    intr: Tensor              # [nw*nf,4]
+    p: Tensor                 # [nw,3,N]
+    D: Tensor                 # [nw,N,1]
+    B: Tensor                 # [nw,N,K]
+
+    def as_struct(self) -> Tuple[_lib.BanetKeyframeLevel, list]:
+        conv1 = _chk(self.conv1, "conv1"); nw, N, Cc = conv1.shape
+        conv2 = _chk(self.conv2, "conv2"); nb, h, w, c2 = conv2.shape
+        if nb % nw:
+            raise _lib.BanetError(f"conv2 has {nb} pairs, which is not a multiple of the {nw} windows")
+        nf = nb // nw
+        B = _chk(self.B, "B"); K = B.shape[2]
+        _chk(B, "B", (nw, N, K))
+        intr = _chk(self.intr, "intr", (nb, 4)); p = _chk(self.p, "p", (nw, 3, N)); D = _chk(self.D, "D", (nw, N, 1))
+        keep = [conv1, conv2, intr, p, D, B]
+        return _lib.BanetKeyframeLevel(nw, nf, N, Cc, K, h, w, c2, conv1.data_ptr(), p.data_ptr(), D.data_ptr(), B.data_ptr(),
+                                       conv2.data_ptr(), intr.data_ptr()), keep
+
+
+def lm_keyframe_build(level: KeyframeLevel, R: Tensor, T: Tensor, W: Tensor):
+    """The keyframe build (banet_lm_keyframe_build): R [nw*nf,3,3], T [nw*nf,3,1], W [nw,K,1] -> the window-reduced per-pair system
+    H [nw*nf,P,P], g [nw*nf,P], rbar_sum [nw*nf,C], nvalid [nw*nf]: banet_lm_build's per-pair values except that frame 0's depth block holds
+    the window's whole depth block and the other frames' depth blocks are zero."""
+    lib = load()
+    st, keep = level.as_struct()
+    nw, nb, K, Cc = st.nw, st.nw * st.nf, st.K, st.C
+    P = 6 + K
+    R = _chk(R, "R", (nb, 3, 3)); T = _chk(T, "T", (nb, 3, 1)); Wt = _chk(W.reshape(nw, K, 1), "W", (nw, K, 1))
+    dev = R.device
+    H = torch.empty(nb, P, P, device=dev); g = torch.empty(nb, P, device=dev)
+    rbar = torch.empty(nb, Cc, device=dev); nvalid = torch.empty(nb, device=dev)
+    nbytes = lib.banet_lm_keyframe_build_workspace_bytes(C.byref(st))
+    ws = _ws(nbytes, dev)
+    check(lib.banet_lm_keyframe_build(C.byref(st), R.data_ptr(), T.data_ptr(), Wt.data_ptr(), H.data_ptr(), g.data_ptr(), rbar.data_ptr(),
+                                      nvalid.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "banet_lm_keyframe_build")
+    return H, g, rbar, nvalid
+
+
+def lm_keyframe_build_bwd(level: KeyframeLevel, R: Tensor, T: Tensor, W: Tensor, dH: Tensor, dg: Tensor, drbar_sum: Tensor,
+                          exact_sym: bool = False):
+    """Backward of lm_keyframe_build (banet_lm_keyframe_build_bwd) -> dconv1 [nw,N,C], dconv2 [nw*nf,h,w,3C], dD [nw,N,1], dB [nw,N,K],
+    dR, dT [nw*nf,...], dW [nw,K,1].  Only frame 0's depth block of dH is read."""
+    lib = load()
+    st, keep = level.as_struct()
+    nw, nb, K, Cc, N = st.nw, st.nw * st.nf, st.K, st.C, st.N
+    P = 6 + K
+    R = _chk(R, "R", (nb, 3, 3)); T = _chk(T, "T", (nb, 3, 1)); Wt = _chk(W.reshape(nw, K, 1), "W", (nw, K, 1))
+    dH = _chk(dH, "dH", (nb, P, P)); dg = _chk(dg.reshape(nb, P), "dg", (nb, P)); dr = _chk(drbar_sum, "drbar_sum", (nb, Cc))
+    dev = R.device
+    dconv1 = torch.empty(nw, N, Cc, device=dev); dconv2 = torch.empty(nb, st.h, st.w, 3 * Cc, device=dev)
+    dD = torch.empty(nw, N, 1, device=dev); dB = torch.empty(nw, N, K, device=dev)
+    dR = torch.empty(nb, 3, 3, device=dev); dT = torch.empty(nb, 3, 1, device=dev); dW = torch.empty(nw, K, 1, device=dev)
+    check(lib.banet_lm_keyframe_build_bwd(C.byref(st), R.data_ptr(), T.data_ptr(), Wt.data_ptr(), dH.data_ptr(), dg.data_ptr(), dr.data_ptr(),
+                                          int(bool(exact_sym)), dconv1.data_ptr(), dconv2.data_ptr(), dD.data_ptr(), dB.data_ptr(), dR.data_ptr(),
+                                          dT.data_ptr(), dW.data_ptr(), _stream()), "banet_lm_keyframe_build_bwd")
+    return dconv1, dconv2, dD, dB, dR, dT, dW
+
+
+def lm_keyframe_run(levels: Sequence[KeyframeLevel], iters_per_level: int, R: Tensor, T: Tensor, W: Tensor,
+                    mlp_packed: Optional[Sequence[Optional[Tensor]]] = None, l2_regularizer_base: float = 1000.0,
+                    lambda_fixed: float = -1.0, damping_eps: float = 1e-5, undamped_last: bool = True,
+                    precision: int = _lib.PREC_AUTO, workspace: Optional[Tensor] = None):
+    """Joint coarse-to-fine solve of nw keyframe windows with the keyframe tensors once per window (banet_lm_keyframe_run): per iteration
+    one keyframe build and one window step.  R [nw*nf,3,3], T [nw*nf,3,1], W [nw,K,1].  Returns new (R, T, W [nw,K,1], status [nw*nf])."""
+    lib = load()
+    structs, keep = [], []
+    for lv in levels:
+        s, k = lv.as_struct(); structs.append(s); keep.append(k)
+    arr = (_lib.BanetKeyframeLevel * len(structs))(*structs)
+    nw, nb, K = structs[0].nw, structs[0].nw * structs[0].nf, structs[0].K
+    mlp_ptrs = (C.c_void_p * len(structs))()
+    have = False
+    for i in range(len(structs)):
+        m = None if mlp_packed is None else mlp_packed[i]
+        if m is not None:
+            m = _chk(m, "mlp_packed"); keep.append(m); have = True
+            if m.numel() != lib.banet_mlp_param_count(structs[i].C):
+                raise _lib.BanetError("mlp_packed size mismatch")
+        mlp_ptrs[i] = None if m is None else m.data_ptr()
+    opts = BanetSolveOpts(float(damping_eps), int(undamped_last), 0)
+    nbytes = lib.banet_lm_keyframe_run_workspace_bytes(arr, len(structs), int(precision))
+    R = _chk(R, "R", (nb, 3, 3)).clone(); T = _chk(T, "T", (nb, 3, 1)).clone(); Wt = _chk(W.reshape(nw, K, 1), "W", (nw, K, 1)).clone()
+    ws = workspace if workspace is not None and workspace.numel() >= nbytes else _ws(nbytes, R.device)
+    status = torch.empty(nb, device=R.device, dtype=torch.int32)
+    check(lib.banet_lm_keyframe_run(arr, len(structs), int(iters_per_level), mlp_ptrs if have else None, float(l2_regularizer_base), float(lambda_fixed),
+                                    C.byref(opts), int(precision), R.data_ptr(), T.data_ptr(), Wt.data_ptr(), status.data_ptr(), ws.data_ptr(),
+                                    ws.numel(), _stream()), "banet_lm_keyframe_run")
+    return R, T, Wt, status
+
+
 class LMRunGraph:
     """`banet_lm_run` captured ONCE into a CUDA graph and replayed: the library call allocates nothing and never synchronises, so the whole
     coarse-to-fine loop (3 launches per LM iteration) is capturable as it is.  For small or sparse problems (the reference's 4096-point

@@ -300,6 +300,62 @@ int    banet_lm_window_batch_solve_update_bwd(const float* H, const float* g, co
                                               void* ws, size_t ws_bytes, banet_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * (3e) Keyframe-layout window batches — (3d)'s windows with the keyframe tensors given ONCE per window instead of once per frame.  Every
+ *      frame of window w samples the same keyframe points with the same depth D + B.W_w, so the build contracts the basis once per window:
+ *        sum_f H_dd,f = B^T diag(sum_f s_f) B,   [H_cd,f | g_d,f]^T = B^T [v_f | t_f]   (s_f = jd^T M_f jd per point)
+ *      one contraction against K + 7 nf columns where (3d)'s per-pair build does nf contractions against K + 7 (fp32 SIMT arithmetic).
+ *      Output, the WINDOW-REDUCED per-pair system: H [nw*nf,P,P], g [nw*nf,P], rbar_sum [nw*nf,C], nvalid [nw*nf] hold banet_lm_build's
+ *      per-pair values (H_cc,f, H_cd,f and its mirror, g_f, rbar_f, nvalid_f) except the depth blocks: frame 0's holds the window's whole
+ *      depth block sum_f H_dd,f, every other frame's is exactly zero.  H stays exactly symmetric.  The window steps ((3c) and (3d)) only
+ *      sum the depth blocks over the frames, so banet_lm_window_batch_solve_update(_bwd) and banet_lm_window_solve_update(_bwd) take this
+ *      layout unchanged (the same step as the replicated layout, to fp32 rounding).
+ *      Conventions of (3d): pair w*nf + f = (keyframe of window w -> frame f); R, T, status per pair; W [nw,K,1] and lambda [nw] per window.
+ *      Every sum of the forward is taken in a fixed order (partial slots reduced in fp64): bit-reproducible, independent of the workspace.
+ *      Argument errors, reported before any CUDA call: null pointers, nw, nf, N, C, K <= 0, h or w < 2, conv2_channels not 3C or C,
+ *      vmatrix_batch_scramble != 0: BANET_ERR_BAD_ARG; K > 256, C > 2048, the F2-only layout in the backward, a TF32 precision in the run:
+ *      BANET_ERR_UNSUPPORTED; workspace too small: BANET_ERR_WORKSPACE.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct banet_keyframe_level {
+    int nw, nf, N, C, K;      /* windows, frames per window, keyframe points, feature channels, depth bases (K >= 1) */
+    int h, w;                 /* conv2 map size at this level */
+    int conv2_channels;       /* 3*C: [F2|gx|gy]; C: F2 only (forward only) */
+    const float* conv1;       /* [nw,N,C]      the keyframe's features, once per window */
+    const float* p;           /* [nw,3,N]      its rays */
+    const float* D;           /* [nw,N,1]      its depth */
+    const float* B;           /* [nw,N,K]      its depth basis */
+    const float* conv2;       /* [nw*nf,h,w,conv2_channels]  per pair */
+    const float* intr;        /* [nw*nf,4]     per pair */
+} banet_keyframe_level_t;
+
+/* The keyframe build: R [nw*nf,3,3], T [nw*nf,3,1], W [nw,K,1] (read directly, one row per window) -> the window-reduced H, g, rbar_sum,
+ * nvalid above. */
+size_t banet_lm_keyframe_build_workspace_bytes(const banet_keyframe_level_t* lv);
+int    banet_lm_keyframe_build(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W,
+                               float* H, float* g, float* rbar_sum, float* nvalid, void* ws, size_t ws_bytes, banet_stream_t stream);
+/* Its backward: dH [nw*nf,P,P] (not symmetric, as the window steps' backward emits it), dg [nw*nf,P], drbar_sum [nw*nf,C] ->
+ * dconv1 [nw,N,C], dconv2 [nw*nf,h,w,3C], dD [nw,N,1], dB [nw,N,K], dR [nw*nf,3,3], dT [nw*nf,3,1], dW [nw,K,1]; every output is
+ * overwritten.  Only frame 0's depth block of dH is read (S_dd by exact_sym as in banet_lm_build_bwd): the other frames' depth blocks are
+ * constants (zero) in the forward, so this is the exact adjoint of the forward; the window steps' backward writes the same depth-block
+ * gradient into every frame, and the others are ignored.  dconv1, dD, dB are summed over the frames in a fixed order and stored once
+ * (bit-reproducible); dconv2, dR, dT, dW are accumulated with atomics.  conv2 must be the 3C layout.  The window's S_dd lives in shared
+ * memory with at least one frame's blocks: K*K + 14 K + 17 C + 250 floats must fit 220 KB (K <= 225 at C = 128), else BANET_ERR_UNSUPPORTED;
+ * more frames than fit are walked in chunks.  No workspace. */
+int    banet_lm_keyframe_build_bwd(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W,
+                                   const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
+                                   float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
+                                   banet_stream_t stream);
+/* Whole coarse-to-fine solve (banet_lm_window_batch_run with keyframe levels): each iteration is one keyframe-build launch (plus its fp64
+ * slot reduction) and one window-step launch, the lambda-MLP or lambda_fixed as in (3d).  W [nw,K,1] is read by the build directly (no
+ * per-pair copies).  levels[l].nw, nf, K must agree across levels.  precision: BANET_PREC_AUTO or BANET_PREC_FP32_SIMT (AUTO resolves to
+ * FP32_SIMT: there is no tensor-core keyframe build); the TF32 modes are rejected with BANET_ERR_UNSUPPORTED. */
+size_t banet_lm_keyframe_run_workspace_bytes(const banet_keyframe_level_t* levels, int nlevels, int precision);
+int    banet_lm_keyframe_run(const banet_keyframe_level_t* levels, int nlevels, int iters_per_level,
+                             const float* const* mlp_weights, float l2_regularizer_base, float lambda_fixed,
+                             const banet_solve_opts_t* opts, int precision,
+                             float* R, float* T, float* W, int32_t* status,
+                             void* ws, size_t ws_bytes, banet_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * (4) The legacy pose-only keyframe tracker loop: legacy/ba.py:83-145 (`Tracker.trackTF`) with CameraIteration (:147-214) or, with
  *     early termination, CameraIteration2 (:226-345: lambda-MLP step, residual re-evaluated at the updated pose, step kept only if it
  *     decreased) — accept / reject and the per-level termination test run on the device, per pair, without host synchronisation.
