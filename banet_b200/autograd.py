@@ -85,8 +85,11 @@ def lambda_mlp(avg_residual: Tensor, params: Sequence[Tuple[Tensor, Tensor]]) ->
 def iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base: Optional[float],
               damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None):
     """One differentiable LM iteration.  B/W None -> CameraIteration (bundlenet.py:122-191), else BundleIteration (:193-278).
-    intr [nb,4].  Returns (R', T', W')."""
+    intr [nb,4]; conv2 [nb,h,w,3C] = [F2|gx|gy], or [nb,h,w,C] (F2 only: [F2|gx|gy] is built here with the differentiable
+    grad_fixed_concat, so the gradient reaches F2).  Returns (R', T', W')."""
     nb, N, C = conv1.shape
+    if conv2.shape[-1] == C:
+        conv2 = grad_fixed_concat(conv2)
     h, w = conv2.shape[1], conv2.shape[2]
     fx, fy, ox, oy = [intr[:, i:i + 1] for i in range(4)]
     bundle = B is not None
@@ -134,7 +137,8 @@ def iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_b
 
 # ------------------------------------------------------------------------------------------ fused path
 class _LMBuildFn(torch.autograd.Function):
-    """(H, g, rbar_sum) = banet_lm_build(...); backward = banet_lm_build_bwd.  conv2 is the [F2|gx|gy] tensor."""
+    """(H, g, rbar_sum) = banet_lm_build(...); backward = banet_lm_build_bwd.  conv2 is the [F2|gx|gy] tensor or F2 only; dconv2 comes back
+    in conv2's layout."""
 
     @staticmethod
     def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, precision, exact_sym, grid):
@@ -318,7 +322,8 @@ def depth_compose(init_depth: Tensor, basis: Tensor, W: Tensor) -> Tensor:
 def iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base: Optional[float],
                     damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None,
                     precision: int = 0, grid=None, return_status: bool = False):
-    """One differentiable LM iteration on the fused kernels.  Same arguments / returns as `iteration`.
+    """One differentiable LM iteration on the fused kernels.  Same arguments / returns as `iteration`; an F2-only conv2 [nb,h,w,C] goes
+    straight into the build and its backward (the gradient stencil's adjoint runs inside banet_lm_build_bwd).
     precision: contraction mode of the FORWARD build (the backward is fp32); default FP32_SIMT, the reference's arithmetic type."""
     nb, N, C = conv1.shape
     bundle = B is not None
@@ -344,7 +349,7 @@ def window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_
                            damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None,
                            precision: int = 0, grid=None, return_status: bool = False):
     """One differentiable LM iteration of a keyframe window (the joint solve of ops.lm_window_run) on the fused kernels: nf pairs
-    (keyframe -> frame f) share W [K,1]; R [nf,3,3], T [nf,3,1] and conv2 [nf,h,w,3C] are per frame.  The keyframe tensors conv1, p, D, B
+    (keyframe -> frame f) share W [K,1]; R [nf,3,3], T [nf,3,1] and conv2 [nf,h,w,3C] (or [nf,h,w,C], F2 only) are per frame.  The keyframe tensors conv1, p, D, B
     (and intr) may be given once ([1,...]): they are broadcast to the frames and their gradients summed over them.  lambda: from the mean
     |residual| over all points of all frames through the MLP (times l2_regularizer_base), or lambda_override [1].
     Returns (R', T', W' [K,1]) (, status [nf])."""
@@ -372,12 +377,12 @@ def window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_param
                                  damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None,
                                  precision: int = 0, grid=None, return_status: bool = False):
     """One differentiable LM iteration of a batch of nw keyframe windows of nf frames (window_iteration_fused per window, one launch each
-    for the build, the step and their backwards).  R [nw,nf,3,3], T [nw,nf,3,1], conv2 [nw,nf,h,w,3C] per frame, W [nw,K,1] per window; the
-    keyframe tensors conv1, p, D, B (and intr) are [nw,nf,...] or [nw,1,...] (broadcast to the frames, their gradients summed over them).
+    for the build, the step and their backwards).  R [nw,nf,3,3], T [nw,nf,3,1], conv2 [nw,nf,h,w,3C] (or [nw,nf,h,w,C], F2 only) per frame,
+    W [nw,K,1] per window; the keyframe tensors conv1, p, D, B (and intr) are [nw,nf,...] or [nw,1,...] (broadcast to the frames, their gradients summed over them).
     lambda per window: from the mean |residual| over its nf * N points through the MLP (times l2_regularizer_base), or lambda_override [nw].
     Given WITHOUT a frame axis (conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K]; intr [nw,nf|1,4]), the keyframe tensors take the keyframe
     build (banet_lm_keyframe_build / _bwd): nothing is copied per frame and their gradients come back as [nw,...]; precision must be AUTO or
-    FP32_SIMT there.
+    FP32_SIMT there, and conv2 must be [F2|gx|gy] when it requires grad (the keyframe backward takes that layout only).
     Returns (R' [nw,nf,3,3], T' [nw,nf,3,1], W' [nw,K,1]) (, status [nw,nf])."""
     if conv1.dim() == 3:
         return _keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base, damping_eps, exact_sym,

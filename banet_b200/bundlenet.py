@@ -149,10 +149,10 @@ class BundleNet(torch.nn.Module):
 
     def WindowIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, l2_regularizer_base=None, level=None):
         """One joint LM iteration of a keyframe window (an extension; the reference's layer is 2-view): the nf pairs (keyframe -> frame f)
-        share the keyframe depth D + B.W.  Arguments as BundleIteration with R [nf,3,3], T [nf,3,1], conv2 [nf,h,w,3C] per frame and
+        share the keyframe depth D + B.W.  Arguments as BundleIteration with R [nf,3,3], T [nf,3,1], conv2 [nf,h,w,3C] (or F2 only, [nf,h,w,C]) per frame and
         W [K,1] shared; the keyframe tensors conv1, p, D, B may be given once ([1,...]) or per frame.  -> (updatedR, updatedT, updatedW [K,1]).
         Differentiable (banet_lm_window_solve_update_bwd) whenever gradients are being recorded; there is no reference_split twin.
-        A batch of nw windows: R [nw,nf,3,3], T [nw,nf,3,1], conv2 [nw,nf,h,w,3C], W [nw,K,1], keyframe tensors and fx, fy, ox, oy
+        A batch of nw windows: R [nw,nf,3,3], T [nw,nf,3,1], conv2 [nw,nf,h,w,3C] (or [nw,nf,h,w,C]), W [nw,K,1], keyframe tensors and fx, fy, ox, oy
         [nw,1,...] or [nw,nf,...] -> ([nw,nf,3,3], [nw,nf,3,1], [nw,K,1]), last_status [nw,nf] (banet_lm_window_batch_*)."""
         base = 1.0 if l2_regularizer_base is None else float(l2_regularizer_base)
         if self.vmatrix_batch_scramble:

@@ -37,14 +37,59 @@ struct BwdParams {
 };
 
 __device__ __forceinline__ float sgnf(float v) { return v > 0.f ? 1.f : (v < 0.f ? -1.f : 0.f); }
+__device__ __forceinline__ int reflect1(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }     // tf.pad REFLECT by one
+
+// conv2 layouts of the build backward.  F2-only: the gradient channels are the forward's on-the-fly stencil at each tap,
+//   gx_tau = 1/2 (F[y, rho(x+1)] - F[y, rho(x-1)]),  gy_tau = 1/2 (F[rho(y+1), x] - F[rho(y-1), x]),
+// so its adjoint scatters w_tau df into the tap and +-1/2 w_tau dgx, +-1/2 w_tau dgy into the tap's four stencil neighbours (20 addresses;
+// the atomics keep texels that the reflect and the clamp make coincide correct).  Summing an interior point's 20 contributions into its 12
+// distinct texels first (12 atomics) was slower on an H100 at every measured size (DESIGN.md §4), so every point takes the plain scatter.
+constexpr int BWD_3C = 0, BWD_F2 = 1;
+
+// Pixel coordinates of the four taps (bit 0: x0 / x1, bit 1: y0 / y1) and of their stencil neighbours in an F2-only map.
+struct FlyTaps {
+    int cx[2], ex[2], wx[2], cy[2], sy[2], ny[2];
+    __device__ __forceinline__ FlyTaps(int x0, int x1, int y0, int y1, int h, int w) {
+        cx[0] = x0; cx[1] = x1; cy[0] = y0; cy[1] = y1;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            ex[i] = reflect1(cx[i] + 1, w); wx[i] = reflect1(cx[i] - 1, w);
+            sy[i] = reflect1(cy[i] + 1, h); ny[i] = reflect1(cy[i] - 1, h);
+        }
+    }
+    // channel c of the tap values t, the tap x-gradients g and y-gradients k
+    __device__ __forceinline__ void load(const float* img, int w, int C, int c, float t[4], float g[4], float k[4]) const {
+#pragma unroll
+        for (int tp = 0; tp < 4; ++tp) {
+            const int xx = cx[tp & 1];
+            const size_t row = (size_t)cy[tp >> 1] * w;
+            t[tp] = __ldg(img + (row + xx) * C + c);
+            g[tp] = 0.5f * (__ldg(img + (row + ex[tp & 1]) * C + c) - __ldg(img + (row + wx[tp & 1]) * C + c));
+            k[tp] = 0.5f * (__ldg(img + ((size_t)sy[tp >> 1] * w + xx) * C + c) - __ldg(img + ((size_t)ny[tp >> 1] * w + xx) * C + c));
+        }
+    }
+    // the adjoint of load for one channel: df on the values, dgx / dgy on the gradients, each tap weighted by wt
+    __device__ __forceinline__ void scatter(float* dimg, int w, int C, int c, const float wt[4], float df, float dgx, float dgy) const {
+#pragma unroll
+        for (int tp = 0; tp < 4; ++tp) {
+            const int xx = cx[tp & 1];
+            const size_t row = (size_t)cy[tp >> 1] * w;
+            const float hx = 0.5f * wt[tp] * dgx, hy = 0.5f * wt[tp] * dgy;
+            atomicAdd(dimg + (row + xx) * C + c, wt[tp] * df);
+            atomicAdd(dimg + (row + ex[tp & 1]) * C + c, hx); atomicAdd(dimg + (row + wx[tp & 1]) * C + c, -hx);
+            atomicAdd(dimg + ((size_t)sy[tp >> 1] * w + xx) * C + c, hy); atomicAdd(dimg + ((size_t)ny[tp >> 1] * w + xx) * C + c, -hy);
+        }
+    }
+};
 
 // smem layout (floats): S_dd [K][K] | S_cd [6][K] | S_dc [K][6] | S_cc [36] | ghat [P] | W [K] | pose [16] | rhat [C]
-template <int BWD_KL>
+template <int BWD_KL, int LAYOUT>
 __global__ void __launch_bounds__(BWD_THREADS, 2)
 lm_build_bwd_kernel(const BwdParams prm)
 {
     extern __shared__ __align__(16) float sm[];
-    const int K = prm.K, C = prm.C, N = prm.N, h = prm.h, w = prm.w, P = 6 + K, C3 = 3 * C;
+    constexpr bool FLY = LAYOUT != BWD_3C;
+    const int K = prm.K, C = prm.C, N = prm.N, h = prm.h, w = prm.w, P = 6 + K, C3 = FLY ? C : 3 * C;   // C3: conv2's channel stride
     float* Sdd = sm;
     float* Scd = Sdd + (size_t)K * K;
     float* Sdc = Scd + 6 * K;
@@ -150,9 +195,19 @@ lm_build_bwd_kernel(const BwdParams prm)
             // ---- pass 1: M = G^T G, q = G^T d (lanes over channels) ----------------------------------------------------------------
             float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f;
             for (int c = lane; c < C; c += 32) {
-                const float f2 = w00 * __ldg(img + o00 + c) + w01 * __ldg(img + o01 + c) + w10 * __ldg(img + o10 + c) + w11 * __ldg(img + o11 + c);
-                const float gx = w00 * __ldg(img + o00 + C + c) + w01 * __ldg(img + o01 + C + c) + w10 * __ldg(img + o10 + C + c) + w11 * __ldg(img + o11 + C + c);
-                const float gy = w00 * __ldg(img + o00 + 2 * C + c) + w01 * __ldg(img + o01 + 2 * C + c) + w10 * __ldg(img + o10 + 2 * C + c) + w11 * __ldg(img + o11 + 2 * C + c);
+                float f2, gx, gy;
+                if constexpr (FLY) {
+                    const FlyTaps fly(x0, x1, y0, y1, h, w);
+                    float t[4], g[4], k[4];
+                    fly.load(img, w, C, c, t, g, k);
+                    f2 = w00 * t[0] + w01 * t[1] + w10 * t[2] + w11 * t[3];
+                    gx = w00 * g[0] + w01 * g[1] + w10 * g[2] + w11 * g[3];
+                    gy = w00 * k[0] + w01 * k[1] + w10 * k[2] + w11 * k[3];
+                } else {
+                    f2 = w00 * __ldg(img + o00 + c) + w01 * __ldg(img + o01 + c) + w10 * __ldg(img + o10 + c) + w11 * __ldg(img + o11 + c);
+                    gx = w00 * __ldg(img + o00 + C + c) + w01 * __ldg(img + o01 + C + c) + w10 * __ldg(img + o10 + C + c) + w11 * __ldg(img + o11 + C + c);
+                    gy = w00 * __ldg(img + o00 + 2 * C + c) + w01 * __ldg(img + o01 + 2 * C + c) + w10 * __ldg(img + o10 + 2 * C + c) + w11 * __ldg(img + o11 + 2 * C + c);
+                }
                 const float d = __ldg(c1 + c) - f2;
                 m11 = fmaf(gx, gx, m11); m12 = fmaf(gx, gy, m12); m22 = fmaf(gy, gy, m22); q1 = fmaf(gx, d, q1); q2 = fmaf(gy, d, q2);
             }
@@ -221,9 +276,17 @@ lm_build_bwd_kernel(const BwdParams prm)
             // ---- pass 2: dd, dG per channel -> dconv1, scatter into dconv2, coordinate gradient ------------------------------------------
             float du = 0.f, dv = 0.f;
             for (int c = lane; c < C; c += 32) {
-                const float t00 = __ldg(img + o00 + c), t01 = __ldg(img + o01 + c), t10 = __ldg(img + o10 + c), t11 = __ldg(img + o11 + c);
-                const float g00 = __ldg(img + o00 + C + c), g01 = __ldg(img + o01 + C + c), g10 = __ldg(img + o10 + C + c), g11 = __ldg(img + o11 + C + c);
-                const float k00 = __ldg(img + o00 + 2 * C + c), k01 = __ldg(img + o01 + 2 * C + c), k10 = __ldg(img + o10 + 2 * C + c), k11 = __ldg(img + o11 + 2 * C + c);
+                float t00, t01, t10, t11, g00, g01, g10, g11, k00, k01, k10, k11;
+                if constexpr (FLY) {
+                    const FlyTaps fly(x0, x1, y0, y1, h, w);
+                    float t[4], g[4], k[4];
+                    fly.load(img, w, C, c, t, g, k);
+                    t00 = t[0]; t01 = t[1]; t10 = t[2]; t11 = t[3]; g00 = g[0]; g01 = g[1]; g10 = g[2]; g11 = g[3]; k00 = k[0]; k01 = k[1]; k10 = k[2]; k11 = k[3];
+                } else {
+                    t00 = __ldg(img + o00 + c); t01 = __ldg(img + o01 + c); t10 = __ldg(img + o10 + c); t11 = __ldg(img + o11 + c);
+                    g00 = __ldg(img + o00 + C + c); g01 = __ldg(img + o01 + C + c); g10 = __ldg(img + o10 + C + c); g11 = __ldg(img + o11 + C + c);
+                    k00 = __ldg(img + o00 + 2 * C + c); k01 = __ldg(img + o01 + 2 * C + c); k10 = __ldg(img + o10 + 2 * C + c); k11 = __ldg(img + o11 + 2 * C + c);
+                }
                 const float f2 = w00 * t00 + w01 * t01 + w10 * t10 + w11 * t11;
                 const float gx = w00 * g00 + w01 * g01 + w10 * g10 + w11 * g11;
                 const float gy = w00 * k00 + w01 * k01 + w10 * k10 + w11 * k11;
@@ -232,9 +295,15 @@ lm_build_bwd_kernel(const BwdParams prm)
                 const float dgx = gx * Q00 + gy * Q10 + d * z0, dgy = gx * Q01 + gy * Q11 + d * z1;
                 dc1[c] = dd;
                 const float df = -dd;
-                atomicAdd(dimg + o00 + c, w00 * df); atomicAdd(dimg + o01 + c, w01 * df); atomicAdd(dimg + o10 + c, w10 * df); atomicAdd(dimg + o11 + c, w11 * df);
-                atomicAdd(dimg + o00 + C + c, w00 * dgx); atomicAdd(dimg + o01 + C + c, w01 * dgx); atomicAdd(dimg + o10 + C + c, w10 * dgx); atomicAdd(dimg + o11 + C + c, w11 * dgx);
-                atomicAdd(dimg + o00 + 2 * C + c, w00 * dgy); atomicAdd(dimg + o01 + 2 * C + c, w01 * dgy); atomicAdd(dimg + o10 + 2 * C + c, w10 * dgy); atomicAdd(dimg + o11 + 2 * C + c, w11 * dgy);
+                if constexpr (FLY) {
+                    const float wt[4] = {w00, w01, w10, w11};
+                    const FlyTaps fly(x0, x1, y0, y1, h, w);
+                    fly.scatter(dimg, w, C, c, wt, df, dgx, dgy);
+                } else {
+                    atomicAdd(dimg + o00 + c, w00 * df); atomicAdd(dimg + o01 + c, w01 * df); atomicAdd(dimg + o10 + c, w10 * df); atomicAdd(dimg + o11 + c, w11 * df);
+                    atomicAdd(dimg + o00 + C + c, w00 * dgx); atomicAdd(dimg + o01 + C + c, w01 * dgx); atomicAdd(dimg + o10 + C + c, w10 * dgx); atomicAdd(dimg + o11 + C + c, w11 * dgx);
+                    atomicAdd(dimg + o00 + 2 * C + c, w00 * dgy); atomicAdd(dimg + o01 + 2 * C + c, w01 * dgy); atomicAdd(dimg + o10 + 2 * C + c, w10 * dgy); atomicAdd(dimg + o11 + 2 * C + c, w11 * dgy);
+                }
                 du += df * ((1.f - dy) * (t01 - t00) + dy * (t11 - t10)) + dgx * ((1.f - dy) * (g01 - g00) + dy * (g11 - g10)) + dgy * ((1.f - dy) * (k01 - k00) + dy * (k11 - k10));
                 dv += df * ((1.f - dx) * (t10 - t00) + dx * (t11 - t01)) + dgx * ((1.f - dx) * (g10 - g00) + dx * (g11 - g01)) + dgy * ((1.f - dx) * (k10 - k00) + dx * (k11 - k01));
             }
@@ -276,11 +345,14 @@ int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const 
                  int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, cudaStream_t st)
 {
     const int K = lv->K, P = 6 + K;
-    BANET_REQUIRE(lv->conv2_channels == 3 * lv->C, BANET_ERR_UNSUPPORTED, "lm_build_bwd: conv2 must be the [F2|gx|gy] (3C) layout");
     BANET_REQUIRE(K <= 32 * BWD_KL_MAX, BANET_ERR_UNSUPPORTED, "lm_build_bwd: K=%d > %d", K, 32 * BWD_KL_MAX);
     const size_t smem = ((size_t)K * K + 12 * (size_t)K + 36 + P + K + 16 + lv->C) * sizeof(float);
     BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_build_bwd: K=%d, C=%d need %zu B of shared memory", K, lv->C, smem);
-    void (*kern)(const BwdParams) = K <= 32 ? lm_build_bwd_kernel<1> : (K <= 128 ? lm_build_bwd_kernel<4> : lm_build_bwd_kernel<8>);
+    void (*kern)(const BwdParams);
+    if (lv->conv2_channels == 3 * lv->C)
+        kern = K <= 32 ? lm_build_bwd_kernel<1, BWD_3C> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_3C> : lm_build_bwd_kernel<8, BWD_3C>);
+    else
+        kern = K <= 32 ? lm_build_bwd_kernel<1, BWD_F2> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_F2> : lm_build_bwd_kernel<8, BWD_F2>);
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("lm_build_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
     BwdParams prm;
@@ -291,7 +363,7 @@ int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const 
     prm.exact_sym = exact_sym;
     prm.tiles_per_pair = (lv->N + BWD_TILE - 1) / BWD_TILE;
     prm.total_tiles = (long long)lv->nb * prm.tiles_per_pair;
-    cudaMemsetAsync(dconv2, 0, (size_t)lv->nb * lv->h * lv->w * 3 * lv->C * sizeof(float), st);
+    cudaMemsetAsync(dconv2, 0, (size_t)lv->nb * lv->h * lv->w * lv->conv2_channels * sizeof(float), st);
     cudaMemsetAsync(dR, 0, (size_t)lv->nb * 9 * sizeof(float), st);
     cudaMemsetAsync(dT, 0, (size_t)lv->nb * 3 * sizeof(float), st);
     if (K > 0) cudaMemsetAsync(dW, 0, (size_t)lv->nb * K * sizeof(float), st);

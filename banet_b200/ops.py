@@ -537,7 +537,8 @@ def lm_run_workspace_bytes(levels: Sequence[Level], precision: int = _lib.PREC_A
 
 # ------------------------------------------------------------------------------------------ backward of one iteration
 def lm_build_bwd(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], dH: Tensor, dg: Tensor, drbar_sum: Tensor, exact_sym: bool = False):
-    """Backward of lm_build (banet_lm_build_bwd) -> dconv1, dconv2, dD, dB, dR, dT, dW.  conv2 must be the 3C layout."""
+    """Backward of lm_build (banet_lm_build_bwd) -> dconv1, dconv2, dD, dB, dR, dT, dW.  dconv2 has conv2's layout: [nb,h,w,3C] for
+    [F2|gx|gy], [nb,h,w,C] for F2 only (the adjoint of the on-the-fly gradient stencil is applied inside the kernel)."""
     lib = load()
     st, keep = level.as_struct()
     nb, K, Cc, N = st.nb, st.K, st.C, st.N
@@ -546,7 +547,7 @@ def lm_build_bwd(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], dH: Te
     Wt = None if K == 0 else _chk(W, "W", (nb, K, 1))
     dH = _chk(dH, "dH", (nb, P, P)); dg = _chk(dg.reshape(nb, P), "dg", (nb, P)); dr = _chk(drbar_sum, "drbar_sum", (nb, Cc))
     dev = R.device
-    dconv1 = torch.empty(nb, N, Cc, device=dev); dconv2 = torch.empty(nb, st.h, st.w, 3 * Cc, device=dev)
+    dconv1 = torch.empty(nb, N, Cc, device=dev); dconv2 = torch.empty(nb, st.h, st.w, st.conv2_channels, device=dev)
     dD = torch.empty(nb, N, 1, device=dev); dB = None if K == 0 else torch.empty(nb, N, K, device=dev)
     dR = torch.empty(nb, 3, 3, device=dev); dT = torch.empty(nb, 3, 1, device=dev); dW = None if K == 0 else torch.empty(nb, K, 1, device=dev)
     check(lib.banet_lm_build_bwd(C.byref(st), R.data_ptr(), T.data_ptr(), _ptr(Wt), dH.data_ptr(), dg.data_ptr(), dr.data_ptr(), int(bool(exact_sym)),

@@ -173,9 +173,10 @@ int    banet_lm_step(const float* H, const float* g, const float* rbar_sum, int 
  *      lambda, the MLP variables).  J, G, d and the tiled upstream gradients of utils.cu:613-617 are never formed.
  * ---------------------------------------------------------------------------------------------- */
 /* Backward of banet_lm_build.  dH [nb,P,P] (as the solve's backward emits it: not symmetric), dg [nb,P],
- * drbar_sum [nb,C]  ->  dconv1 [nb,N,C], dconv2 [nb,h,w,3C], dD [nb,N,1], dB [nb,N,K], dR [nb,3,3], dT [nb,3,1],
- * dW [nb,K,1]; every output is overwritten.  conv2 must be the reference's [F2|gx|gy] layout (the F2-only layout
- * adds banet_grad_fixed_concat_bwd).  exact_sym as in banet_eqc_bwd (0 = the reference's 2*A*Ghat). */
+ * drbar_sum [nb,C]  ->  dconv1 [nb,N,C], dconv2 [nb,h,w,conv2_channels], dD [nb,N,1], dB [nb,N,K], dR [nb,3,3],
+ * dT [nb,3,1], dW [nb,K,1]; every output is overwritten.  conv2 may be either layout banet_lm_build takes: the
+ * reference's [F2|gx|gy] (3C), or F2 only (C), whose dconv2 is the gradient w.r.t. F2 through the build's on-the-fly
+ * REFLECT-by-one gradient stencil.  exact_sym as in banet_eqc_bwd (0 = the reference's 2*A*Ghat). */
 int    banet_lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W,
                           const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
                           float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
