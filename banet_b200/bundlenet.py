@@ -203,8 +203,7 @@ class BundleNet(torch.nn.Module):
         """WindowIteration on nw windows with the keyframe tensors once per window (conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K]):
         the keyframe build (banet_lm_keyframe_*), fused autograd path when gradients are recorded, else one iteration of
         ops.lm_keyframe_run.  fp32 SIMT only: a TF32 precision raises."""
-        if self.precision not in (_lib.PREC_AUTO, _lib.PREC_FP32_SIMT):
-            raise RuntimeError(f"precision {self.precision}: the keyframe form of WindowIteration has no tensor-core build; use AUTO or FP32_SIMT")
+        self._require_keyframe_precision()
         nw, nf = R.shape[0], R.shape[1]
         if self._wants_grad(conv1, conv2, D, B, R, T, W):
             if self.training_path == "reference_split":
@@ -218,6 +217,10 @@ class BundleNet(torch.nn.Module):
                                                  mlp_packed=[self.mlp_packed(str(level))], l2_regularizer_base=base, precision=self.precision)
         self._check_status(status.reshape(nw, nf))
         return Rn.reshape(nw, nf, 3, 3), Tn.reshape(nw, nf, 3, 1), Wn
+
+    def _require_keyframe_precision(self) -> None:
+        if self.precision not in (_lib.PREC_AUTO, _lib.PREC_FP32_SIMT):
+            raise RuntimeError(f"precision {self.precision}: the keyframe form of WindowIteration has no tensor-core build; use AUTO or FP32_SIMT")
 
     # ---- level schedulers ----------------------------------------------------------------------
     def _prepare(self, intrisic: Tensor, points: Tensor):
@@ -279,6 +282,88 @@ class BundleNet(torch.nn.Module):
             depth = compose(init_depth.reshape(nb, -1), basis.reshape(nb, -1, K), W)   # :397
             Ds.append(depth.reshape(nb, oh, ow, 1))
         return Rs, Ts, Ds
+
+    def WindowResize(self, intrisic, key_layers, frame_layers, points, basis, init_depth, init_rotation=None, init_translation=None):
+        """BundleResize's schedule (reference bundlenet.py:332-399) for nw keyframe windows of nf frames (an extension): levels 2, 3 x one
+        joint window iteration, the keyframe depth init_depth + basis.W shared by the window's frames.
+          intrisic [nw,4,1]            one camera per window (keyframe rays and every frame's projection)
+          key_layers 4 x [nw,h_l,w_l,C]  the keyframes' feature pyramids;  frame_layers 4 x [nw,nf,h_l,w_l,C]  the frames' (F2 only)
+          points [nw,N,2]              keyframe pixels in the reference's crop coordinates
+          basis [nw,h/2,w/2,K], init_depth [nw,h/2,w/2,1];  init_rotation [nw,nf,3,3], init_translation [nw,nf,3,1] (default I, 0)
+        conv1, p, D, B and W are once per window, conv2, R and T per frame.  -> (Rs [nw,nf,3,3], Ts [nw,nf,3,1], depths [nw,h/2,w/2,1]), one
+        entry per level; last_status [nw,nf], or-ed over the levels.
+        No gradients recorded: one ops.lm_keyframe_run iteration per level on the frames' F2 maps as they are.  Gradients recorded: the keyframe
+        form of autograd.window_batch_iteration_fused per level on [F2|gx|gy] (the keyframe backward takes that layout only); gradients reach
+        both pyramids, the basis, the initial pose and the lambda-MLP parameters, init_depth through the output depth only (:341, :397).
+        AUTO or FP32_SIMT only, like the keyframe form of WindowIteration."""
+        if self.vmatrix_batch_scramble:
+            raise RuntimeError("vmatrix_batch_scramble=True is a 2-view quirk (bundlenet.py:45); the window solve has per-frame VMatrix only")
+        self._require_keyframe_precision()
+        nw, nf, K = self._window_resize_shapes(intrisic, key_layers, frame_layers, points, basis, init_depth, init_rotation, init_translation)
+        _points, intr = self._prepare(intrisic, points)
+        grad = self._wants_grad(*key_layers, *frame_layers, basis, init_rotation, init_translation)
+        resample = _ag.resample if grad else ops.resample
+        compose = _ag.depth_compose if grad or self._wants_grad(init_depth) else ops.depth_compose
+        d = ops.resample(init_depth.detach(), _points, 0.5)                    # :341-343, once per window
+        b = resample(basis, _points, 0.5)                                      # :344
+        p = ops.compute_coordinates(_points, intr, True)                       # :358
+        dev = points.device
+        R = torch.eye(3, device=dev).repeat(nw, nf, 1, 1) if init_rotation is None else init_rotation
+        T = torch.zeros(nw, nf, 3, 1, device=dev) if init_translation is None else init_translation
+        W = torch.zeros(nw, K, 1, device=dev)
+        oh, ow = self.geo.out_hw
+        Rs, Ts, Ds = [], [], []
+        status = None
+        for level in range(2, 4):                                              # :376
+            scale = 2 ** (3 - level)
+            conv1 = resample(key_layers[level], _points, 1.0 / scale)         # :385, once per window
+            F2 = frame_layers[level]
+            if grad:                                                           # :386-389; the keyframe backward takes [F2|gx|gy] only
+                conv2 = _ag.grad_fixed_concat(F2.reshape(nw * nf, *F2.shape[2:])).reshape(*F2.shape[:4], 3 * F2.shape[4])
+            else:                                                              # the keyframe forward derives gx, gy from F2 itself
+                conv2 = F2
+            R, T, W = self._keyframe_batch_iteration(conv1, conv2, (intr / scale).unsqueeze(1), p, d, b, R, T, W, 1000.0, level)   # :393
+            status = self.last_status if status is None else status | self.last_status
+            Rs.append(R); Ts.append(T)
+            depth = compose(init_depth.reshape(nw, -1), basis.reshape(nw, -1, K), W)   # :397
+            Ds.append(depth.reshape(nw, oh, ow, 1))
+        self._check_status(status)
+        return Rs, Ts, Ds
+
+    def _window_resize_shapes(self, intrisic, key_layers, frame_layers, points, basis, init_depth, init_rotation, init_translation):
+        """WindowResize's arguments checked against each other before any kernel runs -> (nw, nf, K).  nw comes from key_layers[3], nf from
+        frame_layers[3]; an error names the argument that disagrees."""
+        def fail(name, t, want):
+            got = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__
+            raise _lib.BanetError(f"WindowResize: {name} must be {want}; got {got}")
+
+        for name, ls in (("key_layers", key_layers), ("frame_layers", frame_layers)):
+            if len(ls) != 4:
+                raise _lib.BanetError(f"WindowResize: {name} must hold the 4 pyramid levels 0..3; got {len(ls)}")
+        if key_layers[3].dim() != 4:
+            fail("key_layers[3]", key_layers[3], "[nw,h,w,C]")
+        if frame_layers[3].dim() != 5:
+            fail("frame_layers[3]", frame_layers[3], "[nw,nf,h,w,C]")
+        nw, nf, C = key_layers[3].shape[0], frame_layers[3].shape[1], key_layers[3].shape[3]
+        for l in (2, 3):
+            kl, fl = key_layers[l], frame_layers[l]
+            if kl.dim() != 4 or kl.shape[0] != nw or kl.shape[3] != C:
+                fail(f"key_layers[{l}]", kl, f"[nw={nw},h,w,C={C}]")
+            if tuple(fl.shape) != (nw, nf, *kl.shape[1:]):
+                fail(f"frame_layers[{l}]", fl, f"[nw,nf,h,w,C] = {(nw, nf, *kl.shape[1:])} (nw of key_layers, the keyframe's map size)")
+        if intrisic.shape[0] != nw or intrisic.numel() != 4 * nw:
+            fail("intrisic", intrisic, f"[nw={nw},4,1]")
+        if points.dim() != 3 or points.shape[0] != nw or points.shape[2] != 2:
+            fail("points", points, f"[nw={nw},N,2]")
+        oh, ow = self.geo.out_hw
+        if basis.dim() != 4 or tuple(basis.shape[:3]) != (nw, oh, ow):
+            fail("basis", basis, f"[nw={nw},{oh},{ow},K]")
+        if tuple(init_depth.shape) != (nw, oh, ow, 1):
+            fail("init_depth", init_depth, f"[nw={nw},{oh},{ow},1]")
+        for name, t, tail in (("init_rotation", init_rotation, (3, 3)), ("init_translation", init_translation, (3, 1))):
+            if t is not None and tuple(t.shape) != (nw, nf, *tail):
+                fail(name, t, f"[nw={nw},nf={nf},{tail[0]},{tail[1]}]")
+        return nw, nf, basis.shape[3]
 
     # ---- training losses (reference bundlenet.py:401-463): stock torch, like the CNN around the layer ---------------------------------
     def lossR(self, predQ: Tensor, gtQ: Tensor) -> Tensor:

@@ -266,3 +266,93 @@ def make_resize_scene(nimg: int, H: int, W: int, C: int, K: int, level_ids=(0, 1
     T0 = torch.cat([T_true + randn(half, 3, 1) * start_trans_noise_m, -T_true + randn(half, 3, 1) * start_trans_noise_m], 0)
     W0 = torch.zeros(nimg, K, 1, device=dev, dtype=dtype)
     return ResizeScene(layers, basis, depth, intr, scales, R0, T0, W0)
+
+
+@dataclass
+class WindowResizeScene:
+    """Inputs of BundleNet.WindowResize (nw keyframe windows of nf frames at the reference's 320 x 256 crop) and the planted solution."""
+    intrisic: torch.Tensor              # [nw,4,1] raw camera, before the crop fix-ups of bundlenet.py:354-357
+    key_layers: List[torch.Tensor]      # 4 x [nw,h_l,w_l,C] keyframe feature maps, levels 0..3
+    frame_layers: List[torch.Tensor]    # 4 x [nw,nf,h_l,w_l,C] frame feature maps (F2)
+    points: torch.Tensor                # [nw,N,2] keyframe pixels in crop coordinates
+    basis: torch.Tensor                 # [nw,128,160,K]
+    init_depth: torch.Tensor            # [nw,128,160,1]
+    R_true: torch.Tensor; T_true: torch.Tensor; W_true: torch.Tensor     # [nw,nf,3,3], [nw,nf,3,1], [nw,K,1]
+    R0: torch.Tensor; T0: torch.Tensor                                   # start pose [nw,nf,3,3], [nw,nf,3,1]
+
+
+def make_window_resize_scene(nw: int, nf: int, C: int, K: int, n_points: Optional[int] = None, seed: int = 1234, device="cpu",
+                             dtype=torch.float32, rot_deg: float = 1.0, trans_m: float = 0.02, w_std: float = 0.02,
+                             start_trans_noise_m: float = 0.01, inverse_warp_iters: int = 12) -> WindowResizeScene:
+    """Planted-solution window batch for BundleNet.WindowResize.  Each window has one keyframe (feature pyramid, half-resolution depth and
+    basis, planted W*) and nf frames with their own planted (R*, T*).  The keyframe's pixel at level l (finest-level pixel / 2**(3-l)) sees
+    depth D + B.W*, sampled from the half-resolution maps as the solver samples them; frame f's feature at pixel v is the keyframe's feature
+    map sampled at the keyframe pixel u whose warp under (R*_f, T*_f, D + B.W*) lands on v.  u is found by a fixed-point iteration
+    u <- u + v - warp(u) (a motion of a few pixels, so it contracts), which makes the residual at the planted solution the bilinear
+    interpolation error of the blurred features rather than zero.  points: the dense level-3 grid (n_points None) or n_points random
+    sub-pixel points, given in the crop coordinates that BundleResize maps to the 320 x 256 grid (bundlenet.py:338-339).  The start pose is
+    (I, T* + noise): at (I, 0) the depth Jacobian vanishes (see the module docstring)."""
+    from .bundlenet import ResizeGeometry
+    geo = ResizeGeometry()
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    dev = torch.device(device)
+
+    def randn(*s_):
+        return torch.randn(*s_, generator=g, dtype=torch.float32).to(dev, dtype)
+
+    def rand(*s_):
+        return torch.rand(*s_, generator=g, dtype=torch.float32).to(dev, dtype)
+
+    hb, wb = geo.out_hw
+    H, W = 2 * hb, 2 * wb
+    intrisic = torch.tensor([280.0, 285.0, 160.0, 120.0], device=dev, dtype=dtype).reshape(1, 4, 1).repeat(nw, 1, 1)
+    k = intrisic[:, :, 0]
+    intr = torch.stack([geo.fx_num * k[:, 0] / geo.fx_den, geo.fy_num * k[:, 1] / geo.fy_den,          # the solver's camera (:354-357)
+                        geo.fx_num * k[:, 2] / geo.fx_den - geo.ox_sub, geo.fy_num * k[:, 3] / geo.fy_den - geo.oy_sub], 1)
+    bm = gaussian_blur_nchw(randn(nw, K, hb, wb), 4.0)
+    basis = (bm * torch.rsqrt(bm.flatten(2).var(dim=2) + 1e-3).view(nw, K, 1, 1)).permute(0, 2, 3, 1).contiguous()
+    dm = gaussian_blur_nchw(1.0 + 2.0 * rand(nw, 1, hb, wb), 4.0).permute(0, 2, 3, 1)
+    dmin = dm.flatten(1).min(1).values.view(nw, 1, 1, 1); dmax = dm.flatten(1).max(1).values.view(nw, 1, 1, 1)
+    depth = (1.0 + 2.0 * (dm - dmin) / (dmax - dmin).clamp_min(1e-6)).contiguous()
+    R_true = rodrigues(randn(nw * nf, 3) * math.radians(rot_deg)).reshape(nw, nf, 3, 3)
+    T_true = randn(nw, nf, 3, 1) * trans_m
+    W_true = randn(nw, K, 1) * w_std
+    dfull = (depth + (basis.reshape(nw, -1, K) @ W_true).reshape(nw, hb, wb, 1)).contiguous()        # D + B.W* on the half-resolution grid
+    if n_points is None:
+        vv, uu = torch.meshgrid(torch.arange(H, device=dev, dtype=dtype), torch.arange(W, device=dev, dtype=dtype), indexing="ij")
+        pts = torch.stack([uu.reshape(-1), vv.reshape(-1)], -1).unsqueeze(0).repeat(nw, 1, 1)
+    else:
+        pts = rand(nw, n_points, 2) * torch.tensor([W - 1.0, H - 1.0], device=dev, dtype=dtype)
+    points = torch.stack([pts[..., 0] * geo.dx / geo.sx + geo.cx, pts[..., 1] * geo.dy / geo.sy + geo.cy], -1)   # inverse of :338-339
+
+    key_layers, frame_layers = [], []
+    for lid in range(4):
+        s_ = 2 ** (3 - lid)
+        h, w = H // s_, W // s_
+        key = torch.empty(nw, h, w, C, device=dev, dtype=dtype)
+        frames = torch.empty(nw, nf, h, w, C, device=dev, dtype=dtype)
+        vv, uu = torch.meshgrid(torch.arange(h, device=dev, dtype=dtype), torch.arange(w, device=dev, dtype=dtype), indexing="ij")
+        vx, vy = uu.reshape(1, -1).expand(nf, -1), vv.reshape(1, -1).expand(nf, -1)
+        for wi in range(nw):
+            f = gaussian_blur_nchw(randn(1, C, h, w), 2.0)
+            key[wi] = (f / f.flatten(2).std(dim=2).clamp_min(1e-6).view(1, C, 1, 1)).permute(0, 2, 3, 1)[0]
+            fx, fy, ox, oy = [intr[wi, i] / s_ for i in range(4)]
+            dmap = dfull[wi:wi + 1].expand(nf, hb, wb, 1)
+
+            def warp(ux, uy):
+                ray = torch.stack([(ux - ox) / fx, (uy - oy) / fy, torch.ones_like(ux)], 1)
+                p = ray / ray.norm(dim=1, keepdim=True)
+                xs = (ux * (s_ / 2.0)).clamp(0.0, wb - 1.0); ys = (uy * (s_ / 2.0)).clamp(0.0, hb - 1.0)   # level pixel -> half-resolution map
+                Dt = bilinear_zero_pad(dmap, xs, ys)                                                      # [nf,h*w,1]
+                X = (R_true[wi] @ p) * Dt.transpose(1, 2) + T_true[wi]
+                return fx * (X[:, 0] / X[:, 2]) + ox, fy * (X[:, 1] / X[:, 2]) + oy
+
+            ux, uy = vx.clone(), vy.clone()
+            for _ in range(inverse_warp_iters):
+                px_, py_ = warp(ux, uy)
+                ux = (ux + (vx - px_)).clamp(-w, 2.0 * w); uy = (uy + (vy - py_)).clamp(-h, 2.0 * h)
+            frames[wi] = bilinear_zero_pad(key[wi:wi + 1].expand(nf, h, w, C), ux, uy).reshape(nf, h, w, C)
+        key_layers.append(key); frame_layers.append(frames)
+    R0 = torch.eye(3, device=dev, dtype=dtype).repeat(nw, nf, 1, 1)
+    T0 = T_true + randn(nw, nf, 3, 1) * start_trans_noise_m
+    return WindowResizeScene(intrisic, key_layers, frame_layers, points.contiguous(), basis, depth, R_true, T_true, W_true, R0, T0)
