@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "lm_build.h"
 #include "tc_utils.cuh"
+#include "mma_role.cuh"
 #include "tmap.h"
 #include <stdlib.h>
 
@@ -585,67 +586,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
     } else {
         // ===================================================================== MMA warps: D = A^T R per tile, accumulated over the pair span
         setmaxnreg_inc<136>();
-        const int mw = warp - (W0 + GW + AW), g = lane >> 2, t = lane & 3;
-        const SlotLayout L{KR, C};
-        // lm_reduce reads the lower block triangle of H_dd only (and mirrors it): m-block i (rows 16i .. 16i+15 of D) needs the n8 column
-        // blocks 0 .. 2i+1, plus the [v | t] block (columns KR .. KR+7).  With 8 m-blocks warp mw takes m-blocks mw and 7-mw: 20 n8 blocks
-        // for every warp.  K = 64 / 32: one m-block per warp.
-        constexpr int NMB = KR / 16, NQ = NMB == 8 ? 20 : 2 * NMB + 1;
-        const int mb0 = mw, mb1 = NMB == 8 ? 7 - mw : -1;
-        const int cnt0 = mw < NMB ? 2 * mb0 + 3 : 0;         // n8 blocks of m-block mb0; the rest of the NQ belong to mb1
-        auto col_of = [&](int q) {                           // first column of accumulator block q (warp-uniform)
-            const int lq = q < cnt0 ? q : q - cnt0, cq = q < cnt0 ? cnt0 : NQ - cnt0;
-            return lq == cq - 1 ? KR : 8 * lq;
-        };
-        float acc[NQ][4];
-#pragma unroll
-        for (int q = 0; q < NQ; ++q) acc[q][0] = acc[q][1] = acc[q][2] = acc[q][3] = 0.f;
-        const uint32_t rhi = smem_u32(base + SM::off_R), rlo = smem_u32(base + SM::off_Rlo), alo = smem_u32(base + SM::off_Alo);
-        int span = 0;
-        int rr = (ntiles > 0) ? (int)((unsigned)t_begin % (unsigned)prm.tiles_per_pair) : 0;
-        for (int j = 0; j < ntiles; ++j) {
-            const int s = j % NST;
-            mbar_wait_parked(rready, j & 1);
-            mbar_wait_parked(&fullB[s], (j / NST) & 1);      // orders the TMA writes of the stage before the fragment loads
-            const uint32_t ahi = smem_u32(base + SM::off_A + s * STAGE_A);
-#pragma unroll 1
-            for (int pass = 0; pass < MODE; ++pass) {        // hi x hi, then A_lo x R, then A x R_lo, into the same accumulators
-                const uint32_t a = pass == 1 ? alo : ahi, r = pass == 2 ? rlo : rhi;
-#pragma unroll 2
-                for (int kk = 0; kk < TILE / 8; ++kk) {
-                    uint32_t f0[4] = {0u, 0u, 0u, 0u}, f1[4] = {0u, 0u, 0u, 0u};
-                    if (cnt0 > 0) load_a_frag(f0, a, 16 * mb0, kk, lane);
-                    if (mb1 >= 0) load_a_frag(f1, a, 16 * mb1, kk, lane);
-#pragma unroll
-                    for (int q = 0; q < NQ; ++q) {
-                        if (q >= cnt0 && mb1 < 0) continue;
-                        const bool first = q < cnt0;
-                        const uint32_t af[4] = {first ? f0[0] : f1[0], first ? f0[1] : f1[1], first ? f0[2] : f1[2], first ? f0[3] : f1[3]};
-                        mma_step_rn(acc[q], af, r, col_of(q), kk, lane);
-                    }
-                }
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(rfree);
-            const bool last_of_pair = (++rr == prm.tiles_per_pair) || (j == ntiles - 1);
-            if (rr == prm.tiles_per_pair) rr = 0;
-            if (last_of_pair) {                              // slot of the span: H_dd column-major (hdd_transposed), ext rows [v | t]
-                float* slot = prm.partials + ((size_t)blockIdx.x * prm.max_span + span) * prm.slot_floats;
-#pragma unroll
-                for (int q = 0; q < NQ; ++q) {
-                    if (q >= cnt0 && mb1 < 0) continue;
-                    const int i0 = 16 * (q < cnt0 ? mb0 : mb1) + g, n0 = col_of(q) + 2 * t;
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const int i = i0 + (e >> 1) * 8, n = n0 + (e & 1);
-                        if (n < KR) slot[(size_t)n * KR + i] = acc[q][e];
-                        else if (n - KR < 7) slot[L.off_ext() + (n - KR) * KR + i] = acc[q][e];
-                        acc[q][e] = 0.f;
-                    }
-                }
-                ++span;
-            }
-        }
+        mma_role<SM, STAGE_A, MODE, KR>(prm, base, fullB, rready, rfree, t_begin, ntiles, warp - (W0 + GW + AW), lane);
     }
 }
 

@@ -138,7 +138,8 @@ __device__ __forceinline__ void mma_step(float (&d)[4], const uint32_t (&af)[4],
     r += kk * 1024;
     mma_tf32_m16n8k8(d, af, lds_tf32(r + frag_off(n, t)), lds_tf32(r + frag_off(n, t + 4)));
 }
-// The same step for long sums: the tensor core forms the 8-pixel product from zero and it is added to d in round-to-nearest fp32.
+// The same step for long sums: the tensor core forms the 8-pixel product from zero and it is added to d in round-to-nearest fp32
+// (the build kernels' MMA role, mma_role.cuh: mma_add_rn, takes the same step on fragments it loads itself).
 // The tensor core's own fp32 accumulation truncates (biased toward zero, see tests/test_gpu_tensorcore.py), which over the
 // thousands of steps of a pair span would bias H_dd.
 __device__ __forceinline__ void mma_step_rn(float (&d)[4], const uint32_t (&af)[4], uint32_t r, int n0, int kk, int lane) {
