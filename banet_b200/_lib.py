@@ -13,18 +13,19 @@ LIB_PATH = os.environ.get("BANET_LIB_PATH") or os.path.join(_HERE, "libbanet.so"
 
 BANET_OK = 0
 PREC_AUTO, PREC_FP32_SIMT, PREC_TF32X1, PREC_TF32X2, PREC_TF32X3, PREC_TF32_LEVELWISE = -1, 0, 1, 2, 3, 4
+DTYPE_F32, DTYPE_BF16 = 0, 1          # banet_level_t::feature_dtype (conv1 and conv2)
 
 c_float_p = C.c_void_p      # raw device pointers
 c_stream = C.c_void_p
 
 
 class BanetLevel(C.Structure):
-    """struct banet_level (include/banet_abi.h)."""
+    """struct banet_level (include/banet_abi.h).  feature_dtype is last, so a struct built without it keeps fp32 features."""
     _fields_ = [("nb", C.c_int), ("N", C.c_int), ("C", C.c_int), ("K", C.c_int),
                 ("h", C.c_int), ("w", C.c_int), ("conv2_channels", C.c_int),
                 ("conv1", C.c_void_p), ("conv2", C.c_void_p), ("intr", C.c_void_p),
                 ("p", C.c_void_p), ("D", C.c_void_p), ("B", C.c_void_p),
-                ("grid_w", C.c_int), ("grid_h", C.c_int)]
+                ("grid_w", C.c_int), ("grid_h", C.c_int), ("feature_dtype", C.c_int)]
 
 
 class BanetKeyframeLevel(C.Structure):
@@ -69,6 +70,7 @@ SIGNATURES = {
     "banet_compute_coordinates": (C.c_int, [c_float_p, c_float_p, C.c_int, C.c_int, C.c_int, c_float_p, c_stream]),
     "banet_grad_fixed_concat": (C.c_int, [c_float_p] + [C.c_int] * 5 + [c_float_p, c_stream]),
     "banet_resample": (C.c_int, [c_float_p, c_float_p, C.c_float] + [C.c_int] * 5 + [c_float_p, c_stream]),
+    "banet_resample_bf16": (C.c_int, [C.c_void_p, c_float_p, C.c_float] + [C.c_int] * 5 + [C.c_void_p, c_stream]),
     "banet_interpolate2d": (C.c_int, [c_float_p, c_float_p, C.c_float] + [C.c_int] * 5 + [c_float_p, c_float_p, c_stream]),
     "banet_lm_build_workspace_bytes": (C.c_size_t, [C.POINTER(BanetLevel), C.c_int]),
     "banet_lm_build": (C.c_int, [C.POINTER(BanetLevel)] + [c_float_p] * 3 + [C.c_int] + [c_float_p] * 4

@@ -138,7 +138,7 @@ def iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_b
 # ------------------------------------------------------------------------------------------ fused path
 class _LMBuildFn(torch.autograd.Function):
     """(H, g, rbar_sum) = banet_lm_build(...); backward = banet_lm_build_bwd.  conv2 is the [F2|gx|gy] tensor or F2 only; dconv2 comes back
-    in conv2's layout."""
+    in conv2's layout.  bfloat16 features are saved as they are; their gradients are accumulated in fp32 by the kernel and cast once."""
 
     @staticmethod
     def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, precision, exact_sym, grid):
@@ -162,7 +162,7 @@ class _LMBuildFn(torch.autograd.Function):
         dg = dg if dg is not None else torch.zeros(nb, P, device=conv1.device)
         drbar = drbar if drbar is not None else torch.zeros(nb, conv1.shape[2], device=conv1.device)
         dconv1, dconv2, dD, dB, dR, dT, dW = ops.lm_build_bwd(lv, R, T, W, dH, dg.contiguous(), drbar.contiguous(), ctx.exact_sym)
-        return dconv1, dconv2, dD, dB, dR, dT, dW, None, None, None, None, None
+        return dconv1.to(conv1.dtype), dconv2.to(conv2.dtype), dD, dB, dR, dT, dW, None, None, None, None, None
 
 
 class _KeyframeBuildFn(torch.autograd.Function):
@@ -279,17 +279,18 @@ class _GradFixedConcatFn(torch.autograd.Function):
 
 
 class _ResampleFn(torch.autograd.Function):
-    """tf.contrib.resampler.resampler w.r.t. the map (the points are constants on this path)."""
+    """tf.contrib.resampler.resampler w.r.t. the map (the points are constants on this path).  A bfloat16 map samples to bfloat16
+    (banet_resample_bf16); its gradient is taken in fp32 (banet_resample_bwd) and cast to bfloat16 once."""
 
     @staticmethod
     def forward(ctx, data, xy, coord_scale):
-        ctx.save_for_backward(xy); ctx.cs = float(coord_scale); ctx.hw = (data.shape[1], data.shape[2])
+        ctx.save_for_backward(xy); ctx.cs = float(coord_scale); ctx.hw = (data.shape[1], data.shape[2]); ctx.dtype = data.dtype
         return ops.resample(data, xy, coord_scale)
 
     @staticmethod
     def backward(ctx, dout):
         (xy,) = ctx.saved_tensors
-        return ops.resample_bwd(dout.contiguous(), xy, ctx.cs, ctx.hw[0], ctx.hw[1]), None, None
+        return ops.resample_bwd(dout.float().contiguous(), xy, ctx.cs, ctx.hw[0], ctx.hw[1]).to(ctx.dtype), None, None
 
 
 class _DepthComposeFn(torch.autograd.Function):
@@ -324,7 +325,8 @@ def iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regular
                     precision: int = 0, grid=None, return_status: bool = False):
     """One differentiable LM iteration on the fused kernels.  Same arguments / returns as `iteration`; an F2-only conv2 [nb,h,w,C] goes
     straight into the build and its backward (the gradient stencil's adjoint runs inside banet_lm_build_bwd).
-    precision: contraction mode of the FORWARD build (the backward is fp32); default FP32_SIMT, the reference's arithmetic type."""
+    precision: contraction mode of the FORWARD build (the backward is fp32); default FP32_SIMT, the reference's arithmetic type.
+    conv1 / conv2 may be bfloat16 (both): they are read as they are, and their gradients come back in bfloat16."""
     nb, N, C = conv1.shape
     bundle = B is not None
     H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, W, intr.detach(), p.detach(), precision, exact_sym, grid)
@@ -418,6 +420,9 @@ def _keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, 
     from . import _lib
     if precision not in (_lib.PREC_AUTO, _lib.PREC_FP32_SIMT):
         raise _lib.BanetError(f"precision {precision}: the keyframe build is fp32 SIMT only (AUTO or FP32_SIMT)")
+    if conv1.dtype != torch.float32 or conv2.dtype != torch.float32:
+        raise _lib.BanetError(f"the keyframe form takes float32 features only (conv1 {conv1.dtype}, conv2 {conv2.dtype}); give the keyframe "
+                              "tensors per frame ([nw,nf,...] or [nw,1,...]) to use bfloat16 features")
     nw, nf = R.shape[0], R.shape[1]
     K = B.shape[-1]
     nb = nw * nf

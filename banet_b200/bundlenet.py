@@ -113,6 +113,8 @@ class BundleNet(torch.nn.Module):
             if self.vmatrix_batch_scramble:
                 raise RuntimeError("vmatrix_batch_scramble=True (the reference's batch-interleaved VMatrix, bundlenet.py:45) is not differentiable here")
             if self.training_path == "reference_split":
+                if conv1.dtype != torch.float32 or conv2.dtype != torch.float32:
+                    raise RuntimeError("training_path='reference_split' takes float32 features; bfloat16 features train on the fused path")
                 Rn, Tn, Wn = _ag.iteration(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base if bundle else None,
                                            exact_sym=self.exact_sym_grad)
                 return Rn, Tn, Wn, None
@@ -202,8 +204,9 @@ class BundleNet(torch.nn.Module):
     def _keyframe_batch_iteration(self, conv1, conv2, intr, p, D, B, R, T, W, base, level):
         """WindowIteration on nw windows with the keyframe tensors once per window (conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K]):
         the keyframe build (banet_lm_keyframe_*), fused autograd path when gradients are recorded, else one iteration of
-        ops.lm_keyframe_run.  fp32 SIMT only: a TF32 precision raises."""
+        ops.lm_keyframe_run.  fp32 SIMT only: a TF32 precision raises, and so do bfloat16 features."""
         self._require_keyframe_precision()
+        self._require_keyframe_features(conv1, conv2)
         nw, nf = R.shape[0], R.shape[1]
         if self._wants_grad(conv1, conv2, D, B, R, T, W):
             if self.training_path == "reference_split":
@@ -217,6 +220,12 @@ class BundleNet(torch.nn.Module):
                                                  mlp_packed=[self.mlp_packed(str(level))], l2_regularizer_base=base, precision=self.precision)
         self._check_status(status.reshape(nw, nf))
         return Rn.reshape(nw, nf, 3, 3), Tn.reshape(nw, nf, 3, 1), Wn
+
+    @staticmethod
+    def _require_keyframe_features(*features) -> None:
+        if any(t.dtype != torch.float32 for t in features):
+            raise RuntimeError("the keyframe form of WindowIteration / WindowResize takes float32 features only; give the keyframe tensors per "
+                               "frame ([nw,1|nf,...]) to WindowIteration for bfloat16 features")
 
     def _require_keyframe_precision(self) -> None:
         if self.precision not in (_lib.PREC_AUTO, _lib.PREC_FP32_SIMT):
@@ -234,9 +243,19 @@ class BundleNet(torch.nn.Module):
                             geo.fy_num * k[:, 3] / geo.fy_den - geo.oy_sub], dim=1).contiguous()
         return _points.detach(), intr.detach()
 
+    @staticmethod
+    def _swapped_f2(layer: Tensor, gfc):
+        """conv2 of bundlenet.py:386-389: the half-swapped pyramid level.  float32: [F2|gx|gy] by grad_fixed_concat (one fused pass); bfloat16:
+        the half-swapped F2 only, whose gradient channels the build derives on the fly (no fp32 3C copy)."""
+        if layer.dtype == torch.bfloat16:
+            h = layer.shape[0] // 2
+            return torch.cat([layer[h:], layer[:h]]).contiguous()
+        return gfc(layer, swap_halves=True)
+
     def CameraResize(self, intrisic, layers, points, _depths, reuse_variables=False):
         """reference bundlenet.py:280-329 -> (rotations, translations), levels 0..3 x 1 iteration.  Differentiable w.r.t. the feature
-        pyramid and the lambda-MLP parameters when gradients are being recorded (the depth is stop_gradient'ed, :288)."""
+        pyramid and the lambda-MLP parameters when gradients are being recorded (the depth is stop_gradient'ed, :288).
+        `layers` may be bfloat16 (an autocast encoder's pyramid): conv1 is then the bfloat16 resample and conv2 the half-swapped F2 only."""
         nb = layers[-1].shape[0]
         _points, intr = self._prepare(intrisic, points)
         grad = self._wants_grad(*layers)
@@ -249,7 +268,7 @@ class BundleNet(torch.nn.Module):
         for level in range(0, 4):
             scale = 2 ** (3 - level)
             layer1 = resample(layers[level], _points, 1.0 / scale)             # :320
-            layer2 = gfc(layers[level], swap_halves=True)                      # :321-324
+            layer2 = self._swapped_f2(layers[level], gfc)                      # :321-324
             R, T, _, _ = self._iterate(layer1, layer2, intr / scale, p, d, None, R, T, None, 1.0, level)
             rotations.append(R); translations.append(T)
         return rotations, translations
@@ -258,7 +277,9 @@ class BundleNet(torch.nn.Module):
                      reuse_variables=False):
         """reference bundlenet.py:332-399 -> (output_rotations, output_translations, output_depths), levels 2,3.  Differentiable w.r.t.
         the feature pyramid, the basis, the initial pose and the lambda-MLP parameters when gradients are being recorded
-        (init_depth enters the LM only through stop_gradient, :341, and the output depth directly, :397)."""
+        (init_depth enters the LM only through stop_gradient, :341, and the output depth directly, :397).
+        `layers` may be bfloat16 (an autocast encoder's pyramid): conv1 is then the bfloat16 resample and conv2 the half-swapped F2 only;
+        their gradients come back in bfloat16.  basis and init_depth stay float32."""
         nb = layers[-1].shape[0]
         K = basis.shape[-1]
         _points, intr = self._prepare(intrisic, points)
@@ -276,7 +297,7 @@ class BundleNet(torch.nn.Module):
         for level in range(2, 4):                                              # :376
             scale = 2 ** (3 - level)
             layer1 = resample(layers[level], _points, 1.0 / scale)             # :385
-            layer2 = gfc(layers[level], swap_halves=True)                      # :386-389
+            layer2 = self._swapped_f2(layers[level], gfc)                      # :386-389
             R, T, W, _ = self._iterate(layer1, layer2, intr / scale, p, d, b, R, T, W, 1000.0, level)   # :393
             Rs.append(R); Ts.append(T)
             depth = compose(init_depth.reshape(nb, -1), basis.reshape(nb, -1, K), W)   # :397
@@ -295,10 +316,11 @@ class BundleNet(torch.nn.Module):
         No gradients recorded: one ops.lm_keyframe_run iteration per level on the frames' F2 maps as they are.  Gradients recorded: the keyframe
         form of autograd.window_batch_iteration_fused per level on [F2|gx|gy] (the keyframe backward takes that layout only); gradients reach
         both pyramids, the basis, the initial pose and the lambda-MLP parameters, init_depth through the output depth only (:341, :397).
-        AUTO or FP32_SIMT only, like the keyframe form of WindowIteration."""
+        AUTO or FP32_SIMT and float32 pyramids only, like the keyframe form of WindowIteration."""
         if self.vmatrix_batch_scramble:
             raise RuntimeError("vmatrix_batch_scramble=True is a 2-view quirk (bundlenet.py:45); the window solve has per-frame VMatrix only")
         self._require_keyframe_precision()
+        self._require_keyframe_features(*key_layers, *frame_layers)
         nw, nf, K = self._window_resize_shapes(intrisic, key_layers, frame_layers, points, basis, init_depth, init_rotation, init_translation)
         _points, intr = self._prepare(intrisic, points)
         grad = self._wants_grad(*key_layers, *frame_layers, basis, init_rotation, init_translation)

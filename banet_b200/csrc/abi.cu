@@ -30,6 +30,8 @@ static int check_level(const banet_level_t* lv, const char* who)
     BANET_REQUIRE(lv->conv2_channels == 3 * lv->C || lv->conv2_channels == lv->C, BANET_ERR_BAD_ARG,
                   "%s: conv2_channels=%d must be 3*C (reference layout) or C (F2 only)", who, lv->conv2_channels);
     BANET_REQUIRE(lv->conv1 && lv->conv2 && lv->intr && lv->p && lv->D, BANET_ERR_BAD_ARG, "%s: null tensor", who);
+    BANET_REQUIRE(lv->feature_dtype == BANET_DTYPE_F32 || lv->feature_dtype == BANET_DTYPE_BF16, BANET_ERR_BAD_ARG,
+                  "%s: feature_dtype=%d must be BANET_DTYPE_F32 (0) or BANET_DTYPE_BF16 (1)", who, lv->feature_dtype);
     BANET_REQUIRE(lv->K == 0 || lv->B, BANET_ERR_BAD_ARG, "%s: K=%d but B is null", who, lv->K);
     BANET_REQUIRE((long long)lv->h * lv->w * lv->conv2_channels < (1LL << 40), BANET_ERR_BAD_ARG, "%s: map too large", who);
     BANET_REQUIRE((lv->grid_w == 0 && lv->grid_h == 0) || (lv->grid_w > 0 && lv->grid_h > 0 && (long long)lv->grid_w * lv->grid_h == lv->N),
@@ -705,6 +707,8 @@ extern "C" int banet_lm_track_legacy(const banet_level_t* levels, int nlevels, c
     for (int l = 0; l < nlevels; ++l) {
         int rc = check_level(&levels[l], "lm_track_legacy");
         if (rc) return rc;
+        BANET_REQUIRE(levels[l].feature_dtype == BANET_DTYPE_F32, BANET_ERR_UNSUPPORTED,
+                      "lm_track_legacy: level %d has bf16 features; the legacy tracker takes fp32 features only", l);
         BANET_REQUIRE(levels[l].K == 0 && levels[l].nb == levels[0].nb && levels[l].conv2_channels == 3 * levels[l].C && level_iters[l] >= 0, BANET_ERR_BAD_ARG,
                       "lm_track_legacy: level %d must be pose-only (K=0) with the [F2|gx|gy] layout and the same batch size", l);
     }

@@ -15,6 +15,7 @@
 // (one CTA per SM); each CTA keeps its accumulators in registers across tiles and writes ONE partial
 // slot per pair it touches; lm_reduce_kernel sums the slots in a fixed order (deterministic, no atomics).
 #include "common.cuh"
+#include "features.cuh"
 #include "lm_build.h"
 
 namespace banet {
@@ -51,7 +52,8 @@ __device__ __forceinline__ int reflect_idx(int i, int n) {      // tf.pad REFLEC
 }
 
 // ---- S2 helper: accumulate one group of VEC channels of one pixel ------------------------------
-template <int VEC> struct ChanVec;
+// TF: element type of the feature loads (float, or bf16 widened exactly on load); the |diff| sums in smem are always fp32
+template <int VEC, typename TF = float> struct ChanVec;
 template <> struct ChanVec<4> {
     float v[4];
     __device__ __forceinline__ void load(const float* p) { float4 t = __ldg(reinterpret_cast<const float4*>(p)); v[0]=t.x; v[1]=t.y; v[2]=t.z; v[3]=t.w; }
@@ -66,8 +68,19 @@ template <> struct ChanVec<1> {
     __device__ __forceinline__ void load_smem(const float* p) { v[0] = p[0]; }
     __device__ __forceinline__ void store_smem(float* p) const { p[0] = v[0]; }
 };
+template <> struct ChanVec<4, bf16> {
+    float v[4];
+    __device__ __forceinline__ void set(uint2 t) { v[0] = bf16_lo(t.x); v[1] = bf16_hi(t.x); v[2] = bf16_lo(t.y); v[3] = bf16_hi(t.y); }
+    __device__ __forceinline__ void load(const bf16* p) { set(__ldg(reinterpret_cast<const uint2*>(p))); }
+    __device__ __forceinline__ void load_stream(const bf16* p) { set(ld_stream_bf4(p)); }
+};
+template <> struct ChanVec<1, bf16> {
+    float v[1];
+    __device__ __forceinline__ void load(const bf16* p) { v[0] = ldg_feat(p); }
+    __device__ __forceinline__ void load_stream(const bf16* p) { v[0] = ld_stream_bf1(p); }
+};
 
-template <int KP, int VEC>
+template <int KP, int VEC, typename TF>
 __global__ void __launch_bounds__(BUILD_THREADS, (KP >= 128) ? 1 : 2)
 lm_build_kernel(const BuildParams prm)
 {
@@ -246,19 +259,20 @@ lm_build_kernel(const BuildParams prm)
                 const float dx = rec[R_DX * TILE_PX + n], dy = rec[R_DY * TILE_PX + n];
                 const int x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
                 const float w00 = (1.f - dx) * (1.f - dy), w01 = dx * (1.f - dy), w10 = (1.f - dx) * dy, w11 = dx * dy;
-                const float* img = prm.conv2 + (size_t)b * h * w * c2;
-                const float* t00 = img + ((size_t)y0 * w + x0) * c2;
-                const float* t01 = img + ((size_t)y0 * w + x1) * c2;
-                const float* t10 = img + ((size_t)y1 * w + x0) * c2;
-                const float* t11 = img + ((size_t)y1 * w + x1) * c2;
-                const float* c1 = prm.conv1 + ((size_t)b * N + n0 + n) * C;
+                const TF* img = static_cast<const TF*>(prm.conv2) + (size_t)b * h * w * c2;
+                const TF* t00 = img + ((size_t)y0 * w + x0) * c2;
+                const TF* t01 = img + ((size_t)y0 * w + x1) * c2;
+                const TF* t10 = img + ((size_t)y1 * w + x0) * c2;
+                const TF* t11 = img + ((size_t)y1 * w + x1) * c2;
+                const TF* c1 = static_cast<const TF*>(prm.conv1) + ((size_t)b * N + n0 + n) * C;
                 float* myRb = sRb + warp * C;
                 for (int c = lane * VEC; c < C; c += 32 * VEC) {
-                    ChanVec<VEC> f1, a00, a01, a10, a11, gx, gy;
+                    ChanVec<VEC, TF> f1, a00, a01, a10, a11;
+                    ChanVec<VEC> gx, gy;
                     f1.load_stream(c1 + c);
                     a00.load(t00 + c); a01.load(t01 + c); a10.load(t10 + c); a11.load(t11 + c);
                     if (!fly_grad) {
-                        ChanVec<VEC> g00, g01, g10, g11;
+                        ChanVec<VEC, TF> g00, g01, g10, g11;
                         g00.load(t00 + C + c); g01.load(t01 + C + c); g10.load(t10 + C + c); g11.load(t11 + C + c);
 #pragma unroll
                         for (int u = 0; u < VEC; ++u) gx.v[u] = w00 * g00.v[u] + w01 * g01.v[u] + w10 * g10.v[u] + w11 * g11.v[u];
@@ -274,7 +288,7 @@ lm_build_kernel(const BuildParams prm)
 #pragma unroll
                         for (int tp = 0; tp < 4; ++tp) {
                             const int xx = xs[tp & 1], yy = ys[tp >> 1];
-                            ChanVec<VEC> e, wv, s, nn;
+                            ChanVec<VEC, TF> e, wv, s, nn;
                             e.load(img + ((size_t)yy * w + reflect_idx(xx + 1, w)) * c2 + c);
                             wv.load(img + ((size_t)yy * w + reflect_idx(xx - 1, w)) * c2 + c);
                             s.load(img + ((size_t)reflect_idx(yy + 1, h) * w + xx) * c2 + c);
@@ -482,11 +496,11 @@ int build_plan(const banet_level_t* lv, int num_sms, BuildPlan* plan)
     return BANET_OK;
 }
 
-template <int KP, int VEC>
+template <int KP, int VEC, typename TF>
 static int launch_build(const BuildParams& prm, int grid, cudaStream_t st)
 {
     const size_t smem = BuildSmem<KP>::bytes(prm.C);
-    auto kern = lm_build_kernel<KP, VEC>;
+    auto kern = lm_build_kernel<KP, VEC, TF>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("lm_build: smem attr (%zu B): %s", smem, cudaGetErrorString(e)); return BANET_ERR_CUDA; }
     kern<<<grid, BUILD_THREADS, smem, st>>>(prm);
@@ -506,11 +520,13 @@ int lm_build_simt(const banet_level_t* lv, const BuildPlan& plan, const float* R
     prm.tiles_per_pair = plan.tiles_per_pair; prm.total_tiles = plan.total_tiles;
     prm.kq_i = 0; prm.kq_j = 0;
     prm.grid_w = 0; prm.grid_h = 0; prm.tiles_x = 0; prm.tiles_y = 0; prm.band_rows = 1; prm.l2_hints = 0; prm.tap_prefetch = 0; prm.hdd_transposed = 0; prm.force_direct = 0; prm.trace = nullptr;
+    const bool bf = lv->feature_dtype == BANET_DTYPE_BF16;
     const bool vec4 = (lv->C % 4 == 0) && (lv->conv2_channels % 4 == 0) &&
-                      ((reinterpret_cast<uintptr_t>(lv->conv1) | reinterpret_cast<uintptr_t>(lv->conv2)) % 16 == 0);
+                      ((reinterpret_cast<uintptr_t>(lv->conv1) | reinterpret_cast<uintptr_t>(lv->conv2)) % (bf ? 8 : 16) == 0);
     int rc;
-#define BANET_DISPATCH(KPV)                                                            \
-    rc = vec4 ? launch_build<KPV, 4>(prm, plan.grid, st) : launch_build<KPV, 1>(prm, plan.grid, st)
+#define BANET_DISPATCH(KPV)                                                                                                    \
+    rc = bf ? (vec4 ? launch_build<KPV, 4, bf16>(prm, plan.grid, st) : launch_build<KPV, 1, bf16>(prm, plan.grid, st))       \
+            : (vec4 ? launch_build<KPV, 4, float>(prm, plan.grid, st) : launch_build<KPV, 1, float>(prm, plan.grid, st))
     switch (plan.KP) {
         case 0:   BANET_DISPATCH(0); break;
         case 16:  BANET_DISPATCH(16); break;

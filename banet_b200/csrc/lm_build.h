@@ -6,7 +6,8 @@ namespace banet {
 
 struct BuildParams {
     int nb, N, C, K, h, w, c2;
-    const float *conv1, *conv2, *intr, *p, *D, *B, *R, *T, *W;
+    const void *conv1, *conv2;        // element type: the level's feature_dtype (the kernels' TF template parameter)
+    const float *intr, *p, *D, *B, *R, *T, *W;
     float* partials;
     int slot_floats, max_span, tiles_per_pair;
     long long total_tiles;

@@ -17,6 +17,7 @@
 //              rready R (A_lo, R_lo) of the tile written | rfree MMAs of the tile done (R, A_lo and the A stage reusable) |
 //              rbdump/rbfree gather<->algebra hand-over of the |diff| sums at a pair change.
 #include "common.cuh"
+#include "features.cuh"
 #include "lm_build.h"
 #include "tc_utils.cuh"
 #include "mma_role.cuh"
@@ -100,7 +101,138 @@ __device__ __forceinline__ TileCoord tile_coord(const BuildParams& prm, long lon
     return tc;
 }
 
-template <int NCH, bool FLY, int MODE, int KBLK = 4>
+// ---- gather warps on bf16 features --------------------------------------------------------------------------------------------------
+// Half-warp per pixel as for fp32; lane hl holds channels CPL*hl .. CPL*hl + CPL-1 (CPL = C/16), so each of the 13 taps is one 16-B
+// (C = 128) or 8-B (C = 64) load.  At C = 64 this is the fp32 lane map and channel order (results bitwise equal to fp32 on the widened
+// maps); at C = 128 a lane's 8 channels are contiguous instead of two groups of 4 64 apart, which reorders the per-pixel channel sums.
+template <int CPL> struct BfTap;
+template <> struct BfTap<8> {
+    using T = uint4;
+    static __device__ __forceinline__ T ld(const bf16* p, uint64_t pol) {
+        T r; asm("ld.global.nc.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p), "l"(pol)); return r; }
+    static __device__ __forceinline__ T ld_stream(const bf16* p, uint64_t pol) {
+        T r; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                          : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p), "l"(pol)); return r; }
+    static __device__ __forceinline__ float ch(const T& v, int i) {
+        const uint32_t u = (i >> 1) == 0 ? v.x : (i >> 1) == 1 ? v.y : (i >> 1) == 2 ? v.z : v.w;
+        return (i & 1) ? bf16_hi(u) : bf16_lo(u);
+    }
+};
+template <> struct BfTap<4> {
+    using T = uint2;
+    static __device__ __forceinline__ T ld(const bf16* p, uint64_t pol) {
+        T r; asm("ld.global.nc.L2::cache_hint.v2.u32 {%0,%1}, [%2], %3;" : "=r"(r.x), "=r"(r.y) : "l"(p), "l"(pol)); return r; }
+    static __device__ __forceinline__ T ld_stream(const bf16* p, uint64_t pol) {
+        T r; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u32 {%0,%1}, [%2], %3;" : "=r"(r.x), "=r"(r.y) : "l"(p), "l"(pol)); return r; }
+    static __device__ __forceinline__ float ch(const T& v, int i) {
+        const uint32_t u = (i >> 1) == 0 ? v.x : v.y;
+        return (i & 1) ? bf16_hi(u) : bf16_lo(u);
+    }
+};
+
+template <int NCH, bool FLY, int NREC>
+__device__ __forceinline__ void gather_bf16(const BuildParams& prm, const int* sTile, float* sRec, float* sRbs, uint64_t* recs, uint64_t* gath,
+                                            uint64_t* rbdump, uint64_t* rbfree, int ntiles, int g, int lane)
+{
+    constexpr int C = 64 * NCH, CPL = C / 16, PXW = TILE / GW;
+    using TB = BfTap<CPL>;
+    const int hw = lane >> 4, hl = lane & 15;
+    const int N = prm.N, h = prm.h, w = prm.w, c2 = prm.c2;
+    float rb[CPL];
+#pragma unroll
+    for (int u = 0; u < CPL; ++u) rb[u] = 0.f;
+    typename TB::T tb[13];
+    int cur_b = -1, ndump = 0;
+    const uint64_t pol_stream = prm.l2_hints >= 1 ? l2_policy_evict_first() : l2_policy_evict_normal();
+    const uint64_t pol_tap = prm.l2_hints >= 2 ? l2_policy_evict_last() : l2_policy_evict_normal();
+
+    auto dump_rb = [&]() {
+        if (ndump > 0) mbar_wait_parked(rbfree, (ndump - 1) & 1);
+#pragma unroll
+        for (int u = 0; u < CPL; ++u) rb[u] += __shfl_xor_sync(0xffffffffu, rb[u], 16);
+        if (hw == 0) {
+#pragma unroll
+            for (int j = 0; j < CPL / 4; ++j)
+                *reinterpret_cast<float4*>(sRbs + g * 128 + CPL * hl + 4 * j) = make_float4(rb[4 * j], rb[4 * j + 1], rb[4 * j + 2], rb[4 * j + 3]);
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(rbdump);
+#pragma unroll
+        for (int u = 0; u < CPL; ++u) rb[u] = 0.f;
+        ++ndump;
+    };
+
+    for (int j = 0; j < ntiles; ++j) {
+        const int s = j % NREC;
+        mbar_wait_parked(&recs[s], (j / NREC) & 1);
+        const int b = sTile[s * 4];
+        if (b != cur_b) { if (cur_b >= 0) dump_rb(); cur_b = b; }
+        float* rec = sRec + (s * TILE + g * PXW) * REC;
+        const bf16* c1b = static_cast<const bf16*>(prm.conv1) + (size_t)b * N * C + CPL * hl;
+        const bf16* img = static_cast<const bf16*>(prm.conv2) + (size_t)b * h * w * c2 + CPL * hl;
+#pragma unroll
+        for (int u = 0; u < PXW / 2; ++u) {
+            const int pl = 2 * u + hw;
+            const float mask = rec[pl * REC + 4];
+            float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f;
+            if (mask != 0.f) {
+                const uint4 o = *reinterpret_cast<const uint4*>(rec + pl * REC);
+                const int n = __float_as_int(rec[pl * REC + 11]);
+                auto ldt = [&](const bf16* q) { return TB::ld(q, pol_tap); };
+                tb[0] = TB::ld_stream(c1b + (size_t)n * C, pol_stream);
+                if constexpr (!FLY) {
+                    const bf16* t00 = img + o.x; const bf16* t01 = img + o.y; const bf16* t10 = img + o.z; const bf16* t11 = img + o.w;
+                    tb[1] = ldt(t00); tb[2] = ldt(t01); tb[3] = ldt(t10); tb[4] = ldt(t11);
+                    tb[5] = ldt(t00 + C); tb[6] = ldt(t01 + C); tb[7] = ldt(t10 + C); tb[8] = ldt(t11 + C);
+                    tb[9] = ldt(t00 + 2 * C); tb[10] = ldt(t01 + 2 * C); tb[11] = ldt(t10 + 2 * C); tb[12] = ldt(t11 + 2 * C);
+                } else {
+                    const uint2 cxy = *reinterpret_cast<const uint2*>(rec + pl * REC + 14);
+                    const bf16* rm = img + o.x; const bf16* r0 = img + o.y; const bf16* r1 = img + o.z; const bf16* rp = img + o.w;
+                    const uint32_t oM = (cxy.x & 0xffffu) * c2, o0 = (cxy.x >> 16) * c2, o1 = (cxy.y & 0xffffu) * c2, oP = (cxy.y >> 16) * c2;
+                    tb[1] = ldt(r0 + oM); tb[2] = ldt(r0 + o0); tb[3] = ldt(r0 + o1); tb[4] = ldt(r0 + oP);      // aM0 a00 a10 aP0
+                    tb[5] = ldt(r1 + oM); tb[6] = ldt(r1 + o0); tb[7] = ldt(r1 + o1); tb[8] = ldt(r1 + oP);      // aM1 a01 a11 aP1
+                    tb[9] = ldt(rm + o0); tb[10] = ldt(rm + o1); tb[11] = ldt(rp + o0); tb[12] = ldt(rp + o1);   // a0m a1m a0p a1p
+                }
+                const float2 dxy = *reinterpret_cast<const float2*>(rec + pl * REC + 12);
+                const float dx = dxy.x, dy = dxy.y;
+                const float w00 = (1.f - dx) * (1.f - dy), w01 = dx * (1.f - dy), w10 = (1.f - dx) * dy, w11 = dx * dy;
+                const float h00 = 0.5f * w00, h01 = 0.5f * w01, h10 = 0.5f * w10, h11 = 0.5f * w11;
+#pragma unroll
+                for (int i = 0; i < CPL; ++i) {
+                    float t[13];
+#pragma unroll
+                    for (int k = 0; k < 13; ++k) t[k] = TB::ch(tb[k], i);
+                    float f2, gx, gy;
+                    if constexpr (!FLY) {
+                        f2 = w00 * t[1] + w01 * t[2] + w10 * t[3] + w11 * t[4];
+                        gx = w00 * t[5] + w01 * t[6] + w10 * t[7] + w11 * t[8];
+                        gy = w00 * t[9] + w01 * t[10] + w10 * t[11] + w11 * t[12];
+                    } else {
+                        f2 = w00 * t[2] + w01 * t[3] + w10 * t[6] + w11 * t[7];
+                        gx = h00 * (t[3] - t[1]) + h01 * (t[4] - t[2]) + h10 * (t[7] - t[5]) + h11 * (t[8] - t[6]);
+                        gy = h00 * (t[6] - t[9]) + h10 * (t[11] - t[2]) + h01 * (t[7] - t[10]) + h11 * (t[12] - t[3]);
+                    }
+                    const float d = t[0] - f2;
+                    m11 = fmaf(gx, gx, m11); m12 = fmaf(gx, gy, m12); m22 = fmaf(gy, gy, m22);
+                    q1 = fmaf(gx, d, q1); q2 = fmaf(gy, d, q2);
+                    rb[i] += fabsf(d);
+                }
+            }
+            m11 = hsum16(m11); m12 = hsum16(m12); m22 = hsum16(m22); q1 = hsum16(q1); q2 = hsum16(q2);
+            if (hl == 0) {           // totals overwrite dx,dy / n of this pixel's record (as the fp32 gather does)
+                *reinterpret_cast<float4*>(rec + pl * REC + 12) = make_float4(m11, m12, m22, q1);
+                rec[pl * REC + 11] = q2;
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&gath[s]);
+    }
+    if (cur_b >= 0) dump_rb();
+}
+
+// TF: feature element type (float or bf16).  bf16 keeps the half-warp per pixel; each tap is ONE load of the lane's C/16 channels
+// (16 B of 8 channels at C = 128, 8 B of 4 at C = 64), widened channel by channel where it is used.
+template <int NCH, bool FLY, int MODE, int KBLK = 4, typename TF = float>
 __global__ void __launch_bounds__(THREADS, 1)
 lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams prm)
 {
@@ -181,7 +313,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                         if (gy < prm.grid_h && tn.tx0 < prm.grid_w) {
                             const size_t n = (size_t)gy * prm.grid_w + tn.tx0;
                             const int wpx = min(8, prm.grid_w - tn.tx0);
-                            prefetch_l2_bulk(prm.conv1 + ((size_t)tn.b * N + n) * C, (uint32_t)(wpx * C * 4));
+                            prefetch_l2_bulk(static_cast<const TF*>(prm.conv1) + ((size_t)tn.b * N + n) * C, (uint32_t)(wpx * C * sizeof(TF)));
                             if ((n & 3) == 0 && (N & 3) == 0) {
                                 const uint32_t by = (uint32_t)(((wpx * 4) + 15) & ~15);
                                 prefetch_l2_bulk(prm.D + (size_t)tn.b * N + n, by);
@@ -191,7 +323,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                         }
                     }
                 } else if (lane == 0) {
-                    prefetch_l2_bulk(prm.conv1 + ((size_t)tn.b * N + tn.n0) * C, (uint32_t)(tn.cnt * C * 4));
+                    prefetch_l2_bulk(static_cast<const TF*>(prm.conv1) + ((size_t)tn.b * N + tn.n0) * C, (uint32_t)(tn.cnt * C * sizeof(TF)));
                     if ((N & 3) == 0) {
                         const uint32_t by = (uint32_t)(((tn.cnt * 4) + 15) & ~15);
                         prefetch_l2_bulk(prm.D + (size_t)tn.b * N + tn.n0, by);
@@ -294,11 +426,11 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                     // pull this pixel's share of the tile's tap footprint into L2 one to two tiles before the gather warps load it: the gather is
                     // bound by the latency of its 13 dependent-free loads, not by their count.  Interior pixels fetch their (x0, y0) texel only;
                     // the tile's border pixels add the halo, so that under a near-unit warp every texel is requested about once.
-                    const float* imgp = prm.conv2 + (size_t)b * h * w * c2;
+                    const TF* imgp = static_cast<const TF*>(prm.conv2) + (size_t)b * h * w * c2;
                     const int px = nlr & 7, py = nlr >> 3;
                     const bool edge_x = !grid2d || px == 7, edge_y = !grid2d || py == 7 || prm.tap_prefetch == 2;
                     if constexpr (!FLY) {
-                        const uint32_t by = (uint32_t)c2 * 4u;
+                        const uint32_t by = (uint32_t)c2 * (uint32_t)sizeof(TF);
                         prefetch_l2_bulk(imgp + o[0], by);
                         if (edge_x && o[1] != o[0]) prefetch_l2_bulk(imgp + o[1], by);
                         if (edge_y && o[2] != o[0]) {
@@ -308,7 +440,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                     } else {
                         const bool first_x = !grid2d || px == 0, first_y = !grid2d || py == 0;
                         const int xs = max(x0 - (first_x ? 1 : 0), 0), xe = min(x0 + (edge_x ? 2 : 0), w - 1);
-                        const uint32_t by = (uint32_t)(xe - xs + 1) * (uint32_t)c2 * 4u;
+                        const uint32_t by = (uint32_t)(xe - xs + 1) * (uint32_t)c2 * (uint32_t)sizeof(TF);
                         prefetch_l2_bulk(imgp + ((size_t)y0 * w + xs) * c2, by);
                         if (first_y && y0 > 0) prefetch_l2_bulk(imgp + ((size_t)(y0 - 1) * w + xs) * c2, by);
                         if (edge_y) {
@@ -331,6 +463,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
     } else if (warp < W0 + GW) {
         // ===================================================================== gather warps: records -> taps -> M, q
         setmaxnreg_inc<112>();
+        if constexpr (sizeof(TF) == 2) { gather_bf16<NCH, FLY, NREC>(prm, sTile, sRec, sRbs, recs, gath, rbdump, rbfree, ntiles, warp - W0, lane); return; }
         const int g = warp - W0, hw = lane >> 4, hl = lane & 15;
         constexpr int PXW = TILE / GW;                       // 8 pixels per warp and tile
         constexpr int NUNIT = (PXW / 2) * NCH;
@@ -368,8 +501,8 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
             const int b = sTile[s * 4];
             if (b != cur_b) { if (cur_b >= 0) dump_rb(); cur_b = b; }
             float* rec = sRec + (s * TILE + g * PXW) * REC;
-            const float* c1b = prm.conv1 + (size_t)b * N * C + 4 * hl;
-            const float* imgb = prm.conv2 + (size_t)b * h * w * c2 + 4 * hl;
+            const float* c1b = static_cast<const float*>(prm.conv1) + (size_t)b * N * C + 4 * hl;
+            const float* imgb = static_cast<const float*>(prm.conv2) + (size_t)b * h * w * c2 + 4 * hl;
 #pragma unroll
             for (int u = 0; u < NUNIT; ++u) {
                 const int pl = 2 * (u / NCH) + hw, co = 64 * (u % NCH), jc = u % NCH;
@@ -590,10 +723,10 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
     }
 }
 
-template <int NCH, bool FLY, int MODE, int KBLK = 4>
+template <int NCH, bool FLY, int MODE, int KBLK = 4, typename TF = float>
 static int launch6(const CUtensorMap& tm, const BuildParams& prm, int grid, cudaStream_t st)
 {
-    auto kern = lm_build_tc6_kernel<NCH, FLY, MODE, KBLK>;
+    auto kern = lm_build_tc6_kernel<NCH, FLY, MODE, KBLK, TF>;
     const int smem = Smem<MODE, FLY>::bytes;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { set_error("lm_build_tc6: smem attr (%d B): %s", smem, cudaGetErrorString(e)); return BANET_ERR_CUDA; }
@@ -601,24 +734,29 @@ static int launch6(const CUtensorMap& tm, const BuildParams& prm, int grid, cuda
     BANET_CUDA_LAUNCH_CHECK("lm_build_tc6_kernel launch");
     return BANET_OK;
 }
-template <int NCH, bool FLY>
+template <int NCH, bool FLY, typename TF>
 static int launch6_mode(int mode, int kblk, const CUtensorMap& tm, const BuildParams& prm, int grid, cudaStream_t st)
 {
     if (kblk != 4) {             // K = 64 / 32 (opt-in, BANET_TC_SMALLK=1): instantiated for the two-pass and the fp32-grade mode only
-        if (kblk == 2) return mode == 3 ? launch6<NCH, FLY, 3, 2>(tm, prm, grid, st) : launch6<NCH, FLY, 2, 2>(tm, prm, grid, st);
-        return mode == 3 ? launch6<NCH, FLY, 3, 1>(tm, prm, grid, st) : launch6<NCH, FLY, 2, 1>(tm, prm, grid, st);
+        if (kblk == 2) return mode == 3 ? launch6<NCH, FLY, 3, 2, TF>(tm, prm, grid, st) : launch6<NCH, FLY, 2, 2, TF>(tm, prm, grid, st);
+        return mode == 3 ? launch6<NCH, FLY, 3, 1, TF>(tm, prm, grid, st) : launch6<NCH, FLY, 2, 1, TF>(tm, prm, grid, st);
     }
-    if (mode == 1) return launch6<NCH, FLY, 1>(tm, prm, grid, st);
-    if (mode == 2) return launch6<NCH, FLY, 2>(tm, prm, grid, st);
-    return launch6<NCH, FLY, 3>(tm, prm, grid, st);
+    if (mode == 1) return launch6<NCH, FLY, 1, 4, TF>(tm, prm, grid, st);
+    if (mode == 2) return launch6<NCH, FLY, 2, 4, TF>(tm, prm, grid, st);
+    return launch6<NCH, FLY, 3, 4, TF>(tm, prm, grid, st);
+}
+template <typename TF>
+static int launch6_type(int mode, bool fly, int nch, int kblk, const CUtensorMap& tm, const BuildParams& prm, int grid, cudaStream_t st)
+{
+    if (nch == 2) return fly ? launch6_mode<2, true, TF>(mode, kblk, tm, prm, grid, st) : launch6_mode<2, false, TF>(mode, kblk, tm, prm, grid, st);
+    return fly ? launch6_mode<1, true, TF>(mode, kblk, tm, prm, grid, st) : launch6_mode<1, false, TF>(mode, kblk, tm, prm, grid, st);
 }
 
 }  // namespace v6
 
-int lm_build_tc6_launch(int mode, bool fly, int nch, int kblk, const CUtensorMap& tm, const BuildParams& prm, int grid, cudaStream_t st)
+int lm_build_tc6_launch(int mode, bool fly, int nch, int kblk, bool is_bf16, const CUtensorMap& tm, const BuildParams& prm, int grid, cudaStream_t st)
 {
-    if (nch == 2) return fly ? v6::launch6_mode<2, true>(mode, kblk, tm, prm, grid, st) : v6::launch6_mode<2, false>(mode, kblk, tm, prm, grid, st);
-    return fly ? v6::launch6_mode<1, true>(mode, kblk, tm, prm, grid, st) : v6::launch6_mode<1, false>(mode, kblk, tm, prm, grid, st);
+    return is_bf16 ? v6::launch6_type<bf16>(mode, fly, nch, kblk, tm, prm, grid, st) : v6::launch6_type<float>(mode, fly, nch, kblk, tm, prm, grid, st);
 }
 
 }  // namespace banet

@@ -238,7 +238,7 @@ lm_build_tc7_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_cons
                     if (gy < prm.grid_h && atx < prm.grid_w) {
                         const size_t n = (size_t)gy * prm.grid_w + atx;
                         const int wpx = min(8, prm.grid_w - atx);
-                        prefetch_l2_bulk(prm.conv1 + ((size_t)ab * N + n) * C, (uint32_t)(wpx * C * 4));
+                        prefetch_l2_bulk(static_cast<const float*>(prm.conv1) + ((size_t)ab * N + n) * C, (uint32_t)(wpx * C * 4));
                         if ((n & 3) == 0 && (N & 3) == 0) {
                             const uint32_t by = (uint32_t)(((wpx * 4) + 15) & ~15);
                             prefetch_l2_bulk(prm.D + (size_t)ab * N + n, by);
@@ -419,7 +419,7 @@ lm_build_tc7_kernel(const __grid_constant__ CUtensorMap tmapB, const __grid_cons
                 rM = (uint32_t)(ym * w * c2); r0 = (uint32_t)(y0 * w * c2); r1 = (uint32_t)(y1 * w * c2); rP = (uint32_t)(yp * w * c2);
                 oM = (uint32_t)(xm * c2 + 4 * ql); o0 = (uint32_t)(x0 * c2 + 4 * ql); o1 = (uint32_t)(x1 * c2 + 4 * ql); oP = (uint32_t)(xp * c2 + 4 * ql);
             }
-            const float* imgb = prm.conv2 + (size_t)b * h * w * c2;
+            const float* imgb = static_cast<const float*>(prm.conv2) + (size_t)b * h * w * c2;
             const uint32_t c1off = (uint32_t)(WIN_BYTES + pxi * 128 + ql * 16);
             u64 m11 = 0ull, m12 = 0ull, m22 = 0ull, q1 = 0ull, q2 = 0ull;        // packed (2 channels) sums of (2gx)^2, (2gx)(2gy), (2gy)^2, (2gx) d, (2gy) d
 #pragma unroll

@@ -17,6 +17,7 @@
 //   dH = dHt (1 + damp lambda on the diagonal), dlambda = sum_i dHt_ii damp_i (H_ii + eps); ddelta from the SE(3) update by forward-mode
 //   dual numbers over the same expressions as pose_update_kernel (lm_solve.cu).
 #include "common.cuh"
+#include "features.cuh"
 #include "lm_build.h"
 #include "pose_bwd.cuh"
 
@@ -29,7 +30,8 @@ constexpr int BWD_KL_MAX = 8;                    // K <= 32 * BWD_KL_MAX
 
 struct BwdParams {
     int nb, N, C, K, h, w;
-    const float *conv1, *conv2, *intr, *p, *D, *B, *R, *T, *W;
+    const void *conv1, *conv2;                   // element type: the kernel's TF (the level's feature_dtype)
+    const float *intr, *p, *D, *B, *R, *T, *W;
     const float *dH, *dg, *drbar;
     float *dconv1, *dconv2, *dD, *dB, *dR, *dT, *dW;
     int exact_sym, tiles_per_pair;
@@ -58,14 +60,15 @@ struct FlyTaps {
         }
     }
     // channel c of the tap values t, the tap x-gradients g and y-gradients k
-    __device__ __forceinline__ void load(const float* img, int w, int C, int c, float t[4], float g[4], float k[4]) const {
+    template <typename TF>
+    __device__ __forceinline__ void load(const TF* img, int w, int C, int c, float t[4], float g[4], float k[4]) const {
 #pragma unroll
         for (int tp = 0; tp < 4; ++tp) {
             const int xx = cx[tp & 1];
             const size_t row = (size_t)cy[tp >> 1] * w;
-            t[tp] = __ldg(img + (row + xx) * C + c);
-            g[tp] = 0.5f * (__ldg(img + (row + ex[tp & 1]) * C + c) - __ldg(img + (row + wx[tp & 1]) * C + c));
-            k[tp] = 0.5f * (__ldg(img + ((size_t)sy[tp >> 1] * w + xx) * C + c) - __ldg(img + ((size_t)ny[tp >> 1] * w + xx) * C + c));
+            t[tp] = ldg_feat(img + (row + xx) * C + c);
+            g[tp] = 0.5f * (ldg_feat(img + (row + ex[tp & 1]) * C + c) - ldg_feat(img + (row + wx[tp & 1]) * C + c));
+            k[tp] = 0.5f * (ldg_feat(img + ((size_t)sy[tp >> 1] * w + xx) * C + c) - ldg_feat(img + ((size_t)ny[tp >> 1] * w + xx) * C + c));
         }
     }
     // the adjoint of load for one channel: df on the values, dgx / dgy on the gradients, each tap weighted by wt
@@ -83,7 +86,8 @@ struct FlyTaps {
 };
 
 // smem layout (floats): S_dd [K][K] | S_cd [6][K] | S_dc [K][6] | S_cc [36] | ghat [P] | W [K] | pose [16] | rhat [C]
-template <int BWD_KL, int LAYOUT>
+// TF: feature element type (float or bf16, widened on load); dconv1 / dconv2 are fp32 for both
+template <int BWD_KL, int LAYOUT, typename TF>
 __global__ void __launch_bounds__(BWD_THREADS, 2)
 lm_build_bwd_kernel(const BwdParams prm)
 {
@@ -152,7 +156,7 @@ lm_build_bwd_kernel(const BwdParams prm)
             cur_b = b;
         }
         const float fx = sPose[12], fy = sPose[13], ox = sPose[14], oy = sPose[15];
-        const float* img = prm.conv2 + (size_t)b * h * w * C3;
+        const TF* img = static_cast<const TF*>(prm.conv2) + (size_t)b * h * w * C3;
         float* dimg = prm.dconv2 + (size_t)b * h * w * C3;
 
         for (int pi = warp; pi < cnt; pi += BWD_WARPS) {
@@ -191,7 +195,7 @@ lm_build_bwd_kernel(const BwdParams prm)
             const float dx = u - fu, dy = v - fv;
             const float w00 = (1.f - dx) * (1.f - dy), w01 = dx * (1.f - dy), w10 = (1.f - dx) * dy, w11 = dx * dy;
             const size_t o00 = ((size_t)y0 * w + x0) * C3, o01 = ((size_t)y0 * w + x1) * C3, o10 = ((size_t)y1 * w + x0) * C3, o11 = ((size_t)y1 * w + x1) * C3;
-            const float* c1 = prm.conv1 + gi * C;
+            const TF* c1 = static_cast<const TF*>(prm.conv1) + gi * C;
             // ---- pass 1: M = G^T G, q = G^T d (lanes over channels) ----------------------------------------------------------------
             float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f;
             for (int c = lane; c < C; c += 32) {
@@ -204,11 +208,11 @@ lm_build_bwd_kernel(const BwdParams prm)
                     gx = w00 * g[0] + w01 * g[1] + w10 * g[2] + w11 * g[3];
                     gy = w00 * k[0] + w01 * k[1] + w10 * k[2] + w11 * k[3];
                 } else {
-                    f2 = w00 * __ldg(img + o00 + c) + w01 * __ldg(img + o01 + c) + w10 * __ldg(img + o10 + c) + w11 * __ldg(img + o11 + c);
-                    gx = w00 * __ldg(img + o00 + C + c) + w01 * __ldg(img + o01 + C + c) + w10 * __ldg(img + o10 + C + c) + w11 * __ldg(img + o11 + C + c);
-                    gy = w00 * __ldg(img + o00 + 2 * C + c) + w01 * __ldg(img + o01 + 2 * C + c) + w10 * __ldg(img + o10 + 2 * C + c) + w11 * __ldg(img + o11 + 2 * C + c);
+                    f2 = w00 * ldg_feat(img + o00 + c) + w01 * ldg_feat(img + o01 + c) + w10 * ldg_feat(img + o10 + c) + w11 * ldg_feat(img + o11 + c);
+                    gx = w00 * ldg_feat(img + o00 + C + c) + w01 * ldg_feat(img + o01 + C + c) + w10 * ldg_feat(img + o10 + C + c) + w11 * ldg_feat(img + o11 + C + c);
+                    gy = w00 * ldg_feat(img + o00 + 2 * C + c) + w01 * ldg_feat(img + o01 + 2 * C + c) + w10 * ldg_feat(img + o10 + 2 * C + c) + w11 * ldg_feat(img + o11 + 2 * C + c);
                 }
-                const float d = __ldg(c1 + c) - f2;
+                const float d = ldg_feat(c1 + c) - f2;
                 m11 = fmaf(gx, gx, m11); m12 = fmaf(gx, gy, m12); m22 = fmaf(gy, gy, m22); q1 = fmaf(gx, d, q1); q2 = fmaf(gy, d, q2);
             }
             m11 = warp_sum(m11); m12 = warp_sum(m12); m22 = warp_sum(m22); q1 = warp_sum(q1); q2 = warp_sum(q2);
@@ -283,14 +287,14 @@ lm_build_bwd_kernel(const BwdParams prm)
                     fly.load(img, w, C, c, t, g, k);
                     t00 = t[0]; t01 = t[1]; t10 = t[2]; t11 = t[3]; g00 = g[0]; g01 = g[1]; g10 = g[2]; g11 = g[3]; k00 = k[0]; k01 = k[1]; k10 = k[2]; k11 = k[3];
                 } else {
-                    t00 = __ldg(img + o00 + c); t01 = __ldg(img + o01 + c); t10 = __ldg(img + o10 + c); t11 = __ldg(img + o11 + c);
-                    g00 = __ldg(img + o00 + C + c); g01 = __ldg(img + o01 + C + c); g10 = __ldg(img + o10 + C + c); g11 = __ldg(img + o11 + C + c);
-                    k00 = __ldg(img + o00 + 2 * C + c); k01 = __ldg(img + o01 + 2 * C + c); k10 = __ldg(img + o10 + 2 * C + c); k11 = __ldg(img + o11 + 2 * C + c);
+                    t00 = ldg_feat(img + o00 + c); t01 = ldg_feat(img + o01 + c); t10 = ldg_feat(img + o10 + c); t11 = ldg_feat(img + o11 + c);
+                    g00 = ldg_feat(img + o00 + C + c); g01 = ldg_feat(img + o01 + C + c); g10 = ldg_feat(img + o10 + C + c); g11 = ldg_feat(img + o11 + C + c);
+                    k00 = ldg_feat(img + o00 + 2 * C + c); k01 = ldg_feat(img + o01 + 2 * C + c); k10 = ldg_feat(img + o10 + 2 * C + c); k11 = ldg_feat(img + o11 + 2 * C + c);
                 }
                 const float f2 = w00 * t00 + w01 * t01 + w10 * t10 + w11 * t11;
                 const float gx = w00 * g00 + w01 * g01 + w10 * g10 + w11 * g11;
                 const float gy = w00 * k00 + w01 * k01 + w10 * k10 + w11 * k11;
-                const float d = __ldg(c1 + c) - f2;
+                const float d = ldg_feat(c1 + c) - f2;
                 const float dd = gx * z0 + gy * z1 + sRh[c] * sgnf(d);
                 const float dgx = gx * Q00 + gy * Q10 + d * z0, dgy = gx * Q01 + gy * Q11 + d * z1;
                 dc1[c] = dd;
@@ -341,6 +345,13 @@ lm_build_bwd_kernel(const BwdParams prm)
     if (cur_b >= 0) commit(cur_b);
 }
 
+template <typename TF>
+static void (*select_bwd_kernel(int K, bool c3))(const BwdParams)
+{
+    if (c3) return K <= 32 ? lm_build_bwd_kernel<1, BWD_3C, TF> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_3C, TF> : lm_build_bwd_kernel<8, BWD_3C, TF>);
+    return K <= 32 ? lm_build_bwd_kernel<1, BWD_F2, TF> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_F2, TF> : lm_build_bwd_kernel<8, BWD_F2, TF>);
+}
+
 int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dH, const float* dg, const float* drbar,
                  int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, cudaStream_t st)
 {
@@ -349,10 +360,10 @@ int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const 
     const size_t smem = ((size_t)K * K + 12 * (size_t)K + 36 + P + K + 16 + lv->C) * sizeof(float);
     BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_build_bwd: K=%d, C=%d need %zu B of shared memory", K, lv->C, smem);
     void (*kern)(const BwdParams);
-    if (lv->conv2_channels == 3 * lv->C)
-        kern = K <= 32 ? lm_build_bwd_kernel<1, BWD_3C> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_3C> : lm_build_bwd_kernel<8, BWD_3C>);
+    if (lv->feature_dtype == BANET_DTYPE_BF16)
+        kern = select_bwd_kernel<bf16>(K, lv->conv2_channels == 3 * lv->C);
     else
-        kern = K <= 32 ? lm_build_bwd_kernel<1, BWD_F2> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_F2> : lm_build_bwd_kernel<8, BWD_F2>);
+        kern = select_bwd_kernel<float>(K, lv->conv2_channels == 3 * lv->C);
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("lm_build_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
     BwdParams prm;

@@ -1,6 +1,7 @@
 // Level pre-/post-steps: rays, grad_fixed(+concat,+half swap), bilinear resampler, depth composition.
 // All are one-pass streaming kernels (HBM-bound, coalesced along the channel axis).
 #include "common.cuh"
+#include "features.cuh"
 #include "lm_build.h"
 
 namespace banet {
@@ -74,9 +75,13 @@ __global__ void interpolate2d_kernel(const float* __restrict__ data, const float
     if (mask && lane == 0) mask[pt] = (x >= 0.f && x <= (float)(w - 1) && y >= 0.f && y <= (float)(h - 1)) ? 1.f : 0.f;
 }
 
-// tf.contrib.resampler.resampler: bilinear, zero outside.  Warp per point, lanes over channels.
-__global__ void resample_kernel(const float* __restrict__ data, const float* __restrict__ xy, float cs,
-                                int nb, int h, int w, int C, int N, float* __restrict__ out)
+// tf.contrib.resampler.resampler: bilinear, zero outside.  Warp per point, lanes over channels.  TF: float, or bf16 in and out (fp32
+// arithmetic, rounded to nearest on store).
+__device__ __forceinline__ void store_feat(float* p, float v) { *p = v; }
+__device__ __forceinline__ void store_feat(bf16* p, float v) { *p = __float2bfloat16_rn(v); }
+template <typename TF>
+__global__ void resample_kernel(const TF* __restrict__ data, const float* __restrict__ xy, float cs,
+                                int nb, int h, int w, int C, int N, TF* __restrict__ out)
 {
     const long long pt = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
@@ -88,16 +93,16 @@ __global__ void resample_kernel(const float* __restrict__ data, const float* __r
     const bool fin = isfinite(x) && isfinite(y) && fabsf(x) < 1e9f && fabsf(y) < 1e9f;
     const int x0 = fin ? (int)fx : -10, y0 = fin ? (int)fy : -10;
     const float wt[4] = {(1.f - dx) * (1.f - dy), dx * (1.f - dy), (1.f - dx) * dy, dx * dy};
-    const float* img = data + (size_t)b * h * w * C;
-    float* o = out + (size_t)pt * C;
+    const TF* img = data + (size_t)b * h * w * C;
+    TF* o = out + (size_t)pt * C;
     for (int c = lane; c < C; c += 32) {
         float acc = 0.f;
 #pragma unroll
         for (int tp = 0; tp < 4; ++tp) {
             const int xx = x0 + (tp & 1), yy = y0 + (tp >> 1);
-            if (xx >= 0 && xx < w && yy >= 0 && yy < h) acc = fmaf(wt[tp], __ldg(img + ((size_t)yy * w + xx) * C + c), acc);
+            if (xx >= 0 && xx < w && yy >= 0 && yy < h) acc = fmaf(wt[tp], ldg_feat(img + ((size_t)yy * w + xx) * C + c), acc);
         }
-        o[c] = acc;
+        store_feat(o + c, acc);
     }
 }
 
@@ -264,8 +269,19 @@ extern "C" int banet_resample(const float* data, const float* xy, float coord_sc
 {
     BANET_REQUIRE(data && xy && out && nb > 0 && h > 0 && w > 0 && C > 0 && N > 0, BANET_ERR_BAD_ARG, "resample: bad argument");
     const long long thr = (long long)nb * N * 32;
-    resample_kernel<<<(unsigned)((thr + 255) / 256), 256, 0, (cudaStream_t)stream>>>(data, xy, coord_scale, nb, h, w, C, N, out);
+    resample_kernel<float><<<(unsigned)((thr + 255) / 256), 256, 0, (cudaStream_t)stream>>>(data, xy, coord_scale, nb, h, w, C, N, out);
     BANET_CUDA_LAUNCH_CHECK("resample");
+    return BANET_OK;
+}
+
+extern "C" int banet_resample_bf16(const void* data, const float* xy, float coord_scale, int nb, int h, int w, int C, int N,
+                                   void* out, banet_stream_t stream)
+{
+    BANET_REQUIRE(data && xy && out && nb > 0 && h > 0 && w > 0 && C > 0 && N > 0, BANET_ERR_BAD_ARG, "resample_bf16: bad argument");
+    const long long thr = (long long)nb * N * 32;
+    resample_kernel<bf16><<<(unsigned)((thr + 255) / 256), 256, 0, (cudaStream_t)stream>>>(static_cast<const bf16*>(data), xy, coord_scale, nb, h, w,
+                                                                                         C, N, static_cast<bf16*>(out));
+    BANET_CUDA_LAUNCH_CHECK("resample_bf16");
     return BANET_OK;
 }
 

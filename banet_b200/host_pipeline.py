@@ -172,7 +172,9 @@ class ResizeHostSolver:
         conv2 = the other half of the same buffer, F2 only (gradients on the fly in the build kernel, bundlenet.py:92-100, 386-389);
         p = computeCoordinates(points_l, intr / scale_l) (:358);  D, B = resampler(init_depth | basis, points / 2) (:343-344).
     Pairs are cut into chunks inside each half of the batch; the H2D copies of the images a later chunk needs overlap the solve of the
-    current one (copy stream / compute stream)."""
+    current one (copy stream / compute stream).
+    The pyramid keeps the host layers' dtype on the device: a bfloat16 pyramid (an autocast encoder's output) is copied at 2 bytes per
+    element and solved as bfloat16 levels; basis, depth and intrinsics are float32.  `h2d_bytes` counts the real element sizes."""
 
     def __init__(self, layers: Sequence[Tensor], basis: Tensor, init_depth: Tensor, intr: Tensor, scales: Sequence[int], chunks: int = 4,
                  device=None, precision: int = PREC_AUTO):
@@ -189,11 +191,14 @@ class ResizeHostSolver:
         self.ranges = [(o + a, o + b) for a, b in chunk_ranges(self.half, per_half) for o in (0, self.half)]
         self.copy_stream = torch.cuda.Stream(self.dev); self.compute_stream = torch.cuda.Stream(self.dev)
         dev = self.dev
-        self.d_layers = [torch.empty(t.shape, dtype=torch.float32, device=dev) for t in self.h_layers]
+        fdt = self.h_layers[0].dtype
+        if fdt not in (torch.float32, torch.bfloat16) or any(t.dtype != fdt for t in self.h_layers):
+            raise ValueError(f"layers must all be float32 or all bfloat16; got {[t.dtype for t in self.h_layers]}")
+        self.d_layers = [torch.empty(t.shape, dtype=fdt, device=dev) for t in self.h_layers]
         self.d_basis = torch.empty(basis.shape, dtype=torch.float32, device=dev)
         self.d_depth = torch.empty(init_depth.shape, dtype=torch.float32, device=dev)
         self.d_intr = torch.empty(intr.shape, dtype=torch.float32, device=dev)
-        self.h2d_bytes = 4 * (sum(t.numel() for t in self.h_layers) + basis.numel() + init_depth.numel() + intr.numel())
+        self.h2d_bytes = sum(t.numel() * t.element_size() for t in (*self.h_layers, basis, init_depth, intr))
         self.K = int(basis.shape[-1]); self.C = int(self.h_layers[0].shape[-1])
         nmax = max(b - a for a, b in self.ranges)
         self.pts, self.scr = [], []

@@ -16,11 +16,15 @@ from ._lib import BanetLevel, BanetSolveOpts, check, load
 Tensor = torch.Tensor
 
 
-def _chk(t: Tensor, name: str, shape: Optional[Tuple[int, ...]] = None) -> Tensor:
+_FEATURE_DTYPES = {torch.float32: _lib.DTYPE_F32, torch.bfloat16: _lib.DTYPE_BF16}
+
+
+def _chk(t: Tensor, name: str, shape: Optional[Tuple[int, ...]] = None, features: bool = False) -> Tensor:
+    """features=True: a feature map (conv1 / conv2 / resampler data), which may also be bfloat16."""
     if not isinstance(t, torch.Tensor) or not t.is_cuda:
         raise _lib.BanetError(f"{name}: expected a CUDA tensor (banet_b200 has no CPU path)")
-    if t.dtype != torch.float32:
-        raise _lib.BanetError(f"{name}: expected float32, got {t.dtype}")
+    if t.dtype != torch.float32 and not (features and t.dtype == torch.bfloat16):
+        raise _lib.BanetError(f"{name}: expected {'float32 or bfloat16' if features else 'float32'}, got {t.dtype}")
     if shape is not None and tuple(t.shape) != tuple(shape):
         raise _lib.BanetError(f"{name}: expected shape {tuple(shape)}, got {tuple(t.shape)}")
     return t.contiguous()
@@ -119,12 +123,15 @@ def grad_fixed_concat(F: Tensor, swap_halves: bool = False, out: Optional[Tensor
 
 
 def resample(data: Tensor, xy: Tensor, coord_scale: float = 1.0) -> Tensor:
+    """Bilinear sampler, zero outside: data [nb,h,w,C] (float32, or bfloat16: banet_resample_bf16, fp32 arithmetic, the result rounded to
+    bfloat16), xy [nb,N,2] -> [nb,N,C] in data's dtype."""
     lib = load()
-    dt = _chk(data, "data"); nb, h, w, Cc = dt.shape
+    dt = _chk(data, "data", features=True); nb, h, w, Cc = dt.shape
     pts = _chk(xy, "xy"); N = pts.shape[1]
-    out = torch.empty(nb, N, Cc, device=dt.device, dtype=torch.float32)
-    check(lib.banet_resample(dt.data_ptr(), pts.data_ptr(), float(coord_scale), nb, h, w, Cc, N, out.data_ptr(), _stream()),
-          "banet_resample")
+    out = torch.empty(nb, N, Cc, device=dt.device, dtype=dt.dtype)
+    fn = lib.banet_resample_bf16 if dt.dtype == torch.bfloat16 else lib.banet_resample
+    check(fn(dt.data_ptr(), pts.data_ptr(), float(coord_scale), nb, h, w, Cc, N, out.data_ptr(), _stream()),
+          "banet_resample_bf16" if dt.dtype == torch.bfloat16 else "banet_resample")
     return out
 
 
@@ -154,7 +161,7 @@ def depth_compose(init_depth: Tensor, basis: Tensor, W: Tensor) -> Tensor:
 @dataclass
 class Level:
     """One pyramid level in the reference's tensor layouts (see banet_level in include/banet_abi.h)."""
-    conv1: Tensor             # [nb,N,C]
+    conv1: Tensor             # [nb,N,C]      float32, or bfloat16 (conv1 and conv2 the same dtype)
     conv2: Tensor             # [nb,h,w,3C]  ([nb,h,w,C]: F2 only, gradients derived on the fly)
     intr: Tensor              # [nb,4]
     p: Tensor                 # [nb,3,N]
@@ -163,8 +170,10 @@ class Level:
     grid: Optional[Tuple[int, int]] = None   # (grid_w, grid_h) if the N points are a row-major raster grid (locality hint)
 
     def as_struct(self) -> Tuple[BanetLevel, list]:
-        conv1 = _chk(self.conv1, "conv1"); nb, N, Cc = conv1.shape
-        conv2 = _chk(self.conv2, "conv2"); _, h, w, c2 = conv2.shape
+        conv1 = _chk(self.conv1, "conv1", features=True); nb, N, Cc = conv1.shape
+        conv2 = _chk(self.conv2, "conv2", features=True); _, h, w, c2 = conv2.shape
+        if conv1.dtype != conv2.dtype:
+            raise _lib.BanetError(f"conv1 ({conv1.dtype}) and conv2 ({conv2.dtype}) must have the same dtype (float32 or bfloat16)")
         intr = _chk(self.intr, "intr", (nb, 4)); p = _chk(self.p, "p", (nb, 3, N)); D = _chk(self.D, "D", (nb, N, 1))
         B = None if self.B is None else _chk(self.B, "B")
         K = 0 if B is None else B.shape[2]
@@ -177,7 +186,7 @@ class Level:
         if gw * gh not in (0, N):
             raise _lib.BanetError(f"grid {gw}x{gh} does not match N={N}")
         return BanetLevel(nb, N, Cc, K, h, w, c2, conv1.data_ptr(), conv2.data_ptr(), intr.data_ptr(), p.data_ptr(),
-                          D.data_ptr(), _ptr(B), gw, gh), keep
+                          D.data_ptr(), _ptr(B), gw, gh, _FEATURE_DTYPES[conv1.dtype]), keep
 
 
 def lm_build(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], precision: int = _lib.PREC_AUTO):
@@ -401,6 +410,8 @@ class KeyframeLevel:
     B: Tensor                 # [nw,N,K]
 
     def as_struct(self) -> Tuple[_lib.BanetKeyframeLevel, list]:
+        if self.conv1.dtype != torch.float32 or self.conv2.dtype != torch.float32:
+            raise _lib.BanetError(f"keyframe levels take float32 features only (conv1 {self.conv1.dtype}, conv2 {self.conv2.dtype})")
         conv1 = _chk(self.conv1, "conv1"); nw, N, Cc = conv1.shape
         conv2 = _chk(self.conv2, "conv2"); nb, h, w, c2 = conv2.shape
         if nb % nw:
@@ -538,7 +549,8 @@ def lm_run_workspace_bytes(levels: Sequence[Level], precision: int = _lib.PREC_A
 # ------------------------------------------------------------------------------------------ backward of one iteration
 def lm_build_bwd(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], dH: Tensor, dg: Tensor, drbar_sum: Tensor, exact_sym: bool = False):
     """Backward of lm_build (banet_lm_build_bwd) -> dconv1, dconv2, dD, dB, dR, dT, dW.  dconv2 has conv2's layout: [nb,h,w,3C] for
-    [F2|gx|gy], [nb,h,w,C] for F2 only (the adjoint of the on-the-fly gradient stencil is applied inside the kernel)."""
+    [F2|gx|gy], [nb,h,w,C] for F2 only (the adjoint of the on-the-fly gradient stencil is applied inside the kernel).  dconv1 and dconv2
+    are float32 also for bfloat16 features (the kernel accumulates them with fp32 atomics)."""
     lib = load()
     st, keep = level.as_struct()
     nb, K, Cc, N = st.nb, st.K, st.C, st.N

@@ -90,6 +90,10 @@ int banet_grad_fixed_concat(const float* F, int nb, int h, int w, int C, int swa
  *   data [nb,h,w,C], xy [nb,N,2] (sampled at xy*coord_scale) -> out [nb,N,C] */
 int banet_resample(const float* data, const float* xy, float coord_scale, int nb, int h, int w, int C, int N,
                    float* out, banet_stream_t stream);
+/* The same sampler on bf16 maps: data [nb,h,w,C] bf16 -> out [nb,N,C] bf16 (fp32 arithmetic, rounded to nearest on store).
+ * Its backward is banet_resample_bwd (fp32 gradients). */
+int banet_resample_bf16(const void* data, const float* xy, float coord_scale, int nb, int h, int w, int C, int N,
+                        void* out, banet_stream_t stream);
 
 /* The legacy sampler (legacy/utils_python.py:61-117 `interpolate2d`, :177-232 `interpolate2d2`): bilinear with CLAMPED tap indices;
  * mask [nb,N] (optional, may be NULL) = the in-bounds test of :114-116.  Same layouts as banet_resample. */
@@ -100,12 +104,19 @@ int banet_interpolate2d(const float* data, const float* xy, float coord_scale, i
  * (3) Layer level — one LM iteration = BundleNet.BundleIteration (bundlenet.py:193-278) or
  *     BundleNet.CameraIteration (:122-191) when K == 0 / B == NULL.
  * ---------------------------------------------------------------------------------------------- */
+/* Element type of conv1 and conv2 (banet_level_t::feature_dtype).  Every other tensor of the library is fp32.  bf16 features are
+ * widened to fp32 exactly where they are read; all arithmetic stays fp32. */
+#define BANET_DTYPE_F32  0
+#define BANET_DTYPE_BF16 1
+
+/* feature_dtype is the last field, so a zero-initialised struct keeps fp32 features.  It changed sizeof(banet_level_t) and therefore
+ * the stride of every levels[] array: code compiled against a header without the field cannot pass level arrays to this library. */
 typedef struct banet_level {
     int nb, N, C, K;          /* pairs, points per pair, feature channels, depth bases (0 = pose only) */
     int h, w;                 /* conv2 map size at this level */
     int conv2_channels;       /* 3*C: [F2|gx|gy] as in the reference; C: F2 only, gradients derived on the fly */
-    const float* conv1;       /* [nb,N,C]      bundlenet.py:385 */
-    const float* conv2;       /* [nb,h,w,conv2_channels]  :386-389 */
+    const void* conv1;        /* [nb,N,C]      bundlenet.py:385  (element type: feature_dtype) */
+    const void* conv2;        /* [nb,h,w,conv2_channels]  :386-389  (element type: feature_dtype) */
     const float* intr;        /* [nb,4] fx,fy,ox,oy at this level (reference tiles them to [nb,N], :379-382) */
     const float* p;           /* [nb,3,N]      :358 */
     const float* D;           /* [nb,N,1]      :343 */
@@ -113,6 +124,10 @@ typedef struct banet_level {
     int grid_w, grid_h;       /* locality hint, results do not depend on it: 0,0 = unstructured point list; otherwise the N points
                                  are the row-major raster grid x<grid_w, y<grid_h (N == grid_w*grid_h) and the kernels walk it in
                                  8x8 tiles so that every conv2 texel is fetched from HBM about once */
+    int feature_dtype;        /* BANET_DTYPE_F32 (0) or BANET_DTYPE_BF16 (1), for conv1 and conv2 together; any other value is
+                                 BANET_ERR_BAD_ARG.  bf16 levels run the fp32 SIMT build and tensor-core generation 6 (never generation 7),
+                                 are rejected by banet_lm_track_legacy (BANET_ERR_UNSUPPORTED), and their banet_lm_build_bwd writes
+                                 dconv1 / dconv2 as fp32 buffers */
 } banet_level_t;
 
 #define BANET_PREC_AUTO    (-1)   /* the level-wise policy (TF32_LEVELWISE) where the tensor-core path applies (K in {32,64,128}, C in {64,128}), else FP32_SIMT */
@@ -176,7 +191,8 @@ int    banet_lm_step(const float* H, const float* g, const float* rbar_sum, int 
  * drbar_sum [nb,C]  ->  dconv1 [nb,N,C], dconv2 [nb,h,w,conv2_channels], dD [nb,N,1], dB [nb,N,K], dR [nb,3,3],
  * dT [nb,3,1], dW [nb,K,1]; every output is overwritten.  conv2 may be either layout banet_lm_build takes: the
  * reference's [F2|gx|gy] (3C), or F2 only (C), whose dconv2 is the gradient w.r.t. F2 through the build's on-the-fly
- * REFLECT-by-one gradient stencil.  exact_sym as in banet_eqc_bwd (0 = the reference's 2*A*Ghat). */
+ * REFLECT-by-one gradient stencil.  exact_sym as in banet_eqc_bwd (0 = the reference's 2*A*Ghat).  dconv1 and dconv2 are fp32 whatever
+ * the level's feature_dtype (dconv2 is accumulated with fp32 atomics); a bf16 caller rounds them once. */
 int    banet_lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W,
                           const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
                           float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
