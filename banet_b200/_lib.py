@@ -13,19 +13,21 @@ LIB_PATH = os.environ.get("BANET_LIB_PATH") or os.path.join(_HERE, "libbanet.so"
 
 BANET_OK = 0
 PREC_AUTO, PREC_FP32_SIMT, PREC_TF32X1, PREC_TF32X2, PREC_TF32X3, PREC_TF32_LEVELWISE = -1, 0, 1, 2, 3, 4
-DTYPE_F32, DTYPE_BF16 = 0, 1          # banet_level_t::feature_dtype (conv1 and conv2)
+DTYPE_F32, DTYPE_BF16 = 0, 1          # banet_level_t::feature_dtype (conv1 and conv2) and ::basis_dtype (B)
 
 c_float_p = C.c_void_p      # raw device pointers
 c_stream = C.c_void_p
 
 
 class BanetLevel(C.Structure):
-    """struct banet_level (include/banet_abi.h).  feature_dtype is last, so a struct built without it keeps fp32 features."""
+    """struct banet_level (include/banet_abi.h).  feature_dtype and basis_dtype are last, so a struct built without them keeps fp32
+    features and an fp32 basis."""
     _fields_ = [("nb", C.c_int), ("N", C.c_int), ("C", C.c_int), ("K", C.c_int),
                 ("h", C.c_int), ("w", C.c_int), ("conv2_channels", C.c_int),
                 ("conv1", C.c_void_p), ("conv2", C.c_void_p), ("intr", C.c_void_p),
                 ("p", C.c_void_p), ("D", C.c_void_p), ("B", C.c_void_p),
-                ("grid_w", C.c_int), ("grid_h", C.c_int), ("feature_dtype", C.c_int)]
+                ("grid_w", C.c_int), ("grid_h", C.c_int), ("feature_dtype", C.c_int),
+                ("basis_dtype", C.c_int)]
 
 
 class BanetKeyframeLevel(C.Structure):
@@ -112,6 +114,7 @@ SIGNATURES = {
                                         C.POINTER(BanetSolveOpts), C.c_int] + [c_float_p] * 3 + [C.c_void_p]
                               + [C.c_void_p, C.c_size_t, c_stream]),
     "banet_depth_compose": (C.c_int, [c_float_p] * 3 + [C.c_int] * 3 + [c_float_p, c_stream]),
+    "banet_depth_compose_bf16": (C.c_int, [c_float_p, C.c_void_p, c_float_p] + [C.c_int] * 3 + [c_float_p, c_stream]),
     "banet_lm_step": (C.c_int, [c_float_p] * 3 + [C.c_int] * 4 + [c_float_p, C.c_float, c_float_p, C.POINTER(BanetSolveOpts)] + [c_float_p] * 3
                       + [c_float_p] * 3 + [c_float_p, c_float_p, C.c_void_p, c_stream]),
     "banet_lm_track_legacy_workspace_bytes": (C.c_size_t, [C.POINTER(BanetLevel), C.c_int]),
@@ -122,6 +125,7 @@ SIGNATURES = {
     "banet_grad_fixed_concat_bwd": (C.c_int, [c_float_p] + [C.c_int] * 5 + [c_float_p, c_stream]),
     "banet_resample_bwd": (C.c_int, [c_float_p, c_float_p, C.c_float] + [C.c_int] * 5 + [c_float_p, c_stream]),
     "banet_depth_compose_bwd": (C.c_int, [c_float_p] * 3 + [C.c_int] * 3 + [c_float_p, c_float_p, c_stream]),
+    "banet_depth_compose_bwd_bf16": (C.c_int, [c_float_p, C.c_void_p, c_float_p] + [C.c_int] * 3 + [c_float_p, c_float_p, c_stream]),
     "banet_tc_selftest": (C.c_int, [c_float_p] * 3 + [C.c_int, C.c_int, C.c_int, c_stream]),
 }
 

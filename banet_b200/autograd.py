@@ -138,7 +138,8 @@ def iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_b
 # ------------------------------------------------------------------------------------------ fused path
 class _LMBuildFn(torch.autograd.Function):
     """(H, g, rbar_sum) = banet_lm_build(...); backward = banet_lm_build_bwd.  conv2 is the [F2|gx|gy] tensor or F2 only; dconv2 comes back
-    in conv2's layout.  bfloat16 features are saved as they are; their gradients are accumulated in fp32 by the kernel and cast once."""
+    in conv2's layout.  bfloat16 features and a bfloat16 basis are saved as they are; their gradients are accumulated in fp32 by the kernel
+    and cast once."""
 
     @staticmethod
     def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, precision, exact_sym, grid):
@@ -162,6 +163,7 @@ class _LMBuildFn(torch.autograd.Function):
         dg = dg if dg is not None else torch.zeros(nb, P, device=conv1.device)
         drbar = drbar if drbar is not None else torch.zeros(nb, conv1.shape[2], device=conv1.device)
         dconv1, dconv2, dD, dB, dR, dT, dW = ops.lm_build_bwd(lv, R, T, W, dH, dg.contiguous(), drbar.contiguous(), ctx.exact_sym)
+        dB = None if dB is None else dB.to(B.dtype)
         return dconv1.to(conv1.dtype), dconv2.to(conv2.dtype), dD, dB, dR, dT, dW, None, None, None, None, None
 
 
@@ -294,7 +296,8 @@ class _ResampleFn(torch.autograd.Function):
 
 
 class _DepthComposeFn(torch.autograd.Function):
-    """init_depth + basis . W (bundlenet.py:397)."""
+    """init_depth + basis . W (bundlenet.py:397).  A bfloat16 basis is read as it is; its gradient comes back from the kernel in fp32 and
+    is cast to bfloat16 once."""
 
     @staticmethod
     def forward(ctx, init_depth, basis, W):
@@ -305,7 +308,7 @@ class _DepthComposeFn(torch.autograd.Function):
     def backward(ctx, dout):
         basis, W = ctx.saved_tensors
         dbasis, dW = ops.depth_compose_bwd(dout.contiguous(), basis, W)
-        return dout, dbasis, dW
+        return dout, dbasis.to(basis.dtype), dW
 
 
 def grad_fixed_concat(F: Tensor, swap_halves: bool = False) -> Tensor:
@@ -326,7 +329,8 @@ def iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regular
     """One differentiable LM iteration on the fused kernels.  Same arguments / returns as `iteration`; an F2-only conv2 [nb,h,w,C] goes
     straight into the build and its backward (the gradient stencil's adjoint runs inside banet_lm_build_bwd).
     precision: contraction mode of the FORWARD build (the backward is fp32); default FP32_SIMT, the reference's arithmetic type.
-    conv1 / conv2 may be bfloat16 (both): they are read as they are, and their gradients come back in bfloat16."""
+    conv1 / conv2 may be bfloat16 (both), and so may B (independently): they are read as they are, and their gradients come back in
+    bfloat16."""
     nb, N, C = conv1.shape
     bundle = B is not None
     H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, W, intr.detach(), p.detach(), precision, exact_sym, grid)
@@ -420,6 +424,9 @@ def _keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, 
     from . import _lib
     if precision not in (_lib.PREC_AUTO, _lib.PREC_FP32_SIMT):
         raise _lib.BanetError(f"precision {precision}: the keyframe build is fp32 SIMT only (AUTO or FP32_SIMT)")
+    if B.dtype != torch.float32:
+        raise _lib.BanetError(f"the keyframe form takes a float32 basis only (B {B.dtype}); give the keyframe tensors per frame ([nw,nf,...] or "
+                              "[nw,1,...]) to use a bfloat16 basis")
     if conv1.dtype != torch.float32 or conv2.dtype != torch.float32:
         raise _lib.BanetError(f"the keyframe form takes float32 features only (conv1 {conv1.dtype}, conv2 {conv2.dtype}); give the keyframe "
                               "tensors per frame ([nw,nf,...] or [nw,1,...]) to use bfloat16 features")

@@ -115,6 +115,8 @@ class BundleNet(torch.nn.Module):
             if self.training_path == "reference_split":
                 if conv1.dtype != torch.float32 or conv2.dtype != torch.float32:
                     raise RuntimeError("training_path='reference_split' takes float32 features; bfloat16 features train on the fused path")
+                if bundle and B.dtype != torch.float32:
+                    raise RuntimeError("training_path='reference_split' takes a float32 basis; a bfloat16 basis trains on the fused path")
                 Rn, Tn, Wn = _ag.iteration(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base if bundle else None,
                                            exact_sym=self.exact_sym_grad)
                 return Rn, Tn, Wn, None
@@ -204,9 +206,10 @@ class BundleNet(torch.nn.Module):
     def _keyframe_batch_iteration(self, conv1, conv2, intr, p, D, B, R, T, W, base, level):
         """WindowIteration on nw windows with the keyframe tensors once per window (conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K]):
         the keyframe build (banet_lm_keyframe_*), fused autograd path when gradients are recorded, else one iteration of
-        ops.lm_keyframe_run.  fp32 SIMT only: a TF32 precision raises, and so do bfloat16 features."""
+        ops.lm_keyframe_run.  fp32 SIMT only: a TF32 precision raises, and so do bfloat16 features and a bfloat16 basis."""
         self._require_keyframe_precision()
         self._require_keyframe_features(conv1, conv2)
+        self._require_keyframe_basis(B)
         nw, nf = R.shape[0], R.shape[1]
         if self._wants_grad(conv1, conv2, D, B, R, T, W):
             if self.training_path == "reference_split":
@@ -226,6 +229,12 @@ class BundleNet(torch.nn.Module):
         if any(t.dtype != torch.float32 for t in features):
             raise RuntimeError("the keyframe form of WindowIteration / WindowResize takes float32 features only; give the keyframe tensors per "
                                "frame ([nw,1|nf,...]) to WindowIteration for bfloat16 features")
+
+    @staticmethod
+    def _require_keyframe_basis(basis: Tensor) -> None:
+        if basis.dtype != torch.float32:
+            raise RuntimeError(f"the keyframe form of WindowIteration / WindowResize takes a float32 basis only (got {basis.dtype}); give the "
+                               "keyframe tensors per frame ([nw,1|nf,...]) to WindowIteration for a bfloat16 basis")
 
     def _require_keyframe_precision(self) -> None:
         if self.precision not in (_lib.PREC_AUTO, _lib.PREC_FP32_SIMT):
@@ -279,7 +288,9 @@ class BundleNet(torch.nn.Module):
         the feature pyramid, the basis, the initial pose and the lambda-MLP parameters when gradients are being recorded
         (init_depth enters the LM only through stop_gradient, :341, and the output depth directly, :397).
         `layers` may be bfloat16 (an autocast encoder's pyramid): conv1 is then the bfloat16 resample and conv2 the half-swapped F2 only;
-        their gradients come back in bfloat16.  basis and init_depth stay float32."""
+        their gradients come back in bfloat16.  `basis` may be bfloat16 too, independently of the pyramid (an autocast decoder's depth basis):
+        it is sampled by the bfloat16 resample, the output depth is composed on it (banet_depth_compose_bf16), and its gradient comes back in
+        bfloat16.  init_depth stays float32."""
         nb = layers[-1].shape[0]
         K = basis.shape[-1]
         _points, intr = self._prepare(intrisic, points)
@@ -316,11 +327,12 @@ class BundleNet(torch.nn.Module):
         No gradients recorded: one ops.lm_keyframe_run iteration per level on the frames' F2 maps as they are.  Gradients recorded: the keyframe
         form of autograd.window_batch_iteration_fused per level on [F2|gx|gy] (the keyframe backward takes that layout only); gradients reach
         both pyramids, the basis, the initial pose and the lambda-MLP parameters, init_depth through the output depth only (:341, :397).
-        AUTO or FP32_SIMT and float32 pyramids only, like the keyframe form of WindowIteration."""
+        AUTO or FP32_SIMT, float32 pyramids and a float32 basis only, like the keyframe form of WindowIteration."""
         if self.vmatrix_batch_scramble:
             raise RuntimeError("vmatrix_batch_scramble=True is a 2-view quirk (bundlenet.py:45); the window solve has per-frame VMatrix only")
         self._require_keyframe_precision()
         self._require_keyframe_features(*key_layers, *frame_layers)
+        self._require_keyframe_basis(basis)
         nw, nf, K = self._window_resize_shapes(intrisic, key_layers, frame_layers, points, basis, init_depth, init_rotation, init_translation)
         _points, intr = self._prepare(intrisic, points)
         grad = self._wants_grad(*key_layers, *frame_layers, basis, init_rotation, init_translation)

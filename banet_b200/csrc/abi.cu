@@ -32,6 +32,8 @@ static int check_level(const banet_level_t* lv, const char* who)
     BANET_REQUIRE(lv->conv1 && lv->conv2 && lv->intr && lv->p && lv->D, BANET_ERR_BAD_ARG, "%s: null tensor", who);
     BANET_REQUIRE(lv->feature_dtype == BANET_DTYPE_F32 || lv->feature_dtype == BANET_DTYPE_BF16, BANET_ERR_BAD_ARG,
                   "%s: feature_dtype=%d must be BANET_DTYPE_F32 (0) or BANET_DTYPE_BF16 (1)", who, lv->feature_dtype);
+    BANET_REQUIRE(lv->basis_dtype == BANET_DTYPE_F32 || lv->basis_dtype == BANET_DTYPE_BF16, BANET_ERR_BAD_ARG,
+                  "%s: basis_dtype=%d must be BANET_DTYPE_F32 (0) or BANET_DTYPE_BF16 (1)", who, lv->basis_dtype);
     BANET_REQUIRE(lv->K == 0 || lv->B, BANET_ERR_BAD_ARG, "%s: K=%d but B is null", who, lv->K);
     BANET_REQUIRE((long long)lv->h * lv->w * lv->conv2_channels < (1LL << 40), BANET_ERR_BAD_ARG, "%s: map too large", who);
     BANET_REQUIRE((lv->grid_w == 0 && lv->grid_h == 0) || (lv->grid_w > 0 && lv->grid_h > 0 && (long long)lv->grid_w * lv->grid_h == lv->N),

@@ -1,4 +1,4 @@
-// Feature element types of banet_level_t::feature_dtype: float, or bf16 widened to fp32 exactly where it is read.
+// Element types of banet_level_t::feature_dtype and ::basis_dtype: float, or bf16 widened to fp32 exactly where it is read.
 #pragma once
 #include <cuda_bf16.h>
 #include "common.cuh"
@@ -20,5 +20,8 @@ __device__ __forceinline__ float ld_stream_bf1(const bf16* p) {
     asm volatile("ld.global.nc.L1::no_allocate.u16 %0, [%1];" : "=h"(r) : "l"(p));
     return __uint_as_float((uint32_t)r << 16);
 }
+// one element of a read-once stream (the basis rows), widened
+__device__ __forceinline__ float ld_stream_elem(const float* p) { return ld_stream_f1(p); }
+__device__ __forceinline__ float ld_stream_elem(const bf16* p) { return ld_stream_bf1(p); }
 
 }  // namespace banet

@@ -80,7 +80,15 @@ template <> struct ChanVec<1, bf16> {
     __device__ __forceinline__ void load_stream(const bf16* p) { v[0] = ld_stream_bf1(p); }
 };
 
-template <int KP, int VEC, typename TF>
+// 4 consecutive basis entries of a read-once stream, widened (bf16: 8 B, 8-B aligned)
+__device__ __forceinline__ float4 ld_stream_basis4(const float* p) { return ld_stream_f4(p); }
+__device__ __forceinline__ float4 ld_stream_basis4(const bf16* p) {
+    const uint2 u = ld_stream_bf4(p);
+    return make_float4(bf16_lo(u.x), bf16_hi(u.x), bf16_lo(u.y), bf16_hi(u.y));
+}
+
+// TB: basis element type (float, or bf16 widened exactly into the fp32 tile, so everything after S0 is the fp32 kernel's arithmetic)
+template <int KP, int VEC, typename TF, typename TB = float>
 __global__ void __launch_bounds__(BUILD_THREADS, (KP >= 128) ? 1 : 2)
 lm_build_kernel(const BuildParams prm)
 {
@@ -190,19 +198,19 @@ lm_build_kernel(const BuildParams prm)
 
         // ---- S0: stage the basis tile (coalesced, read-once) ------------------------------------
         if constexpr (KP > 0) {
-            const float* Bg = prm.B + ((size_t)b * N + n0) * K;
-            if ((K & 3) == 0) {
+            const TB* Bg = static_cast<const TB*>(prm.B) + ((size_t)b * N + n0) * K;
+            if ((K & 3) == 0 && (sizeof(TB) == 4 || (reinterpret_cast<uintptr_t>(prm.B) & 7) == 0)) {
                 const int k4 = K >> 2, kp4 = KP >> 2;
                 for (int i = tid; i < TILE_PX * kp4; i += BUILD_THREADS) {
                     const int n = i / kp4, q = i - n * kp4;
                     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (n < cnt && q < k4) v = ld_stream_f4(Bg + (size_t)n * K + 4 * q);
+                    if (n < cnt && q < k4) v = ld_stream_basis4(Bg + (size_t)n * K + 4 * q);
                     *reinterpret_cast<float4*>(Bs + n * LDB + 4 * q) = v;
                 }
             } else {
                 for (int i = tid; i < TILE_PX * KP; i += BUILD_THREADS) {
                     const int n = i / KP, k = i - n * KP;
-                    Bs[n * LDB + k] = (n < cnt && k < K) ? ld_stream_f1(Bg + (size_t)n * K + k) : 0.f;
+                    Bs[n * LDB + k] = (n < cnt && k < K) ? ld_stream_elem(Bg + (size_t)n * K + k) : 0.f;
                 }
             }
         }
@@ -496,11 +504,11 @@ int build_plan(const banet_level_t* lv, int num_sms, BuildPlan* plan)
     return BANET_OK;
 }
 
-template <int KP, int VEC, typename TF>
+template <int KP, int VEC, typename TF, typename TB>
 static int launch_build(const BuildParams& prm, int grid, cudaStream_t st)
 {
     const size_t smem = BuildSmem<KP>::bytes(prm.C);
-    auto kern = lm_build_kernel<KP, VEC, TF>;
+    auto kern = lm_build_kernel<KP, VEC, TF, TB>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("lm_build: smem attr (%zu B): %s", smem, cudaGetErrorString(e)); return BANET_ERR_CUDA; }
     kern<<<grid, BUILD_THREADS, smem, st>>>(prm);
@@ -523,12 +531,13 @@ int lm_build_simt(const banet_level_t* lv, const BuildPlan& plan, const float* R
     const bool bf = lv->feature_dtype == BANET_DTYPE_BF16;
     const bool vec4 = (lv->C % 4 == 0) && (lv->conv2_channels % 4 == 0) &&
                       ((reinterpret_cast<uintptr_t>(lv->conv1) | reinterpret_cast<uintptr_t>(lv->conv2)) % (bf ? 8 : 16) == 0);
+    const bool bb = lv->basis_dtype == BANET_DTYPE_BF16;
     int rc;
-#define BANET_DISPATCH(KPV)                                                                                                    \
-    rc = bf ? (vec4 ? launch_build<KPV, 4, bf16>(prm, plan.grid, st) : launch_build<KPV, 1, bf16>(prm, plan.grid, st))       \
-            : (vec4 ? launch_build<KPV, 4, float>(prm, plan.grid, st) : launch_build<KPV, 1, float>(prm, plan.grid, st))
+#define BANET_LAUNCH(KPV, TFV, TBV) (vec4 ? launch_build<KPV, 4, TFV, TBV>(prm, plan.grid, st) : launch_build<KPV, 1, TFV, TBV>(prm, plan.grid, st))
+#define BANET_DISPATCH_TB(KPV, TBV) rc = bf ? BANET_LAUNCH(KPV, bf16, TBV) : BANET_LAUNCH(KPV, float, TBV)
+#define BANET_DISPATCH(KPV) if (bb) BANET_DISPATCH_TB(KPV, bf16); else BANET_DISPATCH_TB(KPV, float)
     switch (plan.KP) {
-        case 0:   BANET_DISPATCH(0); break;
+        case 0:   BANET_DISPATCH_TB(0, float); break;          // no basis
         case 16:  BANET_DISPATCH(16); break;
         case 32:  BANET_DISPATCH(32); break;
         case 64:  BANET_DISPATCH(64); break;
@@ -543,6 +552,8 @@ int lm_build_simt(const banet_level_t* lv, const BuildPlan& plan, const float* R
         default: set_error("lm_build: bad KP %d", plan.KP); return BANET_ERR_UNSUPPORTED;
     }
 #undef BANET_DISPATCH
+#undef BANET_DISPATCH_TB
+#undef BANET_LAUNCH
     if (rc != BANET_OK) return rc;
     return launch_lm_reduce(prm, plan.grid, H, g, rbar_sum, nvalid, st);
 }

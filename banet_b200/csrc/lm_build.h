@@ -7,7 +7,9 @@ namespace banet {
 struct BuildParams {
     int nb, N, C, K, h, w, c2;
     const void *conv1, *conv2;        // element type: the level's feature_dtype (the kernels' TF template parameter)
-    const float *intr, *p, *D, *B, *R, *T, *W;
+    const float *intr, *p, *D;
+    const void* B;                    // element type: the level's basis_dtype (the kernels' TB template parameter)
+    const float *R, *T, *W;
     float* partials;
     int slot_floats, max_span, tiles_per_pair;
     long long total_tiles;

@@ -32,7 +32,9 @@ constexpr int THREADS = (W0 + GW + AW + MW) * 32;               // 640
 constexpr int STAGE_A = 4 * TILE * 128, STAGE_R = 5 * TILE * 128;
 constexpr int REC = 16;
 
-template <int MODE, bool FLY> struct Smem {
+// BB: the basis is bf16.  Its stage holds the same 32-column blocks with 64-B rows (64B swizzle), half the bytes, and needs no A_lo
+// tile: every bf16 value is exact in tf32, so the split-A pass multiplies zero.
+template <int MODE, bool FLY, bool BB = false> struct Smem {
 #ifndef BANET_TC6_NST1
 #define BANET_TC6_NST1 4
 #endif
@@ -49,10 +51,11 @@ template <int MODE, bool FLY> struct Smem {
     // CTA takes is lost to the L1, which holds the gather warps' tap loads in flight and catches the tap overlap of neighbouring pixels.
     static constexpr int NST = MODE == 1 ? BANET_TC6_NST1 : MODE == 2 ? BANET_TC6_NST2 : BANET_TC6_NST3;
     static constexpr int NREC = MODE == 3 ? 2 : BANET_TC6_NREC;
+    static constexpr int STAGE = BB ? STAGE_A / 2 : STAGE_A;           // one basis-tile stage
     static constexpr int off_A = 0;
-    static constexpr int off_R = NST * STAGE_A;
+    static constexpr int off_R = NST * STAGE;
     static constexpr int off_Alo = off_R + STAGE_R;
-    static constexpr int off_Rlo = off_Alo + (MODE >= 2 ? STAGE_A : 0);
+    static constexpr int off_Rlo = off_Alo + (MODE >= 2 && !BB ? STAGE_A : 0);
     static constexpr int off_misc = off_Rlo + (MODE == 3 ? STAGE_R : 0);
     static constexpr int off_bar = off_misc;                           // 22 mbarriers
     static constexpr int off_tile = off_misc + 192;                    // [NREC][4] ints: pair index of the tile in record buffer s
@@ -232,12 +235,17 @@ __device__ __forceinline__ void gather_bf16(const BuildParams& prm, const int* s
 
 // TF: feature element type (float or bf16).  bf16 keeps the half-warp per pixel; each tap is ONE load of the lane's C/16 channels
 // (16 B of 8 channels at C = 128, 8 B of 4 at C = 64), widened channel by channel where it is used.
-template <int NCH, bool FLY, int MODE, int KBLK = 4, typename TF = float>
+// TB: basis element type (float or bf16).  A bf16 tile is staged as it lies in HBM and widened in registers by each role that reads it:
+// the b.W walk (same fp32 order), the R rows, the MMA's A fragments.  It is exact in tf32, so MODE 1 skips its in-place rounding and
+// MODE 2 / 3 skip the split-A pass: results are bitwise those of the fp32 kernel on the widened basis.
+template <int NCH, bool FLY, int MODE, int KBLK = 4, typename TF = float, typename TB = float>
 __global__ void __launch_bounds__(THREADS, 1)
 lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams prm)
 {
-    using SM = Smem<MODE, FLY>;
+    constexpr bool BB = sizeof(TB) == 2;
+    using SM = Smem<MODE, FLY, BB>;
     constexpr int NST = SM::NST, NREC = SM::NREC;
+    constexpr int BLK = BB ? 4096 : 8192;                            // bytes of one 32-column block of the basis tile
     // KBLK = K / 32 basis blocks actually present (K = 128, 64 or 32).  The smem geometry stays that of K = 128 (32-KB stages); blocks
     // >= KBLK are never loaded or read, and the [v | t] block of R follows the last one.
     constexpr int KR = 32 * KBLK, EXTB = KBLK;
@@ -346,7 +354,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                 __syncwarp();
             }
             const int s = j % NST, sr = j % NREC;
-            const unsigned char* As = base + SM::off_A + s * STAGE_A;
+            const unsigned char* As = base + SM::off_A + s * SM::STAGE;
             // global inputs of this lane's pixel first (their latency hides behind the waits and the dot product)
             float p0 = 0.f, p1 = 0.f, p2 = 0.f, D0 = 0.f;
             int n = 0; bool valid = false;
@@ -364,14 +372,22 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
             float mydot;
             {
                 float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+                uint4 bq = make_uint4(0u, 0u, 0u, 0u);               // bf16: the 16-B chunk of columns 8(c/2) .. 8(c/2)+7, one LDS.128 per two steps
 #pragma unroll
                 for (int i = 0; i < 16; ++i) {
                     const int blk = 2 * hf + (i >> 3), c = i & 7;
                     if (KBLK != 4 && blk >= KBLK) continue;
-                    const float4 bv = *reinterpret_cast<const float4*>(As + blk * 8192 + sw128_off(nlr, c));
+                    float4 bv;
+                    if constexpr (BB) {
+                        if ((c & 1) == 0) bq = *reinterpret_cast<const uint4*>(As + blk * BLK + sw64_off(nlr, c >> 1));
+                        const uint32_t u0 = (c & 1) ? bq.z : bq.x, u1 = (c & 1) ? bq.w : bq.y;
+                        bv = make_float4(bf16_lo(u0), bf16_hi(u0), bf16_lo(u1), bf16_hi(u1));
+                    } else {
+                        bv = *reinterpret_cast<const float4*>(As + blk * 8192 + sw128_off(nlr, c));
+                    }
                     const float4 w4 = *reinterpret_cast<const float4*>(myW + blk * 32 + c * 4);
                     acc.x = fmaf(bv.x, w4.x, acc.x); acc.y = fmaf(bv.y, w4.y, acc.y); acc.z = fmaf(bv.z, w4.z, acc.z); acc.w = fmaf(bv.w, w4.w, acc.w);
-                    if constexpr (MODE == 1) {
+                    if constexpr (MODE == 1 && !BB) {
                         // single-pass mode: round the basis tile to tf32 IN PLACE.  The tensor core would truncate it (biased: relH 1e-5);
                         // round-to-nearest is unbiased per launch (relH < 1e-6) but is the SAME perturbation of the basis at every LM
                         // iteration, so its effect adds up coherently over a solve (W off by 1e-3 after 20 iterations).  Stochastic rounding
@@ -387,7 +403,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                                         __uint_as_float((__float_as_uint(bv.w) + ((hs2 >> 13) & 0x1fffu)) & 0xFFFFE000u));
                     }
                 }
-                if constexpr (MODE == 1) fence_proxy_async_smem();      // generic writes before the TMA refill of this stage
+                if constexpr (MODE == 1 && !BB) fence_proxy_async_smem();      // generic writes before the TMA refill of this stage
                 mydot = (acc.x + acc.y) + (acc.z + acc.w);
                 mydot += __shfl_xor_sync(0xffffffffu, mydot, 16);
             }
@@ -595,15 +611,15 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
         auto issue_tma = [&](int t) {                        // basis tile t -> stage t % NST (elected thread)
             const int st = t % NST;
             const TileCoord tc = tile_coord(prm, t_begin + t);
-            mbar_arrive_expect_tx(&fullB[st], KBLK * 8192);
-            unsigned char* dst = base + SM::off_A + st * STAGE_A;
+            mbar_arrive_expect_tx(&fullB[st], KBLK * BLK);
+            unsigned char* dst = base + SM::off_A + st * SM::STAGE;
             if (grid2d) {
 #pragma unroll
-                for (int blk = 0; blk < KBLK; ++blk) tma_load_3d_hint(dst + blk * 8192, &tmapB, blk * 32, tc.tx0, tc.b * prm.grid_h + tc.ty0, &fullB[st], pol_basis);
+                for (int blk = 0; blk < KBLK; ++blk) tma_load_3d_hint(dst + blk * BLK, &tmapB, blk * 32, tc.tx0, tc.b * prm.grid_h + tc.ty0, &fullB[st], pol_basis);
             } else {
                 const int row = tc.b * N + tc.n0;
 #pragma unroll
-                for (int blk = 0; blk < KBLK; ++blk) tma_load_2d_hint(dst + blk * 8192, &tmapB, blk * 32, row, &fullB[st], pol_basis);
+                for (int blk = 0; blk < KBLK; ++blk) tma_load_2d_hint(dst + blk * BLK, &tmapB, blk * 32, row, &fullB[st], pol_basis);
             }
         };
         auto flush = [&](int sp) {               // H_cc / g_c / nvalid and rbar of the span (the MMA warps write H_dd and the [v | t] columns)
@@ -637,7 +653,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
             const int s = j % NST, sr = j % NREC;
             const bool last_of_pair = (++rr == prm.tiles_per_pair) || (j == ntiles - 1);
             if (rr == prm.tiles_per_pair) rr = 0;
-            const unsigned char* As = base + SM::off_A + s * STAGE_A;
+            const unsigned char* As = base + SM::off_A + s * SM::STAGE;
             if (awi == 0) TC6_TRACE(1, j, 0);
             mbar_wait_parked(&gath[sr], (j / NREC) & 1);
             if (awi == 0) TC6_TRACE(1, j, 1);
@@ -694,6 +710,28 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
             }
             // R rows (and the split parts): elementwise on the lane's half row, so walk the PHYSICAL 16-B slots (rotated by the row: every
             // quarter-warp touches 8 distinct bank groups) and skip the swizzle arithmetic
+            if constexpr (BB) {
+                // bf16 tile: walk the lane's 16-B chunks (8 columns each, logical chunk m of block blk, every quarter-warp on 8 distinct bank
+                // groups), widen, and write the two fp32 chunks 2m, 2m+1 of the R row
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    const int blk = 2 * hf + (i >> 2), m = i & 3;
+                    if (KBLK != 4 && blk >= KBLK) continue;
+                    const uint4 q = *reinterpret_cast<const uint4*>(As + blk * BLK + sw64_off(nlr, m));
+                    const float bw[8] = {bf16_lo(q.x), bf16_hi(q.x), bf16_lo(q.y), bf16_hi(q.y), bf16_lo(q.z), bf16_hi(q.z), bf16_lo(q.w), bf16_hi(q.w)};
+#pragma unroll
+                    for (int hc = 0; hc < 2; ++hc) {
+                        const uint32_t off = blk * 8192 + sw128_off(nlr, 2 * m + hc);
+                        const float4 pv = make_float4(sn * bw[4 * hc], sn * bw[4 * hc + 1], sn * bw[4 * hc + 2], sn * bw[4 * hc + 3]);
+                        float4 hv;
+                        if constexpr (MODE == 3) hv = make_float4(tf32_rna(pv.x), tf32_rna(pv.y), tf32_rna(pv.z), tf32_rna(pv.w));
+                        else hv = make_float4(tf32_rna_bits(pv.x), tf32_rna_bits(pv.y), tf32_rna_bits(pv.z), tf32_rna_bits(pv.w));
+                        *reinterpret_cast<float4*>(Rs + off) = hv;
+                        if constexpr (MODE == 3)
+                            *reinterpret_cast<float4*>(base + SM::off_Rlo + off) = make_float4(pv.x - hv.x, pv.y - hv.y, pv.z - hv.z, pv.w - hv.w);
+                    }
+                }
+            } else {
             const uint32_t rowoff = hf * 16384 + nlr * 128;
 #pragma unroll
             for (int i = 0; i < 16; ++i) {
@@ -710,6 +748,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                 if constexpr (MODE == 3)
                     *reinterpret_cast<float4*>(base + SM::off_Rlo + off) = make_float4(pv.x - hv.x, pv.y - hv.y, pv.z - hv.z, pv.w - hv.w);
             }
+            }
             if (awi == 0) TC6_TRACE(1, j, 4);
             __syncwarp();
             if (lane == 0) mbar_arrive(rready);
@@ -719,44 +758,47 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
     } else {
         // ===================================================================== MMA warps: D = A^T R per tile, accumulated over the pair span
         setmaxnreg_inc<136>();
-        mma_role<SM, STAGE_A, MODE, KR>(prm, base, fullB, rready, rfree, t_begin, ntiles, warp - (W0 + GW + AW), lane);
+        mma_role<SM, SM::STAGE, MODE, KR, BB>(prm, base, fullB, rready, rfree, t_begin, ntiles, warp - (W0 + GW + AW), lane);
     }
 }
 
-template <int NCH, bool FLY, int MODE, int KBLK = 4, typename TF = float>
+template <int NCH, bool FLY, int MODE, int KBLK, typename TF, typename TB>
 static int launch6(const CUtensorMap& tm, const BuildParams& prm, int grid, cudaStream_t st)
 {
-    auto kern = lm_build_tc6_kernel<NCH, FLY, MODE, KBLK, TF>;
-    const int smem = Smem<MODE, FLY>::bytes;
+    auto kern = lm_build_tc6_kernel<NCH, FLY, MODE, KBLK, TF, TB>;
+    const int smem = Smem<MODE, FLY, sizeof(TB) == 2>::bytes;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { set_error("lm_build_tc6: smem attr (%d B): %s", smem, cudaGetErrorString(e)); return BANET_ERR_CUDA; }
     kern<<<grid, THREADS, smem, st>>>(tm, prm);
     BANET_CUDA_LAUNCH_CHECK("lm_build_tc6_kernel launch");
     return BANET_OK;
 }
-template <int NCH, bool FLY, typename TF>
+template <int NCH, bool FLY, typename TF, typename TB>
 static int launch6_mode(int mode, int kblk, const CUtensorMap& tm, const BuildParams& prm, int grid, cudaStream_t st)
 {
     if (kblk != 4) {             // K = 64 / 32 (opt-in, BANET_TC_SMALLK=1): instantiated for the two-pass and the fp32-grade mode only
-        if (kblk == 2) return mode == 3 ? launch6<NCH, FLY, 3, 2, TF>(tm, prm, grid, st) : launch6<NCH, FLY, 2, 2, TF>(tm, prm, grid, st);
-        return mode == 3 ? launch6<NCH, FLY, 3, 1, TF>(tm, prm, grid, st) : launch6<NCH, FLY, 2, 1, TF>(tm, prm, grid, st);
+        if (kblk == 2) return mode == 3 ? launch6<NCH, FLY, 3, 2, TF, TB>(tm, prm, grid, st) : launch6<NCH, FLY, 2, 2, TF, TB>(tm, prm, grid, st);
+        return mode == 3 ? launch6<NCH, FLY, 3, 1, TF, TB>(tm, prm, grid, st) : launch6<NCH, FLY, 2, 1, TF, TB>(tm, prm, grid, st);
     }
-    if (mode == 1) return launch6<NCH, FLY, 1, 4, TF>(tm, prm, grid, st);
-    if (mode == 2) return launch6<NCH, FLY, 2, 4, TF>(tm, prm, grid, st);
-    return launch6<NCH, FLY, 3, 4, TF>(tm, prm, grid, st);
+    if (mode == 1) return launch6<NCH, FLY, 1, 4, TF, TB>(tm, prm, grid, st);
+    if (mode == 2) return launch6<NCH, FLY, 2, 4, TF, TB>(tm, prm, grid, st);
+    return launch6<NCH, FLY, 3, 4, TF, TB>(tm, prm, grid, st);
 }
-template <typename TF>
+template <typename TF, typename TB>
 static int launch6_type(int mode, bool fly, int nch, int kblk, const CUtensorMap& tm, const BuildParams& prm, int grid, cudaStream_t st)
 {
-    if (nch == 2) return fly ? launch6_mode<2, true, TF>(mode, kblk, tm, prm, grid, st) : launch6_mode<2, false, TF>(mode, kblk, tm, prm, grid, st);
-    return fly ? launch6_mode<1, true, TF>(mode, kblk, tm, prm, grid, st) : launch6_mode<1, false, TF>(mode, kblk, tm, prm, grid, st);
+    if (nch == 2) return fly ? launch6_mode<2, true, TF, TB>(mode, kblk, tm, prm, grid, st) : launch6_mode<2, false, TF, TB>(mode, kblk, tm, prm, grid, st);
+    return fly ? launch6_mode<1, true, TF, TB>(mode, kblk, tm, prm, grid, st) : launch6_mode<1, false, TF, TB>(mode, kblk, tm, prm, grid, st);
 }
 
 }  // namespace v6
 
-int lm_build_tc6_launch(int mode, bool fly, int nch, int kblk, bool is_bf16, const CUtensorMap& tm, const BuildParams& prm, int grid, cudaStream_t st)
+int lm_build_tc6_launch(int mode, bool fly, int nch, int kblk, bool is_bf16, bool basis_bf16, const CUtensorMap& tm, const BuildParams& prm, int grid,
+                        cudaStream_t st)
 {
-    return is_bf16 ? v6::launch6_type<bf16>(mode, fly, nch, kblk, tm, prm, grid, st) : v6::launch6_type<float>(mode, fly, nch, kblk, tm, prm, grid, st);
+    if (basis_bf16)
+        return is_bf16 ? v6::launch6_type<bf16, bf16>(mode, fly, nch, kblk, tm, prm, grid, st) : v6::launch6_type<float, bf16>(mode, fly, nch, kblk, tm, prm, grid, st);
+    return is_bf16 ? v6::launch6_type<bf16, float>(mode, fly, nch, kblk, tm, prm, grid, st) : v6::launch6_type<float, float>(mode, fly, nch, kblk, tm, prm, grid, st);
 }
 
 }  // namespace banet

@@ -21,7 +21,8 @@
 //   7 (lm_build_tc7.cu)  F2-only conv2 + dense grid: the tile's F2 footprint is staged into shared memory by TMA (channel chunks),
 //                        the 12 gradient/bilinear taps of every pixel come from LDS; per-tile fallback to global taps when the
 //                        footprint of a tile does not fit the staged window.  MODE 1 and 2.
-//   6 (lm_build_tc6.cu)  everything (both conv2 layouts, dense grids and point lists, every mode, fp32 and bf16 features): taps by ld.global.
+//   6 (lm_build_tc6.cu)  everything (both conv2 layouts, dense grids and point lists, every mode, fp32 and bf16 features, fp32 and bf16
+//                        bases): taps by ld.global.
 #include "common.cuh"
 #include "lm_build.h"
 #include "tc_utils.cuh"
@@ -31,7 +32,8 @@ namespace banet {
 
 constexpr int TC_TILE = 64;
 
-int lm_build_tc6_launch(int mode, bool fly, int nch, int kblk, bool is_bf16, const CUtensorMap& tm, const BuildParams& prm, int grid, cudaStream_t st);
+int lm_build_tc6_launch(int mode, bool fly, int nch, int kblk, bool is_bf16, bool basis_bf16, const CUtensorMap& tm, const BuildParams& prm, int grid,
+                        cudaStream_t st);
 int lm_build_tc7_launch(int mode, int nch, int kblk, const CUtensorMap& tmB, const CUtensorMap& tmF, const CUtensorMap& tmC, const BuildParams& prm, int grid,
                         cudaStream_t st);
 bool lm_build_tc7_supported(int mode, int nch, int kblk);
@@ -41,14 +43,14 @@ static banet_tuning_t g_tuning = {0, 0, 4, 0, 0, 0};
 void set_tuning(const banet_tuning_t& t) { g_tuning = t; }
 const banet_tuning_t& tuning() { return g_tuning; }
 
-// Generation 7 applies to fp32 features in the F2-only layout on a dense grid (tap coordinates are packed in 16 bits), modes 1 and 2.  The default
+// Generation 7 applies to fp32 features and an fp32 basis in the F2-only layout on a dense grid (tap coordinates are packed in 16 bits), modes 1 and 2.  The default
 // (tc_generation = 0) is generation 6 everywhere: in interleaved A/B runs on an H100 80GB HBM3 (400 W power limit, 32 pairs, F2-only
 // layout) generation 7 took 25.5 vs 21.5 ms at 640x480 and 5.8 vs 5.4 ms at 320x240 in TF32X1, and 2.3x as long in TF32X2 (its
 // gather warps run on 64 registers and spill, see DESIGN.md §4).  banet_set_tuning(tc_generation = 7) forces it where it applies.
 static bool use_gen7(const banet_level_t* lv, int mode, int kblk)
 {
     const bool wanted = g_tuning.tc_generation == 7;
-    return wanted && lv->feature_dtype == BANET_DTYPE_F32 && lv->conv2_channels == lv->C && lv->grid_w > 0 && lv->h < 65536 && lv->w < 65536 &&
+    return wanted && lv->feature_dtype == BANET_DTYPE_F32 && lv->basis_dtype == BANET_DTYPE_F32 && lv->conv2_channels == lv->C && lv->grid_w > 0 && lv->h < 65536 && lv->w < 65536 &&
            lm_build_tc7_supported(mode, lv->C / 64, kblk);
 }
 
@@ -88,8 +90,9 @@ int lm_build_tc(const banet_level_t* lv, const BuildPlan& plan, int mode, const 
     if (kblk != 4 && mode == 1) mode = 2;          // K = 64 / 32: the single-pass mode is not instantiated
     CUtensorMap tm;
     int rc;
-    if (lv->grid_w > 0) rc = make_tmap_f32_3d_sw128(&tm, lv->B, (uint64_t)lv->nb * lv->grid_h, lv->grid_w, lv->K, 8, 8, 32);
-    else rc = make_tmap_f32_2d_sw128(&tm, lv->B, (uint64_t)lv->nb * lv->N, lv->K, TC_TILE, 32);
+    const bool basis_bf16 = lv->basis_dtype == BANET_DTYPE_BF16;     // 32-column blocks either way: 128-B rows (fp32) or 64-B rows (bf16)
+    if (lv->grid_w > 0) rc = make_tmap_basis_3d(&tm, lv->B, basis_bf16, (uint64_t)lv->nb * lv->grid_h, lv->grid_w, lv->K, 8, 8, 32);
+    else rc = make_tmap_basis_2d(&tm, lv->B, basis_bf16, (uint64_t)lv->nb * lv->N, lv->K, TC_TILE, 32);
     if (rc) return rc;
     const bool fly = lv->conv2_channels == lv->C;
     BuildParams prm;
@@ -124,7 +127,7 @@ int lm_build_tc(const banet_level_t* lv, const BuildPlan& plan, int mode, const 
         prm.band_rows = lv->grid_w > 0 && band > 1 ? band : 1;
         prm.l2_hints = g_tuning.tc6_l2_hints > 0 ? g_tuning.tc6_l2_hints - 1 : kTc6DefaultL2Hints;
         prm.tap_prefetch = g_tuning.tc6_tap_prefetch > 0 ? g_tuning.tc6_tap_prefetch - 1 : kTc6DefaultTapPrefetch;
-        rc = lm_build_tc6_launch(mode, fly, nch, kblk, lv->feature_dtype == BANET_DTYPE_BF16, tm, prm, plan.grid, st);
+        rc = lm_build_tc6_launch(mode, fly, nch, kblk, lv->feature_dtype == BANET_DTYPE_BF16, basis_bf16, tm, prm, plan.grid, st);
     }
     if (rc) return rc;
     return launch_lm_reduce(prm, plan.grid, H, g, rbar_sum, nvalid, st);

@@ -31,7 +31,9 @@ constexpr int BWD_KL_MAX = 8;                    // K <= 32 * BWD_KL_MAX
 struct BwdParams {
     int nb, N, C, K, h, w;
     const void *conv1, *conv2;                   // element type: the kernel's TF (the level's feature_dtype)
-    const float *intr, *p, *D, *B, *R, *T, *W;
+    const float *intr, *p, *D;
+    const void* B;                               // element type: the kernel's TB (the level's basis_dtype)
+    const float *R, *T, *W;
     const float *dH, *dg, *drbar;
     float *dconv1, *dconv2, *dD, *dB, *dR, *dT, *dW;
     int exact_sym, tiles_per_pair;
@@ -86,8 +88,8 @@ struct FlyTaps {
 };
 
 // smem layout (floats): S_dd [K][K] | S_cd [6][K] | S_dc [K][6] | S_cc [36] | ghat [P] | W [K] | pose [16] | rhat [C]
-// TF: feature element type (float or bf16, widened on load); dconv1 / dconv2 are fp32 for both
-template <int BWD_KL, int LAYOUT, typename TF>
+// TF: feature element type (float or bf16, widened on load); dconv1 / dconv2 are fp32 for both.  TB: the same for the basis; dB is fp32.
+template <int BWD_KL, int LAYOUT, typename TF, typename TB = float>
 __global__ void __launch_bounds__(BWD_THREADS, 2)
 lm_build_bwd_kernel(const BwdParams prm)
 {
@@ -168,7 +170,7 @@ lm_build_bwd_kernel(const BwdParams prm)
 #pragma unroll
             for (int i = 0; i < BWD_KL; ++i) {
                 const int k = lane + 32 * i;
-                bl[i] = (k < K) ? ld_stream_f1(prm.B + gi * K + k) : 0.f;
+                bl[i] = (k < K) ? ld_stream_elem(static_cast<const TB*>(prm.B) + gi * K + k) : 0.f;
                 if (k < K) bw = fmaf(bl[i], sW[k], bw);
             }
             bw = warp_sum(bw);
@@ -345,11 +347,11 @@ lm_build_bwd_kernel(const BwdParams prm)
     if (cur_b >= 0) commit(cur_b);
 }
 
-template <typename TF>
+template <typename TF, typename TB>
 static void (*select_bwd_kernel(int K, bool c3))(const BwdParams)
 {
-    if (c3) return K <= 32 ? lm_build_bwd_kernel<1, BWD_3C, TF> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_3C, TF> : lm_build_bwd_kernel<8, BWD_3C, TF>);
-    return K <= 32 ? lm_build_bwd_kernel<1, BWD_F2, TF> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_F2, TF> : lm_build_bwd_kernel<8, BWD_F2, TF>);
+    if (c3) return K <= 32 ? lm_build_bwd_kernel<1, BWD_3C, TF, TB> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_3C, TF, TB> : lm_build_bwd_kernel<8, BWD_3C, TF, TB>);
+    return K <= 32 ? lm_build_bwd_kernel<1, BWD_F2, TF, TB> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_F2, TF, TB> : lm_build_bwd_kernel<8, BWD_F2, TF, TB>);
 }
 
 int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dH, const float* dg, const float* drbar,
@@ -360,10 +362,9 @@ int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const 
     const size_t smem = ((size_t)K * K + 12 * (size_t)K + 36 + P + K + 16 + lv->C) * sizeof(float);
     BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_build_bwd: K=%d, C=%d need %zu B of shared memory", K, lv->C, smem);
     void (*kern)(const BwdParams);
-    if (lv->feature_dtype == BANET_DTYPE_BF16)
-        kern = select_bwd_kernel<bf16>(K, lv->conv2_channels == 3 * lv->C);
-    else
-        kern = select_bwd_kernel<float>(K, lv->conv2_channels == 3 * lv->C);
+    const bool c3 = lv->conv2_channels == 3 * lv->C, bff = lv->feature_dtype == BANET_DTYPE_BF16, bfb = K > 0 && lv->basis_dtype == BANET_DTYPE_BF16;
+    if (bfb) kern = bff ? select_bwd_kernel<bf16, bf16>(K, c3) : select_bwd_kernel<float, bf16>(K, c3);
+    else kern = bff ? select_bwd_kernel<bf16, float>(K, c3) : select_bwd_kernel<float, float>(K, c3);
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("lm_build_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
     BwdParams prm;

@@ -19,6 +19,9 @@
 //   R, half group (columns 32G .. 32G+15, G = mb / 2, the last columns of an m-block with mb even): two accumulator blocks j = 0, 1;
 //     fragment column g of block j is column 32G + 2g + j, one LDS.64 per pixel row (the walk of the A pairs, same 2-way conflict).
 //   [v | t] block: fragment column g is column KR + g, as the algebra warps write it; scalar loads.
+//   A on a bf16 basis (BB; 64-B rows, 64B swizzle): columns 2g and 2g+1 are one 32-bit word, so (a0, a1) at pixel t and (a2, a3) at
+//     pixel t+4 are one LDS.32 each, widened by a shift and a mask (exact tf32 values).  Rows t and t+2 are 128 B apart: the same 2-way
+//     bank conflict.  The split-A pass is skipped (A_lo = 0); the passes left keep their order.
 // Accumulator element e (fragment row g + 8(e >> 1), column 2t + (e & 1)) holds row i = 16mb + 2g + (e >> 1) and column
 //   n = 32G + 4t + 16(e & 1) + j (full group), 32G + 4t + 2(e & 1) + j (half group), KR + 2t + (e & 1) ([v | t]).
 #pragma once
@@ -84,7 +87,7 @@ template <int MB> struct MmaAcc {                      // accumulators of one m-
     }
 };
 
-template <class SM, int STAGE_A, int MODE, int KR, int MB0, int MB1>
+template <class SM, int STAGE_A, int MODE, int KR, int MB0, int MB1, bool BB>
 __device__ __forceinline__ void mma_warp(const BuildParams& prm, const unsigned char* base, uint64_t* fullB, uint64_t* rready,
                                          uint64_t* rfree, long long t_begin, int ntiles, int lane)
 {
@@ -97,6 +100,7 @@ __device__ __forceinline__ void mma_warp(const BuildParams& prm, const unsigned 
     const uint32_t ob0 = t * 128 + ((((g >> 1) | ((g & 1) << 2)) ^ t) << 4);          // R: chunk c(g)
     const uint32_t ob1 = (ob0 ^ 64) + 512;
     const uint32_t ox = EXTB * 8192 + t * 128 + (((g >> 2) ^ t) << 4) + (g & 3) * 4;    // [v | t]: column KR + g
+    const uint32_t oab = t * 64 + (((g >> 2) ^ (t >> 1)) << 4) + (g & 3) * 4;           // bf16 A: columns 2g, 2g+1 of a low-half m-block
     MmaAcc<MB0> acc0;
     MmaAcc<MB1> acc1;
     acc0.zero(); acc1.zero();
@@ -109,13 +113,26 @@ __device__ __forceinline__ void mma_warp(const BuildParams& prm, const unsigned 
         const unsigned char* ahi = base + SM::off_A + s * STAGE_A;
 #pragma unroll 1
         for (int pass = 0; pass < MODE; ++pass) {        // hi x hi, then A_lo x R, then A x R_lo, into the same accumulators
+            if constexpr (BB) { if (pass == 1) continue; }
             const unsigned char* a = pass == 1 ? base + SM::off_Alo : ahi;
             const unsigned char* r = base + (pass == 2 ? SM::off_Rlo : SM::off_R);
 #pragma unroll 1
             for (int kk = 0; kk < 8; ++kk) {
-                const unsigned char* ak = a + kk * 1024;
-                const unsigned char* rk = ak + (r - a);
+                const unsigned char* ak = a + kk * (BB ? 512 : 1024);
+                const unsigned char* rk = BB ? r + kk * 1024 : ak + (r - a);
                 uint32_t f0[4], f1[4];
+                if constexpr (BB) {
+                    if constexpr (MB0 >= 0) {
+                        const uint32_t lo = *reinterpret_cast<const uint32_t*>(ak + (MB0 >> 1) * 4096 + oab + 32 * (MB0 & 1));
+                        const uint32_t hi = *reinterpret_cast<const uint32_t*>(ak + (MB0 >> 1) * 4096 + 256 + oab + 32 * ((MB0 & 1) ^ 1));
+                        f0[0] = lo << 16; f0[1] = lo & 0xFFFF0000u; f0[2] = hi << 16; f0[3] = hi & 0xFFFF0000u;
+                    }
+                    if constexpr (MB1 >= 0) {
+                        const uint32_t lo = *reinterpret_cast<const uint32_t*>(ak + (MB1 >> 1) * 4096 + oab + 32 * (MB1 & 1));
+                        const uint32_t hi = *reinterpret_cast<const uint32_t*>(ak + (MB1 >> 1) * 4096 + 256 + oab + 32 * ((MB1 & 1) ^ 1));
+                        f1[0] = lo << 16; f1[1] = lo & 0xFFFF0000u; f1[2] = hi << 16; f1[3] = hi & 0xFFFF0000u;
+                    }
+                } else {
                 if constexpr (MB0 >= 0) {
                     const uint2 lo = *reinterpret_cast<const uint2*>(ak + (MB0 >> 1) * 8192 + oa + 64 * (MB0 & 1));
                     const uint2 hi = *reinterpret_cast<const uint2*>(ak + (MB0 >> 1) * 8192 + 512 + oa + 64 * ((MB0 & 1) ^ 1));
@@ -125,6 +142,7 @@ __device__ __forceinline__ void mma_warp(const BuildParams& prm, const unsigned 
                     const uint2 lo = *reinterpret_cast<const uint2*>(ak + (MB1 >> 1) * 8192 + oa + 64 * (MB1 & 1));
                     const uint2 hi = *reinterpret_cast<const uint2*>(ak + (MB1 >> 1) * 8192 + 512 + oa + 64 * ((MB1 & 1) ^ 1));
                     f1[0] = lo.x & 0xFFFFE000u; f1[1] = lo.y & 0xFFFFE000u; f1[2] = hi.x & 0xFFFFE000u; f1[3] = hi.y & 0xFFFFE000u;
+                }
                 }
 #pragma unroll
                 for (int G = 0; G < NG; ++G) {
@@ -171,12 +189,12 @@ __device__ __forceinline__ void mma_warp(const BuildParams& prm, const unsigned 
 }
 
 // The MMA warpgroup: dispatch once on the warp index mw (0..3) into its compile-time work split.
-template <class SM, int STAGE_A, int MODE, int KR>
+template <class SM, int STAGE_A, int MODE, int KR, bool BB = false>
 __device__ __forceinline__ void mma_role(const BuildParams& prm, const unsigned char* base, uint64_t* fullB, uint64_t* rready,
                                          uint64_t* rfree, long long t_begin, int ntiles, int mw, int lane)
 {
     constexpr int NMB = KR / 16;
-#define BANET_MMA_WARP(A, B) mma_warp<SM, STAGE_A, MODE, KR, A, B>(prm, base, fullB, rready, rfree, t_begin, ntiles, lane)
+#define BANET_MMA_WARP(A, B) mma_warp<SM, STAGE_A, MODE, KR, A, B, BB>(prm, base, fullB, rready, rfree, t_begin, ntiles, lane)
     if constexpr (NMB == 8) {
         switch (mw) { case 0: BANET_MMA_WARP(0, 7); break; case 1: BANET_MMA_WARP(1, 6); break;
                       case 2: BANET_MMA_WARP(2, 5); break; default: BANET_MMA_WARP(3, 4); break; }

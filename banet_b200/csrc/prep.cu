@@ -106,18 +106,19 @@ __global__ void resample_kernel(const TF* __restrict__ data, const float* __rest
     }
 }
 
-// bundlenet.py:397: depth = init_depth + basis . W.   Warp per output texel.
-__global__ void depth_compose_kernel(const float* __restrict__ init_depth, const float* __restrict__ basis,
+// bundlenet.py:397: depth = init_depth + basis . W.   Warp per output texel.  TB: basis element type (float, or bf16 widened on load).
+template <typename TB>
+__global__ void depth_compose_kernel(const float* __restrict__ init_depth, const TB* __restrict__ basis,
                                      const float* __restrict__ W, int nb, int M, int K, float* __restrict__ out)
 {
     const long long pt = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (pt >= (long long)nb * M) return;
     const int b = (int)(pt / M);
-    const float* br = basis + (size_t)pt * K;
+    const TB* br = basis + (size_t)pt * K;
     const float* wb = W + (size_t)b * K;
     float acc = 0.f;
-    for (int k = lane; k < K; k += 32) acc = fmaf(ld_stream_f1(br + k), __ldg(wb + k), acc);
+    for (int k = lane; k < K; k += 32) acc = fmaf(ld_stream_elem(br + k), __ldg(wb + k), acc);
     acc = warp_sum(acc);
     if (lane == 0) out[pt] = init_depth[pt] + acc;
 }
@@ -178,7 +179,8 @@ __global__ void resample_bwd_kernel(const float* __restrict__ dout, const float*
 }
 
 // Backward of depth_compose: dinit = dout; dbasis[pt][k] = dout[pt] W[k]; dW[k] += sum_pt dout[pt] basis[pt][k] (atomics; dW zero-filled).
-__global__ void depth_compose_bwd_kernel(const float* __restrict__ dout, const float* __restrict__ basis, const float* __restrict__ W,
+template <typename TB>
+__global__ void depth_compose_bwd_kernel(const float* __restrict__ dout, const TB* __restrict__ basis, const float* __restrict__ W,
                                          int nb, int M, int K, float* __restrict__ dbasis, float* __restrict__ dW)
 {
     const int b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -194,7 +196,11 @@ __global__ void depth_compose_bwd_kernel(const float* __restrict__ dout, const f
         for (int m = m0 + warp; m < m1; m += nw) {
             const size_t pt = (size_t)b * M + m;
             const float gv = dout[pt];
-            if (k < K) { acc = fmaf(gv, basis[pt * K + k], acc); dbasis[pt * K + k] = gv * wk; }
+            if (k < K) {
+                float bv;
+                if constexpr (sizeof(TB) == 4) bv = basis[pt * K + k]; else bv = ldg_feat(basis + pt * K + k);
+                acc = fmaf(gv, bv, acc); dbasis[pt * K + k] = gv * wk;
+            }
         }
         if (k < K) atomicAdd(&sacc[k], acc);
     }
@@ -227,15 +233,39 @@ extern "C" int banet_resample_bwd(const float* dout, const float* xy, float coor
     return BANET_OK;
 }
 
+namespace {
+template <typename TB>
+int depth_compose_bwd(const float* dout, const TB* basis, const float* W, int nb, int M, int K, float* dbasis, float* dW, cudaStream_t st,
+                      const char* who)
+{
+    BANET_REQUIRE(dout && basis && W && dbasis && dW && nb > 0 && M > 0 && K > 0 && K <= 8192, BANET_ERR_BAD_ARG, "%s: bad argument", who);
+    cudaMemsetAsync(dW, 0, (size_t)nb * K * sizeof(float), st);
+    int gx = (M + 1023) / 1024; if (gx < 1) gx = 1; if (gx > 64) gx = 64;
+    depth_compose_bwd_kernel<TB><<<dim3(gx, nb), 256, K * sizeof(float), st>>>(dout, basis, W, nb, M, K, dbasis, dW);
+    BANET_CUDA_LAUNCH_CHECK(who);
+    return BANET_OK;
+}
+template <typename TB>
+int depth_compose(const float* init_depth, const TB* basis, const float* W, int nb, int M, int K, float* out, cudaStream_t st, const char* who)
+{
+    BANET_REQUIRE(init_depth && basis && W && out && nb > 0 && M > 0 && K > 0, BANET_ERR_BAD_ARG, "%s: bad argument", who);
+    const long long thr = (long long)nb * M * 32;
+    depth_compose_kernel<TB><<<(unsigned)((thr + 255) / 256), 256, 0, st>>>(init_depth, basis, W, nb, M, K, out);
+    BANET_CUDA_LAUNCH_CHECK(who);
+    return BANET_OK;
+}
+}  // namespace
+
 extern "C" int banet_depth_compose_bwd(const float* dout, const float* basis, const float* W, int nb, int M, int K,
                                        float* dbasis, float* dW, banet_stream_t stream)
 {
-    BANET_REQUIRE(dout && basis && W && dbasis && dW && nb > 0 && M > 0 && K > 0 && K <= 8192, BANET_ERR_BAD_ARG, "depth_compose_bwd: bad argument");
-    cudaMemsetAsync(dW, 0, (size_t)nb * K * sizeof(float), (cudaStream_t)stream);
-    int gx = (M + 1023) / 1024; if (gx < 1) gx = 1; if (gx > 64) gx = 64;
-    depth_compose_bwd_kernel<<<dim3(gx, nb), 256, K * sizeof(float), (cudaStream_t)stream>>>(dout, basis, W, nb, M, K, dbasis, dW);
-    BANET_CUDA_LAUNCH_CHECK("depth_compose_bwd");
-    return BANET_OK;
+    return depth_compose_bwd(dout, basis, W, nb, M, K, dbasis, dW, (cudaStream_t)stream, "depth_compose_bwd");
+}
+
+extern "C" int banet_depth_compose_bwd_bf16(const float* dout, const void* basis, const float* W, int nb, int M, int K,
+                                            float* dbasis, float* dW, banet_stream_t stream)
+{
+    return depth_compose_bwd(dout, static_cast<const bf16*>(basis), W, nb, M, K, dbasis, dW, (cudaStream_t)stream, "depth_compose_bwd_bf16");
 }
 
 extern "C" int banet_compute_coordinates(const float* points, const float* intr, int nb, int N, int normalize,
@@ -298,9 +328,11 @@ extern "C" int banet_interpolate2d(const float* data, const float* xy, float coo
 extern "C" int banet_depth_compose(const float* init_depth, const float* basis, const float* W, int nb, int M, int K,
                                    float* out, banet_stream_t stream)
 {
-    BANET_REQUIRE(init_depth && basis && W && out && nb > 0 && M > 0 && K > 0, BANET_ERR_BAD_ARG, "depth_compose: bad argument");
-    const long long thr = (long long)nb * M * 32;
-    depth_compose_kernel<<<(unsigned)((thr + 255) / 256), 256, 0, (cudaStream_t)stream>>>(init_depth, basis, W, nb, M, K, out);
-    BANET_CUDA_LAUNCH_CHECK("depth_compose");
-    return BANET_OK;
+    return depth_compose(init_depth, basis, W, nb, M, K, out, (cudaStream_t)stream, "depth_compose");
+}
+
+extern "C" int banet_depth_compose_bf16(const float* init_depth, const void* basis, const float* W, int nb, int M, int K,
+                                        float* out, banet_stream_t stream)
+{
+    return depth_compose(init_depth, static_cast<const bf16*>(basis), W, nb, M, K, out, (cudaStream_t)stream, "depth_compose_bf16");
 }

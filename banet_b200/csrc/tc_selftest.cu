@@ -78,7 +78,7 @@ extern "C" int banet_tc_selftest(const float* A, const float* R, float* D, int m
 {
     BANET_REQUIRE(A && R && D, BANET_ERR_BAD_ARG, "tc_selftest: null pointer");
     CUtensorMap tm;
-    int rc = make_tmap_f32_2d_sw128(&tm, A, ST_PX, ST_M, ST_PX, 32);
+    int rc = make_tmap_basis_2d(&tm, A, false, ST_PX, ST_M, ST_PX, 32);
     if (rc) return rc;
     const size_t smem = 65536 + 40960 + 1024;
     cudaError_t e = cudaFuncSetAttribute(tc_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -151,6 +151,9 @@ __device__ __forceinline__ void mma_step_rn(float (&d)[4], const uint32_t (&af)[
 // Byte offset of (row r, 16-byte chunk c in 0..7) inside one [rows][128 B] block in the 128B swizzle as TMA writes it
 // (CU_TENSOR_MAP_SWIZZLE_128B, block base 1024-B aligned): the chunk index is XORed with (r & 7).
 __device__ __forceinline__ uint32_t sw128_off(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
+// The same for one [rows][64 B] block in the 64B swizzle (CU_TENSOR_MAP_SWIZZLE_64B, block base 512-B aligned): address bits 4-5 are
+// XORed with bits 7-8, so the 16-byte chunk index c in 0..3 is XORed with (r >> 1) & 3.  The bf16 basis tile: 32 columns per row.
+__device__ __forceinline__ uint32_t sw64_off(int r, int c) { return (uint32_t)(r * 64 + ((c ^ ((r >> 1) & 3)) << 4)); }
 
 __device__ __forceinline__ float tf32_rna(float x) {          // round to nearest tf32 (10-bit mantissa), ties away
     uint32_t u;

@@ -174,7 +174,8 @@ class ResizeHostSolver:
     Pairs are cut into chunks inside each half of the batch; the H2D copies of the images a later chunk needs overlap the solve of the
     current one (copy stream / compute stream).
     The pyramid keeps the host layers' dtype on the device: a bfloat16 pyramid (an autocast encoder's output) is copied at 2 bytes per
-    element and solved as bfloat16 levels; basis, depth and intrinsics are float32.  `h2d_bytes` counts the real element sizes."""
+    element and solved as bfloat16 levels.  So does the basis, independently: a bfloat16 host basis is copied at 2 bytes per element and
+    sampled by banet_resample_bf16 into bfloat16 levels.  Depth and intrinsics are float32.  `h2d_bytes` counts the real element sizes."""
 
     def __init__(self, layers: Sequence[Tensor], basis: Tensor, init_depth: Tensor, intr: Tensor, scales: Sequence[int], chunks: int = 4,
                  device=None, precision: int = PREC_AUTO):
@@ -195,7 +196,9 @@ class ResizeHostSolver:
         if fdt not in (torch.float32, torch.bfloat16) or any(t.dtype != fdt for t in self.h_layers):
             raise ValueError(f"layers must all be float32 or all bfloat16; got {[t.dtype for t in self.h_layers]}")
         self.d_layers = [torch.empty(t.shape, dtype=fdt, device=dev) for t in self.h_layers]
-        self.d_basis = torch.empty(basis.shape, dtype=torch.float32, device=dev)
+        if basis.dtype not in (torch.float32, torch.bfloat16):
+            raise ValueError(f"basis must be float32 or bfloat16; got {basis.dtype}")
+        self.d_basis = torch.empty(basis.shape, dtype=basis.dtype, device=dev)
         self.d_depth = torch.empty(init_depth.shape, dtype=torch.float32, device=dev)
         self.d_intr = torch.empty(intr.shape, dtype=torch.float32, device=dev)
         self.h2d_bytes = sum(t.numel() * t.element_size() for t in (*self.h_layers, basis, init_depth, intr))
@@ -206,7 +209,7 @@ class ResizeHostSolver:
             h, w = int(t.shape[1]), int(t.shape[2]); N = h * w
             vv, uu = torch.meshgrid(torch.arange(h, device=dev, dtype=torch.float32), torch.arange(w, device=dev, dtype=torch.float32), indexing="ij")
             self.pts.append(torch.stack([uu.reshape(-1), vv.reshape(-1)], -1).unsqueeze(0).repeat(nmax, 1, 1).contiguous())
-            self.scr.append({"B": torch.empty(nmax, N, self.K, device=dev), "D": torch.empty(nmax, N, 1, device=dev), "p": torch.empty(nmax, 3, N, device=dev)})
+            self.scr.append({"B": torch.empty(nmax, N, self.K, dtype=basis.dtype, device=dev), "D": torch.empty(nmax, N, 1, device=dev), "p": torch.empty(nmax, 3, N, device=dev)})
         self._ws: Optional[Tensor] = None
 
     def _chunk_levels(self, a: int, b: int) -> List[ops.Level]:
@@ -221,8 +224,9 @@ class ResizeHostSolver:
             ops.check(lib.banet_compute_coordinates(pts.data_ptr(), intr_l.data_ptr(), n, N, 1, scr["p"].data_ptr(), ops._stream()), "banet_compute_coordinates")
             ops.check(lib.banet_resample(self.d_depth[a:b].data_ptr(), pts.data_ptr(), s / 2.0, n, int(self.d_depth.shape[1]), int(self.d_depth.shape[2]), 1, N,
                                          scr["D"].data_ptr(), ops._stream()), "banet_resample")
-            ops.check(lib.banet_resample(self.d_basis[a:b].data_ptr(), pts.data_ptr(), s / 2.0, n, int(self.d_basis.shape[1]), int(self.d_basis.shape[2]), self.K, N,
-                                         scr["B"].data_ptr(), ops._stream()), "banet_resample")
+            rs = "banet_resample_bf16" if self.d_basis.dtype == torch.bfloat16 else "banet_resample"
+            ops.check(getattr(lib, rs)(self.d_basis[a:b].data_ptr(), pts.data_ptr(), s / 2.0, n, int(self.d_basis.shape[1]), int(self.d_basis.shape[2]), self.K, N,
+                                       scr["B"].data_ptr(), ops._stream()), rs)
             levels.append(ops.Level(dl[a:b].reshape(n, N, self.C), dl[a2:a2 + n], intr_l, scr["p"][:n], scr["D"][:n], scr["B"][:n], grid=(w, h)))
         return levels
 

@@ -16,11 +16,11 @@ from ._lib import BanetLevel, BanetSolveOpts, check, load
 Tensor = torch.Tensor
 
 
-_FEATURE_DTYPES = {torch.float32: _lib.DTYPE_F32, torch.bfloat16: _lib.DTYPE_BF16}
+_FEATURE_DTYPES = {torch.float32: _lib.DTYPE_F32, torch.bfloat16: _lib.DTYPE_BF16}      # also the basis dtypes
 
 
 def _chk(t: Tensor, name: str, shape: Optional[Tuple[int, ...]] = None, features: bool = False) -> Tensor:
-    """features=True: a feature map (conv1 / conv2 / resampler data), which may also be bfloat16."""
+    """features=True: a feature map (conv1 / conv2 / resampler data) or a depth basis, which may also be bfloat16."""
     if not isinstance(t, torch.Tensor) or not t.is_cuda:
         raise _lib.BanetError(f"{name}: expected a CUDA tensor (banet_b200 has no CPU path)")
     if t.dtype != torch.float32 and not (features and t.dtype == torch.bfloat16):
@@ -147,13 +147,14 @@ def interpolate2d(data: Tensor, xy: Tensor, coord_scale: float = 1.0, with_mask:
 
 
 def depth_compose(init_depth: Tensor, basis: Tensor, W: Tensor) -> Tensor:
-    """init_depth [nb,M], basis [nb,M,K], W [nb,K,1] -> [nb,M]   (reference bundlenet.py:397)."""
+    """init_depth [nb,M], basis [nb,M,K], W [nb,K,1] -> [nb,M]   (reference bundlenet.py:397).  basis may be bfloat16
+    (banet_depth_compose_bf16: widened where it is read); everything else and the result are float32."""
     lib = load()
-    bs = _chk(basis, "basis"); nb, M, K = bs.shape
+    bs = _chk(basis, "basis", features=True); nb, M, K = bs.shape
     d0 = _chk(init_depth, "init_depth", (nb, M)); Wt = _chk(W, "W", (nb, K, 1))
     out = torch.empty(nb, M, device=bs.device, dtype=torch.float32)
-    check(lib.banet_depth_compose(d0.data_ptr(), bs.data_ptr(), Wt.data_ptr(), nb, M, K, out.data_ptr(), _stream()),
-          "banet_depth_compose")
+    name = "banet_depth_compose_bf16" if bs.dtype == torch.bfloat16 else "banet_depth_compose"
+    check(getattr(lib, name)(d0.data_ptr(), bs.data_ptr(), Wt.data_ptr(), nb, M, K, out.data_ptr(), _stream()), name)
     return out
 
 
@@ -166,7 +167,7 @@ class Level:
     intr: Tensor              # [nb,4]
     p: Tensor                 # [nb,3,N]
     D: Tensor                 # [nb,N,1]
-    B: Optional[Tensor]       # [nb,N,K] or None
+    B: Optional[Tensor]       # [nb,N,K] or None; float32 or bfloat16, independent of the features' dtype
     grid: Optional[Tuple[int, int]] = None   # (grid_w, grid_h) if the N points are a row-major raster grid (locality hint)
 
     def as_struct(self) -> Tuple[BanetLevel, list]:
@@ -175,7 +176,7 @@ class Level:
         if conv1.dtype != conv2.dtype:
             raise _lib.BanetError(f"conv1 ({conv1.dtype}) and conv2 ({conv2.dtype}) must have the same dtype (float32 or bfloat16)")
         intr = _chk(self.intr, "intr", (nb, 4)); p = _chk(self.p, "p", (nb, 3, N)); D = _chk(self.D, "D", (nb, N, 1))
-        B = None if self.B is None else _chk(self.B, "B")
+        B = None if self.B is None else _chk(self.B, "B", features=True)
         K = 0 if B is None else B.shape[2]
         if B is not None and tuple(B.shape[:2]) != (nb, N):
             raise _lib.BanetError(f"B: expected [nb,N,K]=[{nb},{N},K], got {tuple(B.shape)}")
@@ -186,7 +187,7 @@ class Level:
         if gw * gh not in (0, N):
             raise _lib.BanetError(f"grid {gw}x{gh} does not match N={N}")
         return BanetLevel(nb, N, Cc, K, h, w, c2, conv1.data_ptr(), conv2.data_ptr(), intr.data_ptr(), p.data_ptr(),
-                          D.data_ptr(), _ptr(B), gw, gh, _FEATURE_DTYPES[conv1.dtype]), keep
+                          D.data_ptr(), _ptr(B), gw, gh, _FEATURE_DTYPES[conv1.dtype], _FEATURE_DTYPES[torch.float32 if B is None else B.dtype]), keep
 
 
 def lm_build(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], precision: int = _lib.PREC_AUTO):
@@ -550,7 +551,7 @@ def lm_run_workspace_bytes(levels: Sequence[Level], precision: int = _lib.PREC_A
 def lm_build_bwd(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], dH: Tensor, dg: Tensor, drbar_sum: Tensor, exact_sym: bool = False):
     """Backward of lm_build (banet_lm_build_bwd) -> dconv1, dconv2, dD, dB, dR, dT, dW.  dconv2 has conv2's layout: [nb,h,w,3C] for
     [F2|gx|gy], [nb,h,w,C] for F2 only (the adjoint of the on-the-fly gradient stencil is applied inside the kernel).  dconv1 and dconv2
-    are float32 also for bfloat16 features (the kernel accumulates them with fp32 atomics)."""
+    are float32 also for bfloat16 features (the kernel accumulates them with fp32 atomics), and dB is float32 also for a bfloat16 basis."""
     lib = load()
     st, keep = level.as_struct()
     nb, K, Cc, N = st.nb, st.K, st.C, st.N
@@ -651,11 +652,13 @@ def resample_bwd(dout: Tensor, xy: Tensor, coord_scale: float, h: int, w: int) -
 
 
 def depth_compose_bwd(dout: Tensor, basis: Tensor, W: Tensor):
+    """-> dbasis [nb,M,K], dW [nb,K,1], both float32 (also for a bfloat16 basis: banet_depth_compose_bwd_bf16)."""
     lib = load()
-    bs = _chk(basis, "basis"); nb, M, K = bs.shape
+    bs = _chk(basis, "basis", features=True); nb, M, K = bs.shape
     g = _chk(dout, "dout", (nb, M)); Wt = _chk(W, "W", (nb, K, 1))
-    dbasis = torch.empty_like(bs); dW = torch.empty(nb, K, 1, device=bs.device)
-    check(lib.banet_depth_compose_bwd(g.data_ptr(), bs.data_ptr(), Wt.data_ptr(), nb, M, K, dbasis.data_ptr(), dW.data_ptr(), _stream()), "banet_depth_compose_bwd")
+    dbasis = torch.empty(nb, M, K, device=bs.device); dW = torch.empty(nb, K, 1, device=bs.device)
+    name = "banet_depth_compose_bwd_bf16" if bs.dtype == torch.bfloat16 else "banet_depth_compose_bwd"
+    check(getattr(lib, name)(g.data_ptr(), bs.data_ptr(), Wt.data_ptr(), nb, M, K, dbasis.data_ptr(), dW.data_ptr(), _stream()), name)
     return dbasis, dW
 
 

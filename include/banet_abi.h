@@ -104,13 +104,14 @@ int banet_interpolate2d(const float* data, const float* xy, float coord_scale, i
  * (3) Layer level — one LM iteration = BundleNet.BundleIteration (bundlenet.py:193-278) or
  *     BundleNet.CameraIteration (:122-191) when K == 0 / B == NULL.
  * ---------------------------------------------------------------------------------------------- */
-/* Element type of conv1 and conv2 (banet_level_t::feature_dtype).  Every other tensor of the library is fp32.  bf16 features are
- * widened to fp32 exactly where they are read; all arithmetic stays fp32. */
+/* Element types of conv1 and conv2 (banet_level_t::feature_dtype) and of the depth basis B (banet_level_t::basis_dtype).  Every other
+ * tensor of the library is fp32.  bf16 inputs are widened to fp32 exactly where they are read; all arithmetic stays fp32. */
 #define BANET_DTYPE_F32  0
 #define BANET_DTYPE_BF16 1
 
-/* feature_dtype is the last field, so a zero-initialised struct keeps fp32 features.  It changed sizeof(banet_level_t) and therefore
- * the stride of every levels[] array: code compiled against a header without the field cannot pass level arrays to this library. */
+/* feature_dtype and basis_dtype are the last fields, so a zero-initialised struct keeps fp32 features and an fp32 basis.  Each of them
+ * changed sizeof(banet_level_t) and therefore the stride of every levels[] array: code compiled against a header without both fields
+ * cannot pass level arrays to this library. */
 typedef struct banet_level {
     int nb, N, C, K;          /* pairs, points per pair, feature channels, depth bases (0 = pose only) */
     int h, w;                 /* conv2 map size at this level */
@@ -120,7 +121,7 @@ typedef struct banet_level {
     const float* intr;        /* [nb,4] fx,fy,ox,oy at this level (reference tiles them to [nb,N], :379-382) */
     const float* p;           /* [nb,3,N]      :358 */
     const float* D;           /* [nb,N,1]      :343 */
-    const float* B;           /* [nb,N,K] or NULL  :344 */
+    const void* B;            /* [nb,N,K] or NULL  :344  (element type: basis_dtype) */
     int grid_w, grid_h;       /* locality hint, results do not depend on it: 0,0 = unstructured point list; otherwise the N points
                                  are the row-major raster grid x<grid_w, y<grid_h (N == grid_w*grid_h) and the kernels walk it in
                                  8x8 tiles so that every conv2 texel is fetched from HBM about once */
@@ -128,6 +129,10 @@ typedef struct banet_level {
                                  BANET_ERR_BAD_ARG.  bf16 levels run the fp32 SIMT build and tensor-core generation 6 (never generation 7),
                                  are rejected by banet_lm_track_legacy (BANET_ERR_UNSUPPORTED), and their banet_lm_build_bwd writes
                                  dconv1 / dconv2 as fp32 buffers */
+    int basis_dtype;          /* BANET_DTYPE_F32 (0) or BANET_DTYPE_BF16 (1) for B, independent of feature_dtype; any other value is
+                                 BANET_ERR_BAD_ARG in every entry that takes levels (also where B is not read: K = 0, the legacy tracker).
+                                 bf16 bases run the fp32 SIMT build and tensor-core generation 6 (never generation 7), and their
+                                 banet_lm_build_bwd writes dB as an fp32 buffer */
 } banet_level_t;
 
 #define BANET_PREC_AUTO    (-1)   /* the level-wise policy (TF32_LEVELWISE) where the tensor-core path applies (K in {32,64,128}, C in {64,128}), else FP32_SIMT */
@@ -192,7 +197,7 @@ int    banet_lm_step(const float* H, const float* g, const float* rbar_sum, int 
  * dT [nb,3,1], dW [nb,K,1]; every output is overwritten.  conv2 may be either layout banet_lm_build takes: the
  * reference's [F2|gx|gy] (3C), or F2 only (C), whose dconv2 is the gradient w.r.t. F2 through the build's on-the-fly
  * REFLECT-by-one gradient stencil.  exact_sym as in banet_eqc_bwd (0 = the reference's 2*A*Ghat).  dconv1 and dconv2 are fp32 whatever
- * the level's feature_dtype (dconv2 is accumulated with fp32 atomics); a bf16 caller rounds them once. */
+ * the level's feature_dtype (dconv2 is accumulated with fp32 atomics), and dB is fp32 whatever its basis_dtype; a bf16 caller rounds them once. */
 int    banet_lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W,
                           const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
                           float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
@@ -217,6 +222,9 @@ int    banet_resample_bwd(const float* dout, const float* xy, float coord_scale,
 /* Backward of banet_depth_compose: dout [nb,M] -> dbasis [nb,M,K], dW [nb,K,1] (overwritten); d init_depth = dout. */
 int    banet_depth_compose_bwd(const float* dout, const float* basis, const float* W, int nb, int M, int K,
                                float* dbasis, float* dW, banet_stream_t stream);
+/* Backward of banet_depth_compose_bf16: basis bf16 [nb,M,K]; dbasis [nb,M,K] and dW [nb,K,1] fp32 (overwritten). */
+int    banet_depth_compose_bwd_bf16(const float* dout, const void* basis, const float* W, int nb, int M, int K,
+                                    float* dbasis, float* dW, banet_stream_t stream);
 
 /* Whole coarse-to-fine solve: for each level, `iters_per_level` iterations of
  * build -> lambda -> solve/update, with W carried across levels (the level loop of
@@ -395,6 +403,9 @@ int    banet_lm_track_legacy(const banet_level_t* levels, int nlevels, const int
  *   basis [nb,M,K] (M = h/2*w/2), W [nb,K,1], init_depth [nb,M] -> out [nb,M] */
 int banet_depth_compose(const float* init_depth, const float* basis, const float* W, int nb, int M, int K,
                         float* out, banet_stream_t stream);
+/* The same on a bf16 basis [nb,M,K] (widened where it is read; init_depth, W and out fp32).  Its backward is banet_depth_compose_bwd_bf16. */
+int banet_depth_compose_bf16(const float* init_depth, const void* basis, const float* W, int nb, int M, int K,
+                             float* out, banet_stream_t stream);
 
 /* Diagnostic (not part of the reference's interface): one 64-pixel k-tile through the TMA + tcgen05 building
  * blocks of the tensor-core build path.  A [64,128], R [64,160] -> D [128,160] = A^T R.
