@@ -20,14 +20,14 @@ c_stream = C.c_void_p
 
 
 class BanetLevel(C.Structure):
-    """struct banet_level (include/banet_abi.h).  feature_dtype and basis_dtype are last, so a struct built without them keeps fp32
-    features and an fp32 basis."""
+    """struct banet_level (include/banet_abi.h).  feature_dtype, basis_dtype and weight are last, so a struct built without them keeps
+    fp32 features, an fp32 basis and no point weights."""
     _fields_ = [("nb", C.c_int), ("N", C.c_int), ("C", C.c_int), ("K", C.c_int),
                 ("h", C.c_int), ("w", C.c_int), ("conv2_channels", C.c_int),
                 ("conv1", C.c_void_p), ("conv2", C.c_void_p), ("intr", C.c_void_p),
                 ("p", C.c_void_p), ("D", C.c_void_p), ("B", C.c_void_p),
                 ("grid_w", C.c_int), ("grid_h", C.c_int), ("feature_dtype", C.c_int),
-                ("basis_dtype", C.c_int)]
+                ("basis_dtype", C.c_int), ("weight", C.c_void_p)]
 
 
 class BanetKeyframeLevel(C.Structure):
@@ -121,6 +121,7 @@ SIGNATURES = {
     "banet_lm_track_legacy": (C.c_int, [C.POINTER(BanetLevel), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_void_p), C.POINTER(BanetLegacyOpts)]
                               + [c_float_p] * 2 + [C.c_void_p, c_float_p, C.c_void_p] + [C.c_void_p, C.c_size_t, c_stream]),
     "banet_lm_build_bwd": (C.c_int, [C.POINTER(BanetLevel)] + [c_float_p] * 6 + [C.c_int] + [c_float_p] * 7 + [c_stream]),
+    "banet_lm_build_bwd_weighted": (C.c_int, [C.POINTER(BanetLevel)] + [c_float_p] * 6 + [C.c_int] + [c_float_p] * 8 + [c_stream]),
     "banet_lm_solve_update_bwd": (C.c_int, [c_float_p] * 4 + [C.c_int, C.c_int, C.POINTER(BanetSolveOpts)] + [c_float_p] * 5 + [c_float_p] * 6 + [c_stream]),
     "banet_grad_fixed_concat_bwd": (C.c_int, [c_float_p] + [C.c_int] * 5 + [c_float_p, c_stream]),
     "banet_resample_bwd": (C.c_int, [c_float_p, c_float_p, C.c_float] + [C.c_int] * 5 + [c_float_p, c_stream]),

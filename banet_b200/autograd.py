@@ -139,32 +139,39 @@ def iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_b
 class _LMBuildFn(torch.autograd.Function):
     """(H, g, rbar_sum) = banet_lm_build(...); backward = banet_lm_build_bwd.  conv2 is the [F2|gx|gy] tensor or F2 only; dconv2 comes back
     in conv2's layout.  bfloat16 features and a bfloat16 basis are saved as they are; their gradients are accumulated in fp32 by the kernel
-    and cast once."""
+    and cast once.  weight [nb,N,1] (or None): the per-point weight of H and g; its gradient is banet_lm_build_bwd_weighted's dweight."""
 
     @staticmethod
-    def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, precision, exact_sym, grid):
-        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=grid)
+    def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, precision, exact_sym, grid, weight):
+        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=grid, weight=weight)
         H, g, rbar, nvalid = ops.lm_build(lv, R, T, W, precision)
-        ctx.save_for_backward(conv1, conv2, D, B if B is not None else conv1.new_empty(0), R, T, W if W is not None else conv1.new_empty(0), intr, p)
-        ctx.has_basis = B is not None
+        empty = conv1.new_empty(0)
+        ctx.save_for_backward(conv1, conv2, D, B if B is not None else empty, R, T, W if W is not None else empty, intr, p,
+                              weight if weight is not None else empty)
+        ctx.has_basis = B is not None; ctx.has_weight = weight is not None
         ctx.exact_sym = bool(exact_sym); ctx.grid = grid
         ctx.mark_non_differentiable(nvalid)
         return H, g, rbar, nvalid
 
     @staticmethod
     def backward(ctx, dH, dg, drbar, _dnvalid):
-        conv1, conv2, D, B, R, T, W, intr, p = ctx.saved_tensors
+        conv1, conv2, D, B, R, T, W, intr, p, weight = ctx.saved_tensors
         if not ctx.has_basis:
             B = None; W = None
-        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=ctx.grid)
+        if not ctx.has_weight:
+            weight = None
+        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=ctx.grid, weight=weight)
         nb = conv1.shape[0]
         P = 6 + (0 if B is None else B.shape[2])
         dH = dH.contiguous() if dH is not None else torch.zeros(nb, P, P, device=conv1.device)
         dg = dg if dg is not None else torch.zeros(nb, P, device=conv1.device)
         drbar = drbar if drbar is not None else torch.zeros(nb, conv1.shape[2], device=conv1.device)
-        dconv1, dconv2, dD, dB, dR, dT, dW = ops.lm_build_bwd(lv, R, T, W, dH, dg.contiguous(), drbar.contiguous(), ctx.exact_sym)
+        want_dw = weight is not None and ctx.needs_input_grad[12]
+        grads = ops.lm_build_bwd(lv, R, T, W, dH, dg.contiguous(), drbar.contiguous(), ctx.exact_sym, return_dweight=want_dw)
+        dconv1, dconv2, dD, dB, dR, dT, dW = grads[:7]
+        dweight = grads[7] if want_dw else None
         dB = None if dB is None else dB.to(B.dtype)
-        return dconv1.to(conv1.dtype), dconv2.to(conv2.dtype), dD, dB, dR, dT, dW, None, None, None, None, None
+        return dconv1.to(conv1.dtype), dconv2.to(conv2.dtype), dD, dB, dR, dT, dW, None, None, None, None, None, dweight
 
 
 class _KeyframeBuildFn(torch.autograd.Function):
@@ -325,15 +332,16 @@ def depth_compose(init_depth: Tensor, basis: Tensor, W: Tensor) -> Tensor:
 
 def iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base: Optional[float],
                     damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None,
-                    precision: int = 0, grid=None, return_status: bool = False):
+                    precision: int = 0, grid=None, return_status: bool = False, weight: Optional[Tensor] = None):
     """One differentiable LM iteration on the fused kernels.  Same arguments / returns as `iteration`; an F2-only conv2 [nb,h,w,C] goes
     straight into the build and its backward (the gradient stencil's adjoint runs inside banet_lm_build_bwd).
     precision: contraction mode of the FORWARD build (the backward is fp32); default FP32_SIMT, the reference's arithmetic type.
     conv1 / conv2 may be bfloat16 (both), and so may B (independently): they are read as they are, and their gradients come back in
-    bfloat16."""
+    bfloat16.  weight [nb,N,1] float32: per-point confidence of the normal equations (H = sum w_n H_n, g = sum w_n g_n; lambda does not
+    see it); differentiable."""
     nb, N, C = conv1.shape
     bundle = B is not None
-    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, W, intr.detach(), p.detach(), precision, exact_sym, grid)
+    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, W, intr.detach(), p.detach(), precision, exact_sym, grid, weight)
     if lambda_override is not None:
         lam = lambda_override.reshape(nb)
     else:
@@ -365,7 +373,7 @@ def window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_
     conv1, intr, p, D, B = frames(conv1), frames(intr), frames(p), frames(D), frames(B)
     N = conv1.shape[1]
     Wf = W.reshape(1, K, 1).expand(nf, K, 1).contiguous()                       # every pair builds with the shared W; dW sums over them
-    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, Wf, intr.detach(), p.detach(), precision, exact_sym, grid)
+    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, Wf, intr.detach(), p.detach(), precision, exact_sym, grid, None)
     if lambda_override is not None:
         lam = lambda_override.reshape(1)
     else:
@@ -401,7 +409,7 @@ def window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_param
     N, C = conv1.shape[1], conv1.shape[2]
     Wf = W.reshape(nw, 1, K, 1).expand(nw, nf, K, 1).reshape(nb, K, 1).contiguous()   # every pair builds with its window's W
     Rf, Tf = R.reshape(nb, 3, 3), T.reshape(nb, 3, 1)
-    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, Rf, Tf, Wf, intr.detach(), p.detach(), precision, exact_sym, grid)
+    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, Rf, Tf, Wf, intr.detach(), p.detach(), precision, exact_sym, grid, None)
     if lambda_override is not None:
         lam = lambda_override.reshape(nw)
     else:

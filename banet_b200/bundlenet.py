@@ -106,13 +106,15 @@ class BundleNet(torch.nn.Module):
         if self.strict_status and int(status.abs().max()) != 0:
             raise RuntimeError(f"LM solve skipped a step for pairs {torch.nonzero(status).flatten().tolist()} (status {status.tolist()})")
 
-    def _iterate(self, conv1, conv2, intr, p, D, B, R, T, W, base, level, grid=None):
-        """One iteration, differentiable or not; returns (R', T', W', aux or None)."""
+    def _iterate(self, conv1, conv2, intr, p, D, B, R, T, W, base, level, grid=None, weight=None):
+        """One iteration, differentiable or not; returns (R', T', W', aux or None).  weight [nb,N,1]: per-point weight of H and g."""
         bundle = B is not None
-        if self._wants_grad(conv1, conv2, D, B, R, T, W):
+        if self._wants_grad(conv1, conv2, D, B, R, T, W, weight):
             if self.vmatrix_batch_scramble:
                 raise RuntimeError("vmatrix_batch_scramble=True (the reference's batch-interleaved VMatrix, bundlenet.py:45) is not differentiable here")
             if self.training_path == "reference_split":
+                if weight is not None:
+                    raise RuntimeError("training_path='reference_split' has no point weights; weighted iterations train on the fused path")
                 if conv1.dtype != torch.float32 or conv2.dtype != torch.float32:
                     raise RuntimeError("training_path='reference_split' takes float32 features; bfloat16 features train on the fused path")
                 if bundle and B.dtype != torch.float32:
@@ -121,34 +123,39 @@ class BundleNet(torch.nn.Module):
                                            exact_sym=self.exact_sym_grad)
                 return Rn, Tn, Wn, None
             Rn, Tn, Wn, status = _ag.iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base if bundle else None,
-                                                     exact_sym=self.exact_sym_grad, precision=self.precision, grid=grid, return_status=True)
+                                                     exact_sym=self.exact_sym_grad, precision=self.precision, grid=grid, return_status=True,
+                                                     weight=weight)
             self._check_status(status)
             return Rn, Tn, Wn, None
-        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=grid)
+        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=grid, weight=weight)
         H, g, rbar, nvalid = ops.lm_build(lv, R, T, W, self.precision)
         lam = ops.lm_lambda(rbar, conv1.shape[1], self.mlp_packed(str(level)), float(base) if bundle else 1.0)
         Rn, Tn, Wn, delta, status = ops.lm_solve_update(H, g, lam, R, T, W, undamped_last=bundle, vmatrix_batch_scramble=self.vmatrix_batch_scramble)
         self._check_status(status)
         return Rn, Tn, Wn, dict(AtA=H, Atb=g, lam=lam, rbar_sum=rbar, nvalid=nvalid, solution=delta, status=status)
 
-    def CameraIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, R, T, l2_regularizer_base=None, level=None, return_aux: bool = False):
+    def CameraIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, R, T, l2_regularizer_base=None, level=None, return_aux: bool = False, *,
+                        weight: Optional[Tensor] = None):
         """reference bundlenet.py:122-191 -> (updatedR, updatedT).  l2_regularizer_base accepted, unused (as there).
-        Differentiable (fused backward kernels) whenever gradients are being recorded; `return_aux` needs the no-grad path."""
+        Differentiable (fused backward kernels) whenever gradients are being recorded; `return_aux` needs the no-grad path.
+        weight [nb,N,1] float32 (an extension): per-point confidence of the normal equations, H = sum_n w_n H_n, g = sum_n w_n g_n; the
+        damping lambda does not see it.  Differentiable on the fused training path."""
         if return_aux:
             with torch.no_grad():
-                Rn, Tn, _, aux = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, None, R, T, None, 1.0, level)
+                Rn, Tn, _, aux = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, None, R, T, None, 1.0, level, weight=weight)
             return Rn, Tn, aux
-        Rn, Tn, _, _ = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, None, R, T, None, 1.0, level)
+        Rn, Tn, _, _ = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, None, R, T, None, 1.0, level, weight=weight)
         return Rn, Tn
 
-    def BundleIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, l2_regularizer_base=None, level=None, return_aux: bool = False):
-        """reference bundlenet.py:193-278 -> (updatedR, updatedT, updatedW)."""
+    def BundleIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, l2_regularizer_base=None, level=None, return_aux: bool = False, *,
+                        weight: Optional[Tensor] = None):
+        """reference bundlenet.py:193-278 -> (updatedR, updatedT, updatedW).  weight [nb,N,1]: as in CameraIteration."""
         base = 1.0 if l2_regularizer_base is None else float(l2_regularizer_base)      # :252-253
         if return_aux:
             with torch.no_grad():
-                Rn, Tn, Wn, aux = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, B, R, T, W, base, level)
+                Rn, Tn, Wn, aux = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, B, R, T, W, base, level, weight=weight)
             return Rn, Tn, Wn, aux
-        Rn, Tn, Wn, _ = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, B, R, T, W, base, level)
+        Rn, Tn, Wn, _ = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, B, R, T, W, base, level, weight=weight)
         return Rn, Tn, Wn
 
     def WindowIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, l2_regularizer_base=None, level=None):
@@ -261,13 +268,15 @@ class BundleNet(torch.nn.Module):
             return torch.cat([layer[h:], layer[:h]]).contiguous()
         return gfc(layer, swap_halves=True)
 
-    def CameraResize(self, intrisic, layers, points, _depths, reuse_variables=False):
+    def CameraResize(self, intrisic, layers, points, _depths, reuse_variables=False, weight: Optional[Tensor] = None):
         """reference bundlenet.py:280-329 -> (rotations, translations), levels 0..3 x 1 iteration.  Differentiable w.r.t. the feature
         pyramid and the lambda-MLP parameters when gradients are being recorded (the depth is stop_gradient'ed, :288).
-        `layers` may be bfloat16 (an autocast encoder's pyramid): conv1 is then the bfloat16 resample and conv2 the half-swapped F2 only."""
+        `layers` may be bfloat16 (an autocast encoder's pyramid): conv1 is then the bfloat16 resample and conv2 the half-swapped F2 only.
+        weight [nb,N,1] float32 (an extension): a per-point confidence at `points`, the same at every level (see CameraIteration);
+        differentiable when it requires grad."""
         nb = layers[-1].shape[0]
         _points, intr = self._prepare(intrisic, points)
-        grad = self._wants_grad(*layers)
+        grad = self._wants_grad(*layers, weight)
         resample, gfc = (_ag.resample, _ag.grad_fixed_concat) if grad else (ops.resample, ops.grad_fixed_concat)
         d = ops.resample(_depths.detach(), _points, 0.5)                       # :289-290
         p = ops.compute_coordinates(_points, intr, True)
@@ -278,23 +287,25 @@ class BundleNet(torch.nn.Module):
             scale = 2 ** (3 - level)
             layer1 = resample(layers[level], _points, 1.0 / scale)             # :320
             layer2 = self._swapped_f2(layers[level], gfc)                      # :321-324
-            R, T, _, _ = self._iterate(layer1, layer2, intr / scale, p, d, None, R, T, None, 1.0, level)
+            R, T, _, _ = self._iterate(layer1, layer2, intr / scale, p, d, None, R, T, None, 1.0, level, weight=weight)
             rotations.append(R); translations.append(T)
         return rotations, translations
 
     def BundleResize(self, intrisic, layers, points, basis, init_depth, init_rotation=None, init_translation=None,
-                     reuse_variables=False):
+                     reuse_variables=False, weight: Optional[Tensor] = None):
         """reference bundlenet.py:332-399 -> (output_rotations, output_translations, output_depths), levels 2,3.  Differentiable w.r.t.
         the feature pyramid, the basis, the initial pose and the lambda-MLP parameters when gradients are being recorded
         (init_depth enters the LM only through stop_gradient, :341, and the output depth directly, :397).
         `layers` may be bfloat16 (an autocast encoder's pyramid): conv1 is then the bfloat16 resample and conv2 the half-swapped F2 only;
         their gradients come back in bfloat16.  `basis` may be bfloat16 too, independently of the pyramid (an autocast decoder's depth basis):
         it is sampled by the bfloat16 resample, the output depth is composed on it (banet_depth_compose_bf16), and its gradient comes back in
-        bfloat16.  init_depth stays float32."""
+        bfloat16.  init_depth stays float32.
+        weight [nb,N,1] float32 (an extension): a per-point confidence at `points`, the same at both levels (see CameraIteration);
+        differentiable when it requires grad."""
         nb = layers[-1].shape[0]
         K = basis.shape[-1]
         _points, intr = self._prepare(intrisic, points)
-        grad = self._wants_grad(*layers, basis, init_depth, init_rotation, init_translation)
+        grad = self._wants_grad(*layers, basis, init_depth, init_rotation, init_translation, weight)
         resample, gfc, compose = (_ag.resample, _ag.grad_fixed_concat, _ag.depth_compose) if grad else (ops.resample, ops.grad_fixed_concat, ops.depth_compose)
         d = ops.resample(init_depth.detach(), _points, 0.5)                    # :341-343
         b = resample(basis, _points, 0.5)                                      # :344
@@ -309,7 +320,7 @@ class BundleNet(torch.nn.Module):
             scale = 2 ** (3 - level)
             layer1 = resample(layers[level], _points, 1.0 / scale)             # :385
             layer2 = self._swapped_f2(layers[level], gfc)                      # :386-389
-            R, T, W, _ = self._iterate(layer1, layer2, intr / scale, p, d, b, R, T, W, 1000.0, level)   # :393
+            R, T, W, _ = self._iterate(layer1, layer2, intr / scale, p, d, b, R, T, W, 1000.0, level, weight=weight)   # :393
             Rs.append(R); Ts.append(T)
             depth = compose(init_depth.reshape(nb, -1), basis.reshape(nb, -1, K), W)   # :397
             Ds.append(depth.reshape(nb, oh, ow, 1))

@@ -189,15 +189,23 @@ extern "C" int banet_lm_step(const float* H, const float* g, const float* rbar_s
                    R_out, T_out, W_out, delta, lambda_out, status, 0, (cudaStream_t)stream);
 }
 
-extern "C" int banet_lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W,
-                                  const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
-                                  float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, banet_stream_t stream)
+extern "C" int banet_lm_build_bwd_weighted(const banet_level_t* lv, const float* R, const float* T, const float* W,
+                                           const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
+                                           float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
+                                           float* dweight, banet_stream_t stream)
 {
     int rc = check_level(lv, "lm_build_bwd");
     if (rc) return rc;
     BANET_REQUIRE(R && T && dH && dg && drbar_sum && dconv1 && dconv2 && dD && dR && dT, BANET_ERR_BAD_ARG, "lm_build_bwd: null pointer");
     BANET_REQUIRE(lv->K == 0 || (W && dB && dW), BANET_ERR_BAD_ARG, "lm_build_bwd: K=%d but W / dB / dW is null", lv->K);
-    return lm_build_bwd(lv, R, T, W, dH, dg, drbar_sum, exact_sym, dconv1, dconv2, dD, dB, dR, dT, dW, (cudaStream_t)stream);
+    return lm_build_bwd(lv, R, T, W, dH, dg, drbar_sum, exact_sym, dconv1, dconv2, dD, dB, dR, dT, dW, dweight, (cudaStream_t)stream);
+}
+
+extern "C" int banet_lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W,
+                                  const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
+                                  float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, banet_stream_t stream)
+{
+    return banet_lm_build_bwd_weighted(lv, R, T, W, dH, dg, drbar_sum, exact_sym, dconv1, dconv2, dD, dB, dR, dT, dW, nullptr, stream);
 }
 
 extern "C" int banet_lm_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int K, const banet_solve_opts_t* opts,
@@ -711,6 +719,8 @@ extern "C" int banet_lm_track_legacy(const banet_level_t* levels, int nlevels, c
         if (rc) return rc;
         BANET_REQUIRE(levels[l].feature_dtype == BANET_DTYPE_F32, BANET_ERR_UNSUPPORTED,
                       "lm_track_legacy: level %d has bf16 features; the legacy tracker takes fp32 features only", l);
+        BANET_REQUIRE(!levels[l].weight, BANET_ERR_UNSUPPORTED,
+                      "lm_track_legacy: level %d has point weights; the tracker's accept / reject test re-evaluates an unweighted residual", l);
         BANET_REQUIRE(levels[l].K == 0 && levels[l].nb == levels[0].nb && levels[l].conv2_channels == 3 * levels[l].C && level_iters[l] >= 0, BANET_ERR_BAD_ARG,
                       "lm_track_legacy: level %d must be pose-only (K=0) with the [F2|gx|gy] layout and the same batch size", l);
     }

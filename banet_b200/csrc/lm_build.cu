@@ -320,7 +320,9 @@ lm_build_kernel(const BuildParams prm)
                     }
                     ra.store_smem(myRb + c);
                 }
-                m11 = warp_sum(m11); m12 = warp_sum(m12); m22 = warp_sum(m22); q1 = warp_sum(q1); q2 = warp_sum(q2);
+                // point weight: scales M and q, i.e. every block of H and g; sum |diff| and nvalid stay unweighted (x * 1.0f is exact)
+                const float wn = prm.weight ? __ldg(prm.weight + (size_t)b * N + n0 + n) : 1.f;
+                m11 = warp_sum(m11) * wn; m12 = warp_sum(m12) * wn; m22 = warp_sum(m22) * wn; q1 = warp_sum(q1) * wn; q2 = warp_sum(q2) * wn;
             }
             if (lane == 0) {
                 rec[R_M11 * TILE_PX + n] = m11; rec[R_M12 * TILE_PX + n] = m12; rec[R_M22 * TILE_PX + n] = m22;
@@ -522,7 +524,7 @@ int lm_build_simt(const banet_level_t* lv, const BuildPlan& plan, const float* R
     BuildParams prm;
     prm.nb = lv->nb; prm.N = lv->N; prm.C = lv->C; prm.K = lv->K; prm.h = lv->h; prm.w = lv->w; prm.c2 = lv->conv2_channels;
     prm.conv1 = lv->conv1; prm.conv2 = lv->conv2; prm.intr = lv->intr; prm.p = lv->p; prm.D = lv->D; prm.B = lv->B;
-    prm.R = R; prm.T = T; prm.W = W;
+    prm.R = R; prm.T = T; prm.W = W; prm.weight = lv->weight;
     prm.partials = reinterpret_cast<float*>(ws);
     prm.slot_floats = plan.slot_floats; prm.max_span = plan.max_span;
     prm.tiles_per_pair = plan.tiles_per_pair; prm.total_tiles = plan.total_tiles;

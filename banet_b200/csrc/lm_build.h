@@ -10,6 +10,7 @@ struct BuildParams {
     const float *intr, *p, *D;
     const void* B;                    // element type: the level's basis_dtype (the kernels' TB template parameter)
     const float *R, *T, *W;
+    const float* weight;              // [nb,N] per-point weight of M, q, or NULL (= 1)
     float* partials;
     int slot_floats, max_span, tiles_per_pair;
     long long total_tiles;
@@ -119,7 +120,7 @@ int lm_track_legacy(const banet_level_t* levels, int nlevels, const int* level_i
 
 // backward of one iteration (lm_bwd.cu)
 int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dH, const float* dg, const float* drbar,
-                 int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, cudaStream_t st);
+                 int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, float* dweight, cudaStream_t st);
 int lm_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int K, const banet_solve_opts_t& opts,
                         const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
                         float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, cudaStream_t st);

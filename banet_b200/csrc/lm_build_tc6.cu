@@ -222,9 +222,10 @@ __device__ __forceinline__ void gather_bf16(const BuildParams& prm, const int* s
                 }
             }
             m11 = hsum16(m11); m12 = hsum16(m12); m22 = hsum16(m22); q1 = hsum16(q1); q2 = hsum16(q2);
-            if (hl == 0) {           // totals overwrite dx,dy / n of this pixel's record (as the fp32 gather does)
-                *reinterpret_cast<float4*>(rec + pl * REC + 12) = make_float4(m11, m12, m22, q1);
-                rec[pl * REC + 11] = q2;
+            if (hl == 0) {           // totals overwrite dx,dy / n of this pixel's record (as the fp32 gather does), times the point weight
+                const float wn = (prm.weight && mask != 0.f) ? __ldg(prm.weight + (size_t)b * N + __float_as_int(rec[pl * REC + 11])) : 1.f;
+                *reinterpret_cast<float4*>(rec + pl * REC + 12) = make_float4(m11 * wn, m12 * wn, m22 * wn, q1 * wn);
+                rec[pl * REC + 11] = q2 * wn;
             }
         }
         __syncwarp();
@@ -583,8 +584,10 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                 if (jc == NCH - 1) {
                     m11 = hsum16(m11); m12 = hsum16(m12); m22 = hsum16(m22); q1 = hsum16(q1); q2 = hsum16(q2);
                     if (hl == 0) {           // totals overwrite dx,dy / n of this pixel's record (no longer needed; the tap offsets stay for the prefetcher)
-                        *reinterpret_cast<float4*>(rec + pl * REC + 12) = make_float4(m11, m12, m22, q1);
-                        rec[pl * REC + 11] = q2;
+                        // point weight (M and q, i.e. every block of H and g; sum |d| stays unweighted): x * 1.0f is exact
+                        const float wn = (prm.weight && mask != 0.f) ? __ldg(prm.weight + (size_t)b * N + __float_as_int(rec[pl * REC + 11])) : 1.f;
+                        *reinterpret_cast<float4*>(rec + pl * REC + 12) = make_float4(m11 * wn, m12 * wn, m22 * wn, q1 * wn);
+                        rec[pl * REC + 11] = q2 * wn;
                     }
                 }
             }

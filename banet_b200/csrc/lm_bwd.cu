@@ -12,7 +12,8 @@
 //   In block form the only K^2 work per pixel is e = b^T S_dd; everything else is O(K):
 //     Y_c = Jc S_cc + jd (b^T S_dc)     Y_d b = Jc (S_cd b) + jd (e.b)     db = s e + S_cd^T v + t ghat_d + dDt W
 //   then the chain rule through the sampler (features: atomics into dconv2; coordinates: tap differences), the projection, the
-//   warp (dR, dT), and the depth update (dD, dB, dW).
+//   warp (dR, dT), and the depth update (dD, dB, dW).  With point weights (H = sum w_n H_n, g = sum w_n g_n) the Ghat / ghat adjoints of
+//   pixel n are scaled by w_n and dw_n = 1/2 <M, Q> + q.z, stored by its one writer.
 // lm_solve_update_bwd_kernel: delta = Ht^-1 g, Ht = H + diag(damp (diag H + eps)) lambda  ->  u = Ht^-1 ddelta, dg = u, dHt = -u delta^T,
 //   dH = dHt (1 + damp lambda on the diagonal), dlambda = sum_i dHt_ii damp_i (H_ii + eps); ddelta from the SE(3) update by forward-mode
 //   dual numbers over the same expressions as pose_update_kernel (lm_solve.cu).
@@ -36,6 +37,8 @@ struct BwdParams {
     const float *R, *T, *W;
     const float *dH, *dg, *drbar;
     float *dconv1, *dconv2, *dD, *dB, *dR, *dT, *dW;
+    const float* weight;                         // [nb,N] point weights, or NULL (= 1)
+    float* dweight;                              // [nb,N] their gradient, or NULL
     int exact_sym, tiles_per_pair;
     long long total_tiles;
 };
@@ -189,7 +192,7 @@ lm_build_bwd_kernel(const BwdParams prm)
                 for (int c = lane; c < C; c += 32) dc1[c] = 0.f;
 #pragma unroll
                 for (int i = 0; i < BWD_KL; ++i) { const int k = lane + 32 * i; if (k < K) prm.dB[gi * K + k] = 0.f; }
-                if (lane == 0) prm.dD[gi] = 0.f;
+                if (lane == 0) { prm.dD[gi] = 0.f; if (prm.dweight) prm.dweight[gi] = 0.f; }
                 continue;
             }
             const float fu = floorf(u), fv = floorf(v);
@@ -270,6 +273,13 @@ lm_build_bwd_kernel(const BwdParams prm)
             float Q00 = yb0 * jd0, Q01 = yb0 * jd1, Q10 = yb1 * jd0, Q11 = yb1 * jd1;
 #pragma unroll
             for (int i = 0; i < 6; ++i) { Q00 = fmaf(Yc0[i], a0[i], Q00); Q01 = fmaf(Yc0[i], a1[i], Q01); Q10 = fmaf(Yc1[i], a0[i], Q10); Q11 = fmaf(Yc1[i], a1[i], Q11); }
+            // ---- point weight: dw = <Ghat, H_n> + <ghat, g_n> = 1/2 <M, Q> + q.z (H_n = J^T M J is symmetric, so this is exact for both
+            //      S conventions).  Every adjoint that comes from Ghat, ghat is point n's times w_n: scaling M, q carries it to dJ and db,
+            //      scaling Q, z to dG and dd; the rhat sign(d) path is not weighted.  Unweighted: w_n = 1 and x * 1.0f is exact.
+            const float wn = prm.weight ? __ldg(prm.weight + gi) : 1.f;
+            if (prm.dweight && lane == 0) prm.dweight[gi] = 0.5f * (m11 * Q00 + m12 * (Q01 + Q10) + m22 * Q11) + (q1 * z0 + q2 * z1);
+            m11 *= wn; m12 *= wn; m22 *= wn; q1 *= wn; q2 *= wn;
+            Q00 *= wn; Q01 *= wn; Q10 *= wn; Q11 *= wn; z0 *= wn; z1 *= wn;
             float dJ0[6], dJ1[6];
 #pragma unroll
             for (int i = 0; i < 6; ++i) { dJ0[i] = m11 * Yc0[i] + m12 * Yc1[i] + q1 * sg[i]; dJ1[i] = m12 * Yc0[i] + m22 * Yc1[i] + q2 * sg[i]; }
@@ -355,7 +365,7 @@ static void (*select_bwd_kernel(int K, bool c3))(const BwdParams)
 }
 
 int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dH, const float* dg, const float* drbar,
-                 int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, cudaStream_t st)
+                 int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, float* dweight, cudaStream_t st)
 {
     const int K = lv->K, P = 6 + K;
     BANET_REQUIRE(K <= 32 * BWD_KL_MAX, BANET_ERR_UNSUPPORTED, "lm_build_bwd: K=%d > %d", K, 32 * BWD_KL_MAX);
@@ -372,6 +382,7 @@ int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const 
     prm.conv1 = lv->conv1; prm.conv2 = lv->conv2; prm.intr = lv->intr; prm.p = lv->p; prm.D = lv->D; prm.B = lv->B; prm.R = R; prm.T = T; prm.W = W;
     prm.dH = dH; prm.dg = dg; prm.drbar = drbar;
     prm.dconv1 = dconv1; prm.dconv2 = dconv2; prm.dD = dD; prm.dB = dB; prm.dR = dR; prm.dT = dT; prm.dW = dW;
+    prm.weight = lv->weight; prm.dweight = dweight;
     prm.exact_sym = exact_sym;
     prm.tiles_per_pair = (lv->N + BWD_TILE - 1) / BWD_TILE;
     prm.total_tiles = (long long)lv->nb * prm.tiles_per_pair;

@@ -169,6 +169,7 @@ class Level:
     D: Tensor                 # [nb,N,1]
     B: Optional[Tensor]       # [nb,N,K] or None; float32 or bfloat16, independent of the features' dtype
     grid: Optional[Tuple[int, int]] = None   # (grid_w, grid_h) if the N points are a row-major raster grid (locality hint)
+    weight: Optional[Tensor] = None          # [nb,N,1] float32 per-point weight of the normal equations (H, g); None = unweighted
 
     def as_struct(self) -> Tuple[BanetLevel, list]:
         conv1 = _chk(self.conv1, "conv1", features=True); nb, N, Cc = conv1.shape
@@ -182,12 +183,14 @@ class Level:
             raise _lib.BanetError(f"B: expected [nb,N,K]=[{nb},{N},K], got {tuple(B.shape)}")
         if conv2.shape[0] != nb:
             raise _lib.BanetError("conv2 batch mismatch")
-        keep = [conv1, conv2, intr, p, D, B]
+        wt = None if self.weight is None else _chk(self.weight, "weight", (nb, N, 1))
+        keep = [conv1, conv2, intr, p, D, B, wt]
         gw, gh = (0, 0) if self.grid is None else self.grid
         if gw * gh not in (0, N):
             raise _lib.BanetError(f"grid {gw}x{gh} does not match N={N}")
         return BanetLevel(nb, N, Cc, K, h, w, c2, conv1.data_ptr(), conv2.data_ptr(), intr.data_ptr(), p.data_ptr(),
-                          D.data_ptr(), _ptr(B), gw, gh, _FEATURE_DTYPES[conv1.dtype], _FEATURE_DTYPES[torch.float32 if B is None else B.dtype]), keep
+                          D.data_ptr(), _ptr(B), gw, gh, _FEATURE_DTYPES[conv1.dtype], _FEATURE_DTYPES[torch.float32 if B is None else B.dtype],
+                          _ptr(wt)), keep
 
 
 def lm_build(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], precision: int = _lib.PREC_AUTO):
@@ -548,10 +551,13 @@ def lm_run_workspace_bytes(levels: Sequence[Level], precision: int = _lib.PREC_A
 
 
 # ------------------------------------------------------------------------------------------ backward of one iteration
-def lm_build_bwd(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], dH: Tensor, dg: Tensor, drbar_sum: Tensor, exact_sym: bool = False):
+def lm_build_bwd(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], dH: Tensor, dg: Tensor, drbar_sum: Tensor, exact_sym: bool = False,
+                 return_dweight: bool = False):
     """Backward of lm_build (banet_lm_build_bwd) -> dconv1, dconv2, dD, dB, dR, dT, dW.  dconv2 has conv2's layout: [nb,h,w,3C] for
     [F2|gx|gy], [nb,h,w,C] for F2 only (the adjoint of the on-the-fly gradient stencil is applied inside the kernel).  dconv1 and dconv2
-    are float32 also for bfloat16 features (the kernel accumulates them with fp32 atomics), and dB is float32 also for a bfloat16 basis."""
+    are float32 also for bfloat16 features (the kernel accumulates them with fp32 atomics), and dB is float32 also for a bfloat16 basis.
+    On a weighted level every gradient carries the point weights.  return_dweight=True appends dweight [nb,N,1] = <dH, H_n> + <dg, g_n>
+    (banet_lm_build_bwd_weighted; on an unweighted level, the gradient at weights of ones)."""
     lib = load()
     st, keep = level.as_struct()
     nb, K, Cc, N = st.nb, st.K, st.C, st.N
@@ -563,10 +569,17 @@ def lm_build_bwd(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], dH: Te
     dconv1 = torch.empty(nb, N, Cc, device=dev); dconv2 = torch.empty(nb, st.h, st.w, st.conv2_channels, device=dev)
     dD = torch.empty(nb, N, 1, device=dev); dB = None if K == 0 else torch.empty(nb, N, K, device=dev)
     dR = torch.empty(nb, 3, 3, device=dev); dT = torch.empty(nb, 3, 1, device=dev); dW = None if K == 0 else torch.empty(nb, K, 1, device=dev)
-    check(lib.banet_lm_build_bwd(C.byref(st), R.data_ptr(), T.data_ptr(), _ptr(Wt), dH.data_ptr(), dg.data_ptr(), dr.data_ptr(), int(bool(exact_sym)),
-                                 dconv1.data_ptr(), dconv2.data_ptr(), dD.data_ptr(), _ptr(dB), dR.data_ptr(), dT.data_ptr(), _ptr(dW), _stream()),
-          "banet_lm_build_bwd")
-    return dconv1, dconv2, dD, dB, dR, dT, dW
+    if not return_dweight:
+        check(lib.banet_lm_build_bwd(C.byref(st), R.data_ptr(), T.data_ptr(), _ptr(Wt), dH.data_ptr(), dg.data_ptr(), dr.data_ptr(), int(bool(exact_sym)),
+                                     dconv1.data_ptr(), dconv2.data_ptr(), dD.data_ptr(), _ptr(dB), dR.data_ptr(), dT.data_ptr(), _ptr(dW), _stream()),
+              "banet_lm_build_bwd")
+        return dconv1, dconv2, dD, dB, dR, dT, dW
+    dweight = torch.empty(nb, N, 1, device=dev)
+    check(lib.banet_lm_build_bwd_weighted(C.byref(st), R.data_ptr(), T.data_ptr(), _ptr(Wt), dH.data_ptr(), dg.data_ptr(), dr.data_ptr(),
+                                          int(bool(exact_sym)), dconv1.data_ptr(), dconv2.data_ptr(), dD.data_ptr(), _ptr(dB), dR.data_ptr(),
+                                          dT.data_ptr(), _ptr(dW), dweight.data_ptr(), _stream()),
+          "banet_lm_build_bwd_weighted")
+    return dconv1, dconv2, dD, dB, dR, dT, dW, dweight
 
 
 def lm_solve_update_bwd(H: Tensor, g: Tensor, lam: Tensor, delta: Tensor, R: Tensor, T: Tensor, dRn: Tensor, dTn: Tensor, dWn: Optional[Tensor],

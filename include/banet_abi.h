@@ -109,9 +109,9 @@ int banet_interpolate2d(const float* data, const float* xy, float coord_scale, i
 #define BANET_DTYPE_F32  0
 #define BANET_DTYPE_BF16 1
 
-/* feature_dtype and basis_dtype are the last fields, so a zero-initialised struct keeps fp32 features and an fp32 basis.  Each of them
- * changed sizeof(banet_level_t) and therefore the stride of every levels[] array: code compiled against a header without both fields
- * cannot pass level arrays to this library. */
+/* feature_dtype, basis_dtype and weight are the last fields, so a zero-initialised struct keeps fp32 features, an fp32 basis and no
+ * point weights.  Each of them changed sizeof(banet_level_t) and therefore the stride of every levels[] array: code compiled against a
+ * header without all three fields cannot pass level arrays to this library. */
 typedef struct banet_level {
     int nb, N, C, K;          /* pairs, points per pair, feature channels, depth bases (0 = pose only) */
     int h, w;                 /* conv2 map size at this level */
@@ -133,6 +133,12 @@ typedef struct banet_level {
                                  BANET_ERR_BAD_ARG in every entry that takes levels (also where B is not read: K = 0, the legacy tracker).
                                  bf16 bases run the fp32 SIMT build and tensor-core generation 6 (never generation 7), and their
                                  banet_lm_build_bwd writes dB as an fp32 buffer */
+    const float* weight;      /* [nb,N,1] or NULL: per-point confidence w_n of the normal equations, H = sum_n w_n J_n^T M_n J_n and
+                                 g = sum_n w_n J_n^T q_n (every block: H_cc, H_cd, H_dd, g_c, g_d); rbar_sum and nvalid stay unweighted,
+                                 so lambda does not see it.  Used as given: a negative weight can make H indefinite (solve status 1), a
+                                 non-finite one gives status 2.  NULL is the unweighted arithmetic bit for bit, and so are weights of
+                                 ones.  Weighted levels never run generation 7 and are rejected by banet_lm_track_legacy
+                                 (BANET_ERR_UNSUPPORTED); the whole-solve entries honour them per pair */
 } banet_level_t;
 
 #define BANET_PREC_AUTO    (-1)   /* the level-wise policy (TF32_LEVELWISE) where the tensor-core path applies (K in {32,64,128}, C in {64,128}), else FP32_SIMT */
@@ -202,6 +208,15 @@ int    banet_lm_build_bwd(const banet_level_t* lv, const float* R, const float* 
                           const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
                           float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
                           banet_stream_t stream);
+/* The same, plus the gradient of the level's point weights: dweight [nb,N,1] (may be NULL; overwritten otherwise),
+ *   dw_n = <dH, H_n> + <dg, g_n>   (H_n, g_n: point n's unweighted contributions; masked points get 0).
+ * On a weighted level every other gradient that comes from dH, dg is point n's times w_n (the drbar_sum path is not weighted);
+ * banet_lm_build_bwd is this call with dweight = NULL.  On an unweighted level dweight is the gradient at weights of ones.
+ * Argument errors are those of banet_lm_build_bwd, reported before any CUDA call. */
+int    banet_lm_build_bwd_weighted(const banet_level_t* lv, const float* R, const float* T, const float* W,
+                                   const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
+                                   float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
+                                   float* dweight, banet_stream_t stream);
 /* Backward of banet_lm_solve_update: gradients of (R',T',W') [dR_out,dT_out,dW_out] -> dH [nb,P,P], dg [nb,P],
  * dlambda [nb], dR, dT, dW.  `delta` [nb,P] is the solution the forward call returned.  Pairs whose forward step was
  * skipped (status != 0, delta = 0) pass the pose/depth gradients through and get zero dH, dg, dlambda.
