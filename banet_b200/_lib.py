@@ -31,11 +31,12 @@ class BanetLevel(C.Structure):
 
 
 class BanetKeyframeLevel(C.Structure):
-    """struct banet_keyframe_level (include/banet_abi.h): the keyframe tensors once per window, the frame tensors per pair."""
+    """struct banet_keyframe_level (include/banet_abi.h): the keyframe tensors once per window, the frame tensors per pair.  weight is
+    last, so a struct built without it has no point weights."""
     _fields_ = [("nw", C.c_int), ("nf", C.c_int), ("N", C.c_int), ("C", C.c_int), ("K", C.c_int),
                 ("h", C.c_int), ("w", C.c_int), ("conv2_channels", C.c_int),
                 ("conv1", C.c_void_p), ("p", C.c_void_p), ("D", C.c_void_p), ("B", C.c_void_p),
-                ("conv2", C.c_void_p), ("intr", C.c_void_p)]
+                ("conv2", C.c_void_p), ("intr", C.c_void_p), ("weight", C.c_void_p)]
 
 
 class BanetSolveOpts(C.Structure):
@@ -109,6 +110,7 @@ SIGNATURES = {
     "banet_lm_keyframe_build_workspace_bytes": (C.c_size_t, [C.POINTER(BanetKeyframeLevel)]),
     "banet_lm_keyframe_build": (C.c_int, [C.POINTER(BanetKeyframeLevel)] + [c_float_p] * 3 + [c_float_p] * 4 + [C.c_void_p, C.c_size_t, c_stream]),
     "banet_lm_keyframe_build_bwd": (C.c_int, [C.POINTER(BanetKeyframeLevel)] + [c_float_p] * 6 + [C.c_int] + [c_float_p] * 7 + [c_stream]),
+    "banet_lm_keyframe_build_bwd_weighted": (C.c_int, [C.POINTER(BanetKeyframeLevel)] + [c_float_p] * 6 + [C.c_int] + [c_float_p] * 8 + [c_stream]),
     "banet_lm_keyframe_run_workspace_bytes": (C.c_size_t, [C.POINTER(BanetKeyframeLevel), C.c_int, C.c_int]),
     "banet_lm_keyframe_run": (C.c_int, [C.POINTER(BanetKeyframeLevel), C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_float, C.c_float,
                                         C.POINTER(BanetSolveOpts), C.c_int] + [c_float_p] * 3 + [C.c_void_p]

@@ -177,27 +177,34 @@ class _LMBuildFn(torch.autograd.Function):
 class _KeyframeBuildFn(torch.autograd.Function):
     """(H, g, rbar_sum) = banet_lm_keyframe_build(...) (the window-reduced per-pair system); backward = banet_lm_keyframe_build_bwd.
     conv1 [nw,N,C], D, B, p once per window; conv2, intr, R, T per pair; W [nw,K,1].  Saves the inputs only: no per-frame copy of the
-    keyframe."""
+    keyframe.  weight [nw*nf,N,1] (or None): the per-(frame, point) weight of H and g; its gradient is
+    banet_lm_keyframe_build_bwd_weighted's dweight."""
 
     @staticmethod
-    def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, exact_sym):
-        lv = ops.KeyframeLevel(conv1, conv2, intr, p, D, B)
+    def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, exact_sym, weight):
+        lv = ops.KeyframeLevel(conv1, conv2, intr, p, D, B, weight=weight)
         H, g, rbar, nvalid = ops.lm_keyframe_build(lv, R, T, W)
-        ctx.save_for_backward(conv1, conv2, D, B, R, T, W, intr, p)
+        ctx.save_for_backward(conv1, conv2, D, B, R, T, W, intr, p, weight if weight is not None else conv1.new_empty(0))
+        ctx.has_weight = weight is not None
         ctx.exact_sym = bool(exact_sym)
         ctx.mark_non_differentiable(nvalid)
         return H, g, rbar, nvalid
 
     @staticmethod
     def backward(ctx, dH, dg, drbar, _dnvalid):
-        conv1, conv2, D, B, R, T, W, intr, p = ctx.saved_tensors
-        lv = ops.KeyframeLevel(conv1, conv2, intr, p, D, B)
+        conv1, conv2, D, B, R, T, W, intr, p, weight = ctx.saved_tensors
+        if not ctx.has_weight:
+            weight = None
+        lv = ops.KeyframeLevel(conv1, conv2, intr, p, D, B, weight=weight)
         nb, P = R.shape[0], 6 + B.shape[2]
         dH = dH.contiguous() if dH is not None else torch.zeros(nb, P, P, device=conv1.device)
         dg = dg if dg is not None else torch.zeros(nb, P, device=conv1.device)
         drbar = drbar if drbar is not None else torch.zeros(nb, conv1.shape[2], device=conv1.device)
-        dconv1, dconv2, dD, dB, dR, dT, dW = ops.lm_keyframe_build_bwd(lv, R, T, W, dH, dg.contiguous(), drbar.contiguous(), ctx.exact_sym)
-        return dconv1, dconv2, dD, dB, dR, dT, dW.reshape(W.shape), None, None, None
+        want_dw = weight is not None and ctx.needs_input_grad[10]
+        grads = ops.lm_keyframe_build_bwd(lv, R, T, W, dH, dg.contiguous(), drbar.contiguous(), ctx.exact_sym, return_dweight=want_dw)
+        dconv1, dconv2, dD, dB, dR, dT, dW = grads[:7]
+        dweight = grads[7] if want_dw else None
+        return dconv1, dconv2, dD, dB, dR, dT, dW.reshape(W.shape), None, None, None, dweight
 
 
 class _LMSolveUpdateFn(torch.autograd.Function):
@@ -359,21 +366,37 @@ def iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regular
     return Rn, Tn, Wn
 
 
+def window_weights(weight: Tensor, nw: Optional[int], nf: int, N: int) -> Tensor:
+    """Point weights of keyframe windows -> the per-pair layout [nw*nf,N,1] (pair w*nf + f).  weight: [nw,nf,N,1] or [nw,1,N,1]
+    (nw None: [nf,N,1] or [1,N,1]), float32; a frame axis of 1 is broadcast to the frames, and its gradient is summed over them."""
+    from . import _lib
+    lead = () if nw is None else (int(nw),)
+    want = "[" + ",".join([str(x) for x in lead] + [f"{nf}|1", str(N), "1"]) + "]"
+    if not isinstance(weight, torch.Tensor) or weight.dtype != torch.float32:
+        raise _lib.BanetError(f"weight: expected a float32 tensor {want}, got {getattr(weight, 'dtype', type(weight).__name__)}")
+    k = len(lead)
+    if weight.dim() != k + 3 or tuple(weight.shape[:k]) != lead or weight.shape[k] not in (1, nf) or tuple(weight.shape[k + 1:]) != (N, 1):
+        raise _lib.BanetError(f"weight: expected shape {want}, got {tuple(weight.shape)}")
+    return weight.expand(*lead, nf, N, 1).reshape(-1, N, 1).contiguous()
+
+
 def window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base: Optional[float],
                            damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None,
-                           precision: int = 0, grid=None, return_status: bool = False):
+                           precision: int = 0, grid=None, return_status: bool = False, weight: Optional[Tensor] = None):
     """One differentiable LM iteration of a keyframe window (the joint solve of ops.lm_window_run) on the fused kernels: nf pairs
     (keyframe -> frame f) share W [K,1]; R [nf,3,3], T [nf,3,1] and conv2 [nf,h,w,3C] (or [nf,h,w,C], F2 only) are per frame.  The keyframe tensors conv1, p, D, B
     (and intr) may be given once ([1,...]): they are broadcast to the frames and their gradients summed over them.  lambda: from the mean
     |residual| over all points of all frames through the MLP (times l2_regularizer_base), or lambda_override [1].
+    weight [nf,N,1] or [1,N,1] float32: per-(frame, point) confidence of the normal equations (lambda does not see it); differentiable.
     Returns (R', T', W' [K,1]) (, status [nf])."""
     nf = R.shape[0]
     K = B.shape[-1]
     frames = lambda t: t.expand(nf, *t.shape[1:]).contiguous() if t.shape[0] == 1 and nf > 1 else t
     conv1, intr, p, D, B = frames(conv1), frames(intr), frames(p), frames(D), frames(B)
     N = conv1.shape[1]
+    wf = None if weight is None else window_weights(weight, None, nf, N)
     Wf = W.reshape(1, K, 1).expand(nf, K, 1).contiguous()                       # every pair builds with the shared W; dW sums over them
-    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, Wf, intr.detach(), p.detach(), precision, exact_sym, grid, None)
+    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, Wf, intr.detach(), p.detach(), precision, exact_sym, grid, wf)
     if lambda_override is not None:
         lam = lambda_override.reshape(1)
     else:
@@ -389,7 +412,7 @@ def window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_
 
 def window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base: Optional[float],
                                  damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None,
-                                 precision: int = 0, grid=None, return_status: bool = False):
+                                 precision: int = 0, grid=None, return_status: bool = False, weight: Optional[Tensor] = None):
     """One differentiable LM iteration of a batch of nw keyframe windows of nf frames (window_iteration_fused per window, one launch each
     for the build, the step and their backwards).  R [nw,nf,3,3], T [nw,nf,3,1], conv2 [nw,nf,h,w,3C] (or [nw,nf,h,w,C], F2 only) per frame,
     W [nw,K,1] per window; the keyframe tensors conv1, p, D, B (and intr) are [nw,nf,...] or [nw,1,...] (broadcast to the frames, their gradients summed over them).
@@ -397,19 +420,22 @@ def window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_param
     Given WITHOUT a frame axis (conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K]; intr [nw,nf|1,4]), the keyframe tensors take the keyframe
     build (banet_lm_keyframe_build / _bwd): nothing is copied per frame and their gradients come back as [nw,...]; precision must be AUTO or
     FP32_SIMT there, and conv2 must be [F2|gx|gy] when it requires grad (the keyframe backward takes that layout only).
+    weight [nw,nf,N,1] or [nw,1,N,1] float32, in both forms: per-(frame, point) confidence of the normal equations (lambda does not see it);
+    differentiable.
     Returns (R' [nw,nf,3,3], T' [nw,nf,3,1], W' [nw,K,1]) (, status [nw,nf])."""
     if conv1.dim() == 3:
         return _keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base, damping_eps, exact_sym,
-                                         lambda_override, precision, return_status)
+                                         lambda_override, precision, return_status, weight)
     nw, nf = R.shape[0], R.shape[1]
     K = B.shape[-1]
     nb = nw * nf
     pairs = lambda t: (t.expand(nw, nf, *t.shape[2:]) if t.shape[1] == 1 and nf > 1 else t).reshape(nb, *t.shape[2:]).contiguous()
     conv1, conv2, intr, p, D, B = pairs(conv1), pairs(conv2), pairs(intr), pairs(p), pairs(D), pairs(B)
     N, C = conv1.shape[1], conv1.shape[2]
+    wf = None if weight is None else window_weights(weight, nw, nf, N)
     Wf = W.reshape(nw, 1, K, 1).expand(nw, nf, K, 1).reshape(nb, K, 1).contiguous()   # every pair builds with its window's W
     Rf, Tf = R.reshape(nb, 3, 3), T.reshape(nb, 3, 1)
-    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, Rf, Tf, Wf, intr.detach(), p.detach(), precision, exact_sym, grid, None)
+    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, Rf, Tf, Wf, intr.detach(), p.detach(), precision, exact_sym, grid, wf)
     if lambda_override is not None:
         lam = lambda_override.reshape(nw)
     else:
@@ -425,7 +451,7 @@ def window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_param
 
 
 def _keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base, damping_eps, exact_sym, lambda_override,
-                              precision, return_status):
+                              precision, return_status, weight=None):
     """window_batch_iteration_fused with the keyframe tensors once per window (conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K]): the
     keyframe build (banet_lm_keyframe_build / _bwd) gives the window-reduced per-pair system, which the window step takes as it is.  Nothing
     of the keyframe is copied per frame; its gradients come back as [nw,...]."""
@@ -448,7 +474,8 @@ def _keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, 
     intr = intr.expand(nw, nf, 4).reshape(nb, 4).contiguous()
     conv2 = conv2.reshape(nb, *conv2.shape[2:])
     Rf, Tf = R.reshape(nb, 3, 3), T.reshape(nb, 3, 1)
-    H, g, rbar_sum, _nvalid = _KeyframeBuildFn.apply(conv1, conv2, D, B, Rf, Tf, W.reshape(nw, K, 1), intr.detach(), p.detach(), exact_sym)
+    wf = None if weight is None else window_weights(weight, nw, nf, N)
+    H, g, rbar_sum, _nvalid = _KeyframeBuildFn.apply(conv1, conv2, D, B, Rf, Tf, W.reshape(nw, K, 1), intr.detach(), p.detach(), exact_sym, wf)
     if lambda_override is not None:
         lam = lambda_override.reshape(nw)
     else:

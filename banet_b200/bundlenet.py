@@ -158,35 +158,40 @@ class BundleNet(torch.nn.Module):
         Rn, Tn, Wn, _ = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, B, R, T, W, base, level, weight=weight)
         return Rn, Tn, Wn
 
-    def WindowIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, l2_regularizer_base=None, level=None):
+    def WindowIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, l2_regularizer_base=None, level=None, *,
+                        weight: Optional[Tensor] = None):
         """One joint LM iteration of a keyframe window (an extension; the reference's layer is 2-view): the nf pairs (keyframe -> frame f)
         share the keyframe depth D + B.W.  Arguments as BundleIteration with R [nf,3,3], T [nf,3,1], conv2 [nf,h,w,3C] (or F2 only, [nf,h,w,C]) per frame and
         W [K,1] shared; the keyframe tensors conv1, p, D, B may be given once ([1,...]) or per frame.  -> (updatedR, updatedT, updatedW [K,1]).
         Differentiable (banet_lm_window_solve_update_bwd) whenever gradients are being recorded; there is no reference_split twin.
         A batch of nw windows: R [nw,nf,3,3], T [nw,nf,3,1], conv2 [nw,nf,h,w,3C] (or [nw,nf,h,w,C]), W [nw,K,1], keyframe tensors and fx, fy, ox, oy
-        [nw,1,...] or [nw,nf,...] -> ([nw,nf,3,3], [nw,nf,3,1], [nw,K,1]), last_status [nw,nf] (banet_lm_window_batch_*)."""
+        [nw,1,...] or [nw,nf,...] -> ([nw,nf,3,3], [nw,nf,3,1], [nw,K,1]), last_status [nw,nf] (banet_lm_window_batch_*).
+        weight (an extension) float32: a per-(frame, keyframe point) confidence of the normal equations (see CameraIteration), [nf|1,N,1] for
+        one window, [nw,nf|1,N,1] for a batch (a frame axis of 1 is broadcast to the frames); differentiable when it requires grad."""
         base = 1.0 if l2_regularizer_base is None else float(l2_regularizer_base)
         if self.vmatrix_batch_scramble:
             raise RuntimeError("vmatrix_batch_scramble=True is a 2-view quirk (bundlenet.py:45); the window solve has per-frame VMatrix only")
         if R.dim() == 4:
-            return self._window_batch_iteration(conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, base, level)
+            return self._window_batch_iteration(conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, base, level, weight)
         nf = R.shape[0]
         intr = _intr_from_tiled(fx, fy, ox, oy)
-        if self._wants_grad(conv1, conv2, D, B, R, T, W):
+        if self._wants_grad(conv1, conv2, D, B, R, T, W, weight):
             if self.training_path == "reference_split":
                 raise RuntimeError("training_path='reference_split' has no torch-graph twin of the window solve; use training_path='fused'")
             Rn, Tn, Wn, status = _ag.window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base,
-                                                            exact_sym=self.exact_sym_grad, precision=self.precision, return_status=True)
+                                                            exact_sym=self.exact_sym_grad, precision=self.precision, return_status=True,
+                                                            weight=weight)
             self._check_status(status)
             return Rn, Tn, Wn
         frames = lambda t: t.expand(nf, *t.shape[1:]) if t.shape[0] == 1 else t
-        lv = ops.Level(frames(conv1), conv2, frames(intr), frames(p), frames(D), frames(B))
+        wf = None if weight is None else _ag.window_weights(weight, None, nf, conv1.shape[1])
+        lv = ops.Level(frames(conv1), conv2, frames(intr), frames(p), frames(D), frames(B), weight=wf)
         Rn, Tn, Wn, status = ops.lm_window_run([lv], 1, R, T, W, mlp_packed=[self.mlp_packed(str(level))], l2_regularizer_base=base,
                                                precision=self.precision)
         self._check_status(status)
         return Rn, Tn, Wn
 
-    def _window_batch_iteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, base, level):
+    def _window_batch_iteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, base, level, weight=None):
         """WindowIteration on a batch of nw windows (R [nw,nf,3,3]): the fused path when gradients are recorded, else one iteration of
         ops.lm_window_batch_run."""
         nw, nf = R.shape[0], R.shape[1]
@@ -195,22 +200,24 @@ class BundleNet(torch.nn.Module):
         if len(ranks) != 1:
             raise RuntimeError("WindowIteration: conv1, p, D, B must all carry a frame axis ([nw,1|nf,...]) or all come without one ([nw,...])")
         if conv1.dim() == 3:
-            return self._keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, base, level)
-        if self._wants_grad(conv1, conv2, D, B, R, T, W):
+            return self._keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, base, level, weight)
+        if self._wants_grad(conv1, conv2, D, B, R, T, W, weight):
             if self.training_path == "reference_split":
                 raise RuntimeError("training_path='reference_split' has no torch-graph twin of the window solve; use training_path='fused'")
             Rn, Tn, Wn, status = _ag.window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base,
-                                                                  exact_sym=self.exact_sym_grad, precision=self.precision, return_status=True)
+                                                                  exact_sym=self.exact_sym_grad, precision=self.precision, return_status=True,
+                                                                  weight=weight)
             self._check_status(status)
             return Rn, Tn, Wn
         pairs = lambda t: (t.expand(nw, nf, *t.shape[2:]) if t.shape[1] == 1 else t).reshape(nw * nf, *t.shape[2:])
-        lv = ops.Level(pairs(conv1), pairs(conv2), pairs(intr), pairs(p), pairs(D), pairs(B))
+        wf = None if weight is None else _ag.window_weights(weight, nw, nf, conv1.shape[2])
+        lv = ops.Level(pairs(conv1), pairs(conv2), pairs(intr), pairs(p), pairs(D), pairs(B), weight=wf)
         Rn, Tn, Wn, status = ops.lm_window_batch_run([lv], nw, 1, R.reshape(nw * nf, 3, 3), T.reshape(nw * nf, 3, 1), W,
                                                      mlp_packed=[self.mlp_packed(str(level))], l2_regularizer_base=base, precision=self.precision)
         self._check_status(status.reshape(nw, nf))
         return Rn.reshape(nw, nf, 3, 3), Tn.reshape(nw, nf, 3, 1), Wn
 
-    def _keyframe_batch_iteration(self, conv1, conv2, intr, p, D, B, R, T, W, base, level):
+    def _keyframe_batch_iteration(self, conv1, conv2, intr, p, D, B, R, T, W, base, level, weight=None):
         """WindowIteration on nw windows with the keyframe tensors once per window (conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K]):
         the keyframe build (banet_lm_keyframe_*), fused autograd path when gradients are recorded, else one iteration of
         ops.lm_keyframe_run.  fp32 SIMT only: a TF32 precision raises, and so do bfloat16 features and a bfloat16 basis."""
@@ -218,14 +225,16 @@ class BundleNet(torch.nn.Module):
         self._require_keyframe_features(conv1, conv2)
         self._require_keyframe_basis(B)
         nw, nf = R.shape[0], R.shape[1]
-        if self._wants_grad(conv1, conv2, D, B, R, T, W):
+        if self._wants_grad(conv1, conv2, D, B, R, T, W, weight):
             if self.training_path == "reference_split":
                 raise RuntimeError("training_path='reference_split' has no torch-graph twin of the window solve; use training_path='fused'")
             Rn, Tn, Wn, status = _ag.window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base,
-                                                                  exact_sym=self.exact_sym_grad, precision=self.precision, return_status=True)
+                                                                  exact_sym=self.exact_sym_grad, precision=self.precision, return_status=True,
+                                                                  weight=weight)
             self._check_status(status)
             return Rn, Tn, Wn
-        lv = ops.KeyframeLevel(conv1, conv2.reshape(nw * nf, *conv2.shape[2:]), intr.expand(nw, nf, 4).reshape(nw * nf, 4), p, D, B)
+        wf = None if weight is None else _ag.window_weights(weight, nw, nf, conv1.shape[1])
+        lv = ops.KeyframeLevel(conv1, conv2.reshape(nw * nf, *conv2.shape[2:]), intr.expand(nw, nf, 4).reshape(nw * nf, 4), p, D, B, weight=wf)
         Rn, Tn, Wn, status = ops.lm_keyframe_run([lv], 1, R.reshape(nw * nf, 3, 3), T.reshape(nw * nf, 3, 1), W,
                                                  mlp_packed=[self.mlp_packed(str(level))], l2_regularizer_base=base, precision=self.precision)
         self._check_status(status.reshape(nw, nf))
@@ -326,7 +335,8 @@ class BundleNet(torch.nn.Module):
             Ds.append(depth.reshape(nb, oh, ow, 1))
         return Rs, Ts, Ds
 
-    def WindowResize(self, intrisic, key_layers, frame_layers, points, basis, init_depth, init_rotation=None, init_translation=None):
+    def WindowResize(self, intrisic, key_layers, frame_layers, points, basis, init_depth, init_rotation=None, init_translation=None,
+                     weight: Optional[Tensor] = None):
         """BundleResize's schedule (reference bundlenet.py:332-399) for nw keyframe windows of nf frames (an extension): levels 2, 3 x one
         joint window iteration, the keyframe depth init_depth + basis.W shared by the window's frames.
           intrisic [nw,4,1]            one camera per window (keyframe rays and every frame's projection)
@@ -338,15 +348,19 @@ class BundleNet(torch.nn.Module):
         No gradients recorded: one ops.lm_keyframe_run iteration per level on the frames' F2 maps as they are.  Gradients recorded: the keyframe
         form of autograd.window_batch_iteration_fused per level on [F2|gx|gy] (the keyframe backward takes that layout only); gradients reach
         both pyramids, the basis, the initial pose and the lambda-MLP parameters, init_depth through the output depth only (:341, :397).
-        AUTO or FP32_SIMT, float32 pyramids and a float32 basis only, like the keyframe form of WindowIteration."""
+        AUTO or FP32_SIMT, float32 pyramids and a float32 basis only, like the keyframe form of WindowIteration.
+        weight [nw,nf,N,1] or [nw,1,N,1] float32 (an extension): a per-(frame, point) confidence at `points`, the same at both levels (see
+        WindowIteration); differentiable when it requires grad."""
         if self.vmatrix_batch_scramble:
             raise RuntimeError("vmatrix_batch_scramble=True is a 2-view quirk (bundlenet.py:45); the window solve has per-frame VMatrix only")
         self._require_keyframe_precision()
         self._require_keyframe_features(*key_layers, *frame_layers)
         self._require_keyframe_basis(basis)
         nw, nf, K = self._window_resize_shapes(intrisic, key_layers, frame_layers, points, basis, init_depth, init_rotation, init_translation)
+        if weight is not None:
+            _ag.window_weights(weight, nw, nf, points.shape[1])                # shape and dtype errors before any kernel runs
         _points, intr = self._prepare(intrisic, points)
-        grad = self._wants_grad(*key_layers, *frame_layers, basis, init_rotation, init_translation)
+        grad = self._wants_grad(*key_layers, *frame_layers, basis, init_rotation, init_translation, weight)
         resample = _ag.resample if grad else ops.resample
         compose = _ag.depth_compose if grad or self._wants_grad(init_depth) else ops.depth_compose
         d = ops.resample(init_depth.detach(), _points, 0.5)                    # :341-343, once per window
@@ -367,7 +381,7 @@ class BundleNet(torch.nn.Module):
                 conv2 = _ag.grad_fixed_concat(F2.reshape(nw * nf, *F2.shape[2:])).reshape(*F2.shape[:4], 3 * F2.shape[4])
             else:                                                              # the keyframe forward derives gx, gy from F2 itself
                 conv2 = F2
-            R, T, W = self._keyframe_batch_iteration(conv1, conv2, (intr / scale).unsqueeze(1), p, d, b, R, T, W, 1000.0, level)   # :393
+            R, T, W = self._keyframe_batch_iteration(conv1, conv2, (intr / scale).unsqueeze(1), p, d, b, R, T, W, 1000.0, level, weight)   # :393
             status = self.last_status if status is None else status | self.last_status
             Rs.append(R); Ts.append(T)
             depth = compose(init_depth.reshape(nw, -1), basis.reshape(nw, -1, K), W)   # :397

@@ -622,9 +622,10 @@ extern "C" int banet_lm_keyframe_build(const banet_keyframe_level_t* lv, const f
     return keyframe_build(lv, plan, R, T, W, H, g, rbar_sum, nvalid, ws, (cudaStream_t)stream);
 }
 
-extern "C" int banet_lm_keyframe_build_bwd(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W,
-                                           const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
-                                           float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, banet_stream_t stream)
+extern "C" int banet_lm_keyframe_build_bwd_weighted(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W,
+                                                    const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
+                                                    float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
+                                                    float* dweight, banet_stream_t stream)
 {
     int rc = check_keyframe_level(lv, "lm_keyframe_build_bwd");
     if (rc) return rc;
@@ -633,7 +634,14 @@ extern "C" int banet_lm_keyframe_build_bwd(const banet_keyframe_level_t* lv, con
     BANET_REQUIRE(lv->conv2_channels == 3 * lv->C, BANET_ERR_UNSUPPORTED, "lm_keyframe_build_bwd: conv2 must be the [F2|gx|gy] (3C) layout");
     BANET_REQUIRE(keyframe_build_bwd_supported(lv->nf, lv->K, lv->C), BANET_ERR_UNSUPPORTED,
                   "lm_keyframe_build_bwd: K=%d, C=%d do not fit shared memory", lv->K, lv->C);
-    return keyframe_build_bwd(lv, R, T, W, dH, dg, drbar_sum, exact_sym, dconv1, dconv2, dD, dB, dR, dT, dW, (cudaStream_t)stream);
+    return keyframe_build_bwd(lv, R, T, W, dH, dg, drbar_sum, exact_sym, dconv1, dconv2, dD, dB, dR, dT, dW, dweight, (cudaStream_t)stream);
+}
+
+extern "C" int banet_lm_keyframe_build_bwd(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W,
+                                           const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
+                                           float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, banet_stream_t stream)
+{
+    return banet_lm_keyframe_build_bwd_weighted(lv, R, T, W, dH, dg, drbar_sum, exact_sym, dconv1, dconv2, dD, dB, dR, dT, dW, nullptr, stream);
 }
 
 extern "C" size_t banet_lm_keyframe_run_workspace_bytes(const banet_keyframe_level_t* levels, int nlevels, int precision)

@@ -111,7 +111,7 @@ int keyframe_build(const banet_keyframe_level_t* lv, const KeyframePlan& plan, c
 bool keyframe_build_bwd_supported(int nf, int K, int C);
 int keyframe_build_bwd(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W, const float* dH, const float* dg,
                        const float* drbar, int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
-                       cudaStream_t st);
+                       float* dweight, cudaStream_t st);
 
 // legacy pose-only tracker loop with device-side accept / reject and early termination (lm_legacy.cu)
 size_t lm_track_legacy_workspace_bytes(const banet_level_t* levels, int nlevels);

@@ -23,6 +23,10 @@
 // once, without atomics (bit-reproducible).  dconv2, dR, dT (per pair) and dW (per window) are accumulated with atomics as in lm_bwd.cu.
 // The depth blocks of the other frames of dH are ignored: they are constants (zero) in the forward, so this is the exact adjoint.
 //
+// Point weights (banet_keyframe_level_t::weight, one per (frame, point), pair w nf + f): the forward scales a point's M, q in each frame after
+// its channel reduction, so every weighted quantity (H_cc, g_c, v_f, t_f, s_f and with s_f the window's depth block) follows; sum |d| and
+// nvalid stay unweighted.  The backward stores dw = 1/2 <M, Q> + q.z per (frame, point) and scales that point's adjoints by w.
+//
 // The per-point code (geometry, gather, Jacobians, the chain rule through the sampler) is that of lm_build.cu / lm_bwd.cu, restated here
 // for a keyframe given once; the existing kernels are left as they are.
 #include "common.cuh"
@@ -51,6 +55,7 @@ struct KeyParams {
     const float *conv1, *p, *D, *B;          // keyframe, [nw,...]
     const float *conv2, *intr, *R, *T;       // per pair, [nw nf,...]
     const float* W;                          // [nw,K]
+    const float* weight;                     // [nw nf,N] point weights per pair, or NULL (= 1)
     float* partials;
     size_t slot_floats;
     int max_span, tiles_per_win;
@@ -236,7 +241,8 @@ keyframe_build_kernel(const KeyParams prm)
             for (int i = 0; i < KT_PX / KT_WARPS; ++i) {
                 const int n = i * KT_WARPS + warp;
                 float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f;
-                if (rec[R_MASK * KT_PX + n] != 0.f) {
+                const bool valid = rec[R_MASK * KT_PX + n] != 0.f;
+                if (valid) {
                     const int x0 = __float_as_int(rec[R_X0 * KT_PX + n]), y0 = __float_as_int(rec[R_Y0 * KT_PX + n]);
                     const float dx = rec[R_DX * KT_PX + n], dy = rec[R_DY * KT_PX + n];
                     const int x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
@@ -296,8 +302,11 @@ keyframe_build_kernel(const KeyParams prm)
                     m11 = warp_sum(m11); m12 = warp_sum(m12); m22 = warp_sum(m22); q1 = warp_sum(q1); q2 = warp_sum(q2);
                 }
                 if (lane == 0) {
-                    rec[R_M11 * KT_PX + n] = m11; rec[R_M12 * KT_PX + n] = m12; rec[R_M22 * KT_PX + n] = m22;
-                    rec[R_Q1 * KT_PX + n] = q1; rec[R_Q2 * KT_PX + n] = q2;
+                    // point weight of (frame f, point n): scales M and q, and through them every weighted quantity of S3 (H_cc, g_c, v_f,
+                    // t_f, s_f); sum |d|, nvalid and R_ANY stay unweighted.  Unweighted: x * 1.0f is exact
+                    const float wn = (prm.weight && valid) ? __ldg(prm.weight + (size_t)b * N + n0 + n) : 1.f;
+                    rec[R_M11 * KT_PX + n] = m11 * wn; rec[R_M12 * KT_PX + n] = m12 * wn; rec[R_M22 * KT_PX + n] = m22 * wn;
+                    rec[R_Q1 * KT_PX + n] = q1 * wn; rec[R_Q2 * KT_PX + n] = q2 * wn;
                 }
             }
             __syncthreads();
@@ -500,6 +509,8 @@ struct KeyBwdParams {
     const float *conv1, *p, *D, *B, *conv2, *intr, *R, *T, *W;
     const float *dH, *dg, *drbar;
     float *dconv1, *dconv2, *dD, *dB, *dR, *dT, *dW;
+    const float* weight;                         // [nw nf,N] point weights per pair, or NULL (= 1)
+    float* dweight;                              // [nw nf,N] their gradient, or NULL
     int exact_sym, nfc, tiles_per_win;
     long long total_tiles;
 };
@@ -626,7 +637,10 @@ keyframe_build_bwd_kernel(const KeyBwdParams prm)
                         const float x = X / Z, y = Y / Z, iZ = 1.0f / Z;
                         const float u = fx * x + ox, v = fy * y + oy;
                         const bool ok = (u >= 0.f) && (u <= (float)(w - 1)) && (v >= 0.f) && (v <= (float)(h - 1)) && isfinite(iZ);
-                        if (!ok) continue;                                   // masked in this frame: no gradient through it
+                        if (!ok) {                                           // masked in this frame: no gradient through it
+                            if (prm.dweight && lane == 0) prm.dweight[b * N + n] = 0.f;
+                            continue;
+                        }
                         const float fu = floorf(u), fv = floorf(v);
                         const int x0 = (int)fu, y0 = (int)fv, x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
                         const float dx = u - fu, dy = v - fv;
@@ -677,6 +691,14 @@ keyframe_build_bwd_kernel(const KeyBwdParams prm)
                         float Q00 = yb0 * jd0, Q01 = yb0 * jd1, Q10 = yb1 * jd0, Q11 = yb1 * jd1;
 #pragma unroll
                         for (int i = 0; i < 6; ++i) { Q00 = fmaf(Yc0[i], a0[i], Q00); Q01 = fmaf(Yc0[i], a1[i], Q01); Q10 = fmaf(Yc1[i], a0[i], Q10); Q11 = fmaf(Yc1[i], a1[i], Q11); }
+                        // ---- point weight of (frame f, point n), as in lm_build_bwd_kernel: dw = 1/2 <M, Q> + q.z, one writer, no atomics.
+                        //      Q holds gamma = b^T S_dd b from frame 0's depth block, so dw is the adjoint of the window-reduced forward (this
+                        //      point's depth contribution lands in frame 0's block).  Then M, q, Q, z carry w to dJ, dj, db, dd, dG; the
+                        //      rhat sign(d) path is not weighted.  Unweighted: w = 1 and x * 1.0f is exact.
+                        const float wn = prm.weight ? __ldg(prm.weight + b * N + n) : 1.f;
+                        if (prm.dweight && lane == 0) prm.dweight[b * N + n] = 0.5f * (m11 * Q00 + m12 * (Q01 + Q10) + m22 * Q11) + (q1 * z0 + q2 * z1);
+                        m11 *= wn; m12 *= wn; m22 *= wn; q1 *= wn; q2 *= wn;
+                        Q00 *= wn; Q01 *= wn; Q10 *= wn; Q11 *= wn; z0 *= wn; z1 *= wn;
                         float dJ0[6], dJ1[6];
 #pragma unroll
                         for (int i = 0; i < 6; ++i) { dJ0[i] = m11 * Yc0[i] + m12 * Yc1[i] + q1 * sg[i]; dJ1[i] = m12 * Yc0[i] + m22 * Yc1[i] + q2 * sg[i]; }
@@ -791,7 +813,7 @@ static KeyParams key_params(const banet_keyframe_level_t* lv, const KeyframePlan
     KeyParams prm;
     prm.nw = lv->nw; prm.nf = lv->nf; prm.N = lv->N; prm.C = lv->C; prm.K = lv->K; prm.h = lv->h; prm.w = lv->w; prm.c2 = lv->conv2_channels;
     prm.conv1 = lv->conv1; prm.p = lv->p; prm.D = lv->D; prm.B = lv->B; prm.conv2 = lv->conv2; prm.intr = lv->intr;
-    prm.R = R; prm.T = T; prm.W = W;
+    prm.R = R; prm.T = T; prm.W = W; prm.weight = lv->weight;
     prm.partials = reinterpret_cast<float*>(ws);
     prm.slot_floats = plan.slot_floats; prm.max_span = plan.max_span; prm.tiles_per_win = plan.tiles_per_win; prm.total_tiles = plan.total_tiles;
     prm.kq_i = 0; prm.kq_j = 0;
@@ -841,7 +863,8 @@ static int key_bwd_nfc(int nf, int K, int C)
 bool keyframe_build_bwd_supported(int nf, int K, int C) { return K >= 1 && K <= 256 && key_bwd_nfc(nf, K, C) > 0; }
 
 int keyframe_build_bwd(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W, const float* dH, const float* dg,
-                       const float* drbar, int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, cudaStream_t st)
+                       const float* drbar, int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
+                       float* dweight, cudaStream_t st)
 {
     const int K = lv->K, C = lv->C, nf = lv->nf;
     const int nfc = key_bwd_nfc(nf, K, C);
@@ -855,6 +878,7 @@ int keyframe_build_bwd(const banet_keyframe_level_t* lv, const float* R, const f
     prm.conv1 = lv->conv1; prm.p = lv->p; prm.D = lv->D; prm.B = lv->B; prm.conv2 = lv->conv2; prm.intr = lv->intr; prm.R = R; prm.T = T; prm.W = W;
     prm.dH = dH; prm.dg = dg; prm.drbar = drbar;
     prm.dconv1 = dconv1; prm.dconv2 = dconv2; prm.dD = dD; prm.dB = dB; prm.dR = dR; prm.dT = dT; prm.dW = dW;
+    prm.weight = lv->weight; prm.dweight = dweight;
     prm.exact_sym = exact_sym; prm.nfc = nfc;
     prm.tiles_per_win = (lv->N + KB_TILE - 1) / KB_TILE;
     prm.total_tiles = (long long)lv->nw * prm.tiles_per_win;

@@ -412,6 +412,7 @@ class KeyframeLevel:
     p: Tensor                 # [nw,3,N]
     D: Tensor                 # [nw,N,1]
     B: Tensor                 # [nw,N,K]
+    weight: Optional[Tensor] = None          # [nw*nf,N,1] float32 per-(frame, point) weight of the normal equations; None = unweighted
 
     def as_struct(self) -> Tuple[_lib.BanetKeyframeLevel, list]:
         if self.conv1.dtype != torch.float32 or self.conv2.dtype != torch.float32:
@@ -424,9 +425,10 @@ class KeyframeLevel:
         B = _chk(self.B, "B"); K = B.shape[2]
         _chk(B, "B", (nw, N, K))
         intr = _chk(self.intr, "intr", (nb, 4)); p = _chk(self.p, "p", (nw, 3, N)); D = _chk(self.D, "D", (nw, N, 1))
-        keep = [conv1, conv2, intr, p, D, B]
+        wt = None if self.weight is None else _chk(self.weight, "weight", (nb, N, 1))
+        keep = [conv1, conv2, intr, p, D, B, wt]
         return _lib.BanetKeyframeLevel(nw, nf, N, Cc, K, h, w, c2, conv1.data_ptr(), p.data_ptr(), D.data_ptr(), B.data_ptr(),
-                                       conv2.data_ptr(), intr.data_ptr()), keep
+                                       conv2.data_ptr(), intr.data_ptr(), _ptr(wt)), keep
 
 
 def lm_keyframe_build(level: KeyframeLevel, R: Tensor, T: Tensor, W: Tensor):
@@ -449,9 +451,11 @@ def lm_keyframe_build(level: KeyframeLevel, R: Tensor, T: Tensor, W: Tensor):
 
 
 def lm_keyframe_build_bwd(level: KeyframeLevel, R: Tensor, T: Tensor, W: Tensor, dH: Tensor, dg: Tensor, drbar_sum: Tensor,
-                          exact_sym: bool = False):
+                          exact_sym: bool = False, return_dweight: bool = False):
     """Backward of lm_keyframe_build (banet_lm_keyframe_build_bwd) -> dconv1 [nw,N,C], dconv2 [nw*nf,h,w,3C], dD [nw,N,1], dB [nw,N,K],
-    dR, dT [nw*nf,...], dW [nw,K,1].  Only frame 0's depth block of dH is read."""
+    dR, dT [nw*nf,...], dW [nw,K,1].  Only frame 0's depth block of dH is read.  On a weighted level every gradient carries the point
+    weights.  return_dweight=True appends dweight [nw*nf,N,1] (banet_lm_keyframe_build_bwd_weighted; on an unweighted level, the gradient
+    at weights of ones)."""
     lib = load()
     st, keep = level.as_struct()
     nw, nb, K, Cc, N = st.nw, st.nw * st.nf, st.K, st.C, st.N
@@ -462,10 +466,17 @@ def lm_keyframe_build_bwd(level: KeyframeLevel, R: Tensor, T: Tensor, W: Tensor,
     dconv1 = torch.empty(nw, N, Cc, device=dev); dconv2 = torch.empty(nb, st.h, st.w, 3 * Cc, device=dev)
     dD = torch.empty(nw, N, 1, device=dev); dB = torch.empty(nw, N, K, device=dev)
     dR = torch.empty(nb, 3, 3, device=dev); dT = torch.empty(nb, 3, 1, device=dev); dW = torch.empty(nw, K, 1, device=dev)
-    check(lib.banet_lm_keyframe_build_bwd(C.byref(st), R.data_ptr(), T.data_ptr(), Wt.data_ptr(), dH.data_ptr(), dg.data_ptr(), dr.data_ptr(),
-                                          int(bool(exact_sym)), dconv1.data_ptr(), dconv2.data_ptr(), dD.data_ptr(), dB.data_ptr(), dR.data_ptr(),
-                                          dT.data_ptr(), dW.data_ptr(), _stream()), "banet_lm_keyframe_build_bwd")
-    return dconv1, dconv2, dD, dB, dR, dT, dW
+    if not return_dweight:
+        check(lib.banet_lm_keyframe_build_bwd(C.byref(st), R.data_ptr(), T.data_ptr(), Wt.data_ptr(), dH.data_ptr(), dg.data_ptr(), dr.data_ptr(),
+                                              int(bool(exact_sym)), dconv1.data_ptr(), dconv2.data_ptr(), dD.data_ptr(), dB.data_ptr(), dR.data_ptr(),
+                                              dT.data_ptr(), dW.data_ptr(), _stream()), "banet_lm_keyframe_build_bwd")
+        return dconv1, dconv2, dD, dB, dR, dT, dW
+    dweight = torch.empty(nb, N, 1, device=dev)
+    check(lib.banet_lm_keyframe_build_bwd_weighted(C.byref(st), R.data_ptr(), T.data_ptr(), Wt.data_ptr(), dH.data_ptr(), dg.data_ptr(),
+                                                   dr.data_ptr(), int(bool(exact_sym)), dconv1.data_ptr(), dconv2.data_ptr(), dD.data_ptr(),
+                                                   dB.data_ptr(), dR.data_ptr(), dT.data_ptr(), dW.data_ptr(), dweight.data_ptr(), _stream()),
+          "banet_lm_keyframe_build_bwd_weighted")
+    return dconv1, dconv2, dD, dB, dR, dT, dW, dweight
 
 
 def lm_keyframe_run(levels: Sequence[KeyframeLevel], iters_per_level: int, R: Tensor, T: Tensor, W: Tensor,

@@ -365,6 +365,13 @@ typedef struct banet_keyframe_level {
     const float* B;           /* [nw,N,K]      its depth basis */
     const float* conv2;       /* [nw*nf,h,w,conv2_channels]  per pair */
     const float* intr;        /* [nw*nf,4]     per pair */
+    const float* weight;      /* [nw*nf,N,1] or NULL: per-point confidence of banet_level_t::weight, one per (frame, keyframe point), pair
+                                 w*nf + f (the per-pair convention of (3d)): frame f's point n adds w * (its H_cc, H_cd, g_c, g_d) to pair
+                                 w*nf + f and w * its H_dd to the window's depth block; rbar_sum and nvalid stay unweighted, so lambda does
+                                 not see it.  NULL is the unweighted arithmetic bit for bit, and so are weights of ones.  It is the last
+                                 field, so a zero-initialised struct stays unweighted; it changed sizeof(banet_keyframe_level_t) and
+                                 therefore the stride of levels[] for banet_lm_keyframe_run: code compiled against a header without it
+                                 cannot pass level arrays to this library */
 } banet_keyframe_level_t;
 
 /* The keyframe build: R [nw*nf,3,3], T [nw*nf,3,1], W [nw,K,1] (read directly, one row per window) -> the window-reduced H, g, rbar_sum,
@@ -384,6 +391,15 @@ int    banet_lm_keyframe_build_bwd(const banet_keyframe_level_t* lv, const float
                                    const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
                                    float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
                                    banet_stream_t stream);
+/* The same, plus the gradient of the level's point weights: dweight [nw*nf,N,1] (may be NULL; overwritten otherwise, one writer per
+ * element, no atomics),  dw = <dH_f, H_{f,n}> + <dg_f, g_{f,n}>  with frame 0's depth block of dH in place of frame f's (the forward adds
+ * frame f's depth contribution to frame 0's block); masked points get 0.  On a weighted level every other gradient that comes from dH, dg
+ * is the point's times its weight (the drbar_sum path is not weighted); banet_lm_keyframe_build_bwd is this call with dweight = NULL.
+ * Argument errors are those of banet_lm_keyframe_build_bwd, reported before any CUDA call. */
+int    banet_lm_keyframe_build_bwd_weighted(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W,
+                                            const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
+                                            float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
+                                            float* dweight, banet_stream_t stream);
 /* Whole coarse-to-fine solve (banet_lm_window_batch_run with keyframe levels): each iteration is one keyframe-build launch (plus its fp64
  * slot reduction) and one window-step launch, the lambda-MLP or lambda_fixed as in (3d).  W [nw,K,1] is read by the build directly (no
  * per-pair copies).  levels[l].nw, nf, K must agree across levels.  precision: BANET_PREC_AUTO or BANET_PREC_FP32_SIMT (AUTO resolves to
