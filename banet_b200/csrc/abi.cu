@@ -61,7 +61,11 @@ int resolve_precision(const banet_level_t* lv, int precision)
     if (precision == BANET_PREC_FP32_SIMT) return precision;
     if (precision == BANET_PREC_TF32X1 || precision == BANET_PREC_TF32X2 || precision == BANET_PREC_TF32X3) {
         if (!tc_supported(lv)) {
-            set_error("precision mode %d (tensor cores) needs K=128, C in {64,128} and 16-B aligned tensors; got K=%d C=%d", precision, lv->K, lv->C);
+            if (lv->conv2_channels == lv->C && lv->w >= 65536)        // tc_supported(): the F2-only gather packs tap columns in 16 bits
+                set_error("precision mode %d (tensor cores) needs w < 65536 in the F2-only layout (tap columns are packed in 16 bits); got w=%d",
+                          precision, lv->w);
+            else
+                set_error("precision mode %d (tensor cores) needs K=128, C in {64,128} and 16-B aligned tensors; got K=%d C=%d", precision, lv->K, lv->C);
             return BANET_ERR_UNSUPPORTED;
         }
         return precision;

@@ -47,12 +47,19 @@ const banet_tuning_t& tuning() { return g_tuning; }
 // (tc_generation = 0) is generation 6 everywhere: in interleaved A/B runs on an H100 80GB HBM3 (400 W power limit, 32 pairs, F2-only
 // layout) generation 7 took 25.5 vs 21.5 ms at 640x480 and 5.8 vs 5.4 ms at 320x240 in TF32X1, and 2.3x as long in TF32X2 (its
 // gather warps run on 64 registers and spill, see DESIGN.md §4).  banet_set_tuning(tc_generation = 7) forces it where it applies.
+// It also needs a map at least as large as its staged F2 window: on a 2 x 2 map it returned non-finite H (tests/test_build_edges.py).
 static bool use_gen7(const banet_level_t* lv, int mode, int kblk)
 {
     const bool wanted = g_tuning.tc_generation == 7;
+    int wx = 0, wy = 0;
+    lm_build_tc7_window(&wx, &wy);
     return wanted && !lv->weight && lv->feature_dtype == BANET_DTYPE_F32 && lv->basis_dtype == BANET_DTYPE_F32 && lv->conv2_channels == lv->C && lv->grid_w > 0 && lv->h < 65536 && lv->w < 65536 &&
-           lm_build_tc7_supported(mode, lv->C / 64, kblk);
+           lv->h >= wy && lv->w >= wx && lm_build_tc7_supported(mode, lv->C / 64, kblk);
 }
+
+// The F2-only gather packs the four tap columns of a pixel into 16 bits each (lm_build_tc6.cu, the geometry warps' cx[]), so that
+// layout needs w < 65536; a wider map resolves to the SIMT kernel under AUTO and is BANET_ERR_UNSUPPORTED in an explicit TF32 mode.
+static bool tc_f2_width_ok(const banet_level_t* lv) { return lv->conv2_channels != lv->C || lv->w < 65536; }
 
 bool tc_supported(const banet_level_t* lv)
 {
@@ -60,7 +67,7 @@ bool tc_supported(const banet_level_t* lv)
     return k_ok && (lv->C == 64 || lv->C == 128) && (lv->conv2_channels == lv->C || lv->conv2_channels == 3 * lv->C) &&
            ((reinterpret_cast<uintptr_t>(lv->conv1) | reinterpret_cast<uintptr_t>(lv->conv2) | reinterpret_cast<uintptr_t>(lv->B)) % 16 == 0) &&
            (long long)lv->nb * lv->N < (1LL << 31) && (long long)lv->nb * ((lv->N + 63) / 64 + 80) < (1LL << 31) &&
-           (long long)lv->h * lv->w * lv->conv2_channels < (1LL << 31);
+           (long long)lv->h * lv->w * lv->conv2_channels < (1LL << 31) && tc_f2_width_ok(lv);
 }
 
 int build_plan_tc(const banet_level_t* lv, int num_sms, BuildPlan* plan)
