@@ -56,6 +56,7 @@ int build_dispatch(const banet_level_t* lv, int resolved, const BuildPlan& plan,
 
 // lambda MLP / solve / update (lm_solve.cu)
 int lm_lambda(const float* rbar_sum, int nb, int N, int C, const float* mlp, float base, float* lambda_out, cudaStream_t st);
+bool lm_solve_uses_double(int P);
 int lm_solve_update(const float* H, const float* g, const float* lambda, int nb, int K, const banet_solve_opts_t& opts,
                     const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
                     float* delta, int32_t* status, int status_accumulate, cudaStream_t st);
@@ -64,6 +65,7 @@ int lm_solve_update(const float* H, const float* g, const float* lambda, int nb,
 struct StepMode { float lambda_exp0; int rbar_per_valid, use_vmatrix, clamp_theta; };
 constexpr StepMode kStepBundleNet = {2.0f, 0, 1, 1};          // bundlenet.py:241-276
 bool lm_step_supported(int P, int C);
+bool lm_step_uses_double(int P, int C);
 int lm_step(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K, const float* mlp, float base, const float* lambda_in,
             const StepMode& mode, const float* nvalid, const banet_solve_opts_t& opts, const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
             float* delta, float* lambda_out, int32_t* status, int status_accumulate, cudaStream_t st);
@@ -125,11 +127,12 @@ int lm_solve_update_bwd(const float* H, const float* g, const float* lambda, con
                         const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
                         float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, cudaStream_t st);
 // its two stages: the SE(3) update backward (ddelta[0:6] of pair b -> ddelta + b * P), and u = Ht^-1 [ddelta[0:npose] | dW'] with dH, dg = u,
-// dlambda, dW = dW' (pairs of P unknowns, the first npose of them poses)
+// dlambda, dW = dW' (pairs of P unknowns, the first npose of them poses).  g [nb,P] is the forward's right-hand side (a non-finite entry
+// skipped the step); use_double: the precision the forward factored in (lm_solve_uses_double / lm_step_uses_double)
 int launch_pose_update_bwd(const float* delta, int nb, int P, const float* R, const float* T, const float* gRn, const float* gTn,
                            float* ddelta, float* dR, float* dT, cudaStream_t st);
 bool solve_bwd_supported(int P);
-int launch_solve_bwd(const float* H, const float* lambda, const float* delta, int nb, int P, int npose, const banet_solve_opts_t& opts,
-                     const float* gWn, float* dH, float* dg, float* dlambda, float* dW, cudaStream_t st);
+int launch_solve_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int P, int npose, bool use_double,
+                     const banet_solve_opts_t& opts, const float* gWn, float* dH, float* dg, float* dlambda, float* dW, cudaStream_t st);
 
 }  // namespace banet

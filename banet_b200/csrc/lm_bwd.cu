@@ -421,8 +421,9 @@ __host__ __device__ __forceinline__ int tri2(int i, int k) { return i * (i + 1) 
 // pairs of the 2-view iteration, 6 nf for the one system of a keyframe window; the remaining P - npose entries of ddelta are dW'.
 template <typename S>
 __global__ void __launch_bounds__(SB_THREADS)
-lm_solve_bwd_kernel(const float* __restrict__ H, const float* __restrict__ lambda, const float* __restrict__ delta, int P, int npose, float eps, int ndamped,
-                    const float* __restrict__ gWn, float* __restrict__ dH, float* __restrict__ dg, float* __restrict__ dlambda, float* __restrict__ dW)
+lm_solve_bwd_kernel(const float* __restrict__ H, const float* __restrict__ g, const float* __restrict__ lambda, const float* __restrict__ delta, int P,
+                    int npose, float eps, int ndamped, const float* __restrict__ gWn, float* __restrict__ dH, float* __restrict__ dg,
+                    float* __restrict__ dlambda, float* __restrict__ dW)
 {
     extern __shared__ __align__(16) unsigned char smraw[];
     S* A = reinterpret_cast<S*>(smraw);                 // packed lower triangle of the damped matrix -> its Cholesky factor
@@ -446,6 +447,7 @@ lm_solve_bwd_kernel(const float* __restrict__ H, const float* __restrict__ lambd
             A[tri2(i, k)] = sv;
         }
     for (int i = tid; i < P; i += SB_THREADS) {
+        if (!isfinite(g[(size_t)b * P + i])) bad = 1;          // the forward skipped the step on a non-finite right-hand side too
         r[i] = (S)delta[(size_t)b * P + i];
         if (i < npose) uu[i] = (S)dg[(size_t)b * P + i];
         else { const float v = gWn[(size_t)b * K + i - npose]; uu[i] = (S)v; dW[(size_t)b * K + i - npose] = v; }       // W' = W + delta_d
@@ -520,27 +522,26 @@ int launch_pose_update_bwd(const float* delta, int nb, int P, const float* R, co
     return BANET_OK;
 }
 
-// packed lower triangle + 3 vectors in shared memory: double up to 200 KB (P <= 220), float beyond
+// packed lower triangle + 3 vectors in shared memory, in the precision of the forward's factorisation: the backward re-derives the forward's
+// skip decision from its own factorisation, so the two must factor alike.  Double needs 205 160 B at the largest pair system (P = 223).
 static size_t solve_bwd_floats(int P) { return (size_t)P * (P + 1) / 2 + 3 * (size_t)P; }
-static bool solve_bwd_double(int P) { return solve_bwd_floats(P) * sizeof(double) <= 200 * 1024; }
-bool solve_bwd_supported(int P) { return solve_bwd_double(P) || solve_bwd_floats(P) * sizeof(float) <= 220 * 1024; }
+bool solve_bwd_supported(int P) { return solve_bwd_floats(P) * sizeof(float) <= 220 * 1024; }
 
-int launch_solve_bwd(const float* H, const float* lambda, const float* delta, int nb, int P, int npose, const banet_solve_opts_t& opts,
-                     const float* gWn, float* dH, float* dg, float* dlambda, float* dW, cudaStream_t st)
+int launch_solve_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int P, int npose, bool use_double,
+                     const banet_solve_opts_t& opts, const float* gWn, float* dH, float* dg, float* dlambda, float* dW, cudaStream_t st)
 {
     const int ndamped = opts.undamped_last ? P - 1 : P;
-    const bool use_double = solve_bwd_double(P);
     const size_t smem = solve_bwd_floats(P) * (use_double ? sizeof(double) : sizeof(float));
-    BANET_REQUIRE(solve_bwd_supported(P), BANET_ERR_UNSUPPORTED, "lm_solve_bwd: P=%d does not fit shared memory", P);
+    BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_solve_bwd: P=%d does not fit shared memory", P);
     cudaError_t e;
     if (use_double) {
         e = cudaFuncSetAttribute(lm_solve_bwd_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) { set_error("lm_solve_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
-        lm_solve_bwd_kernel<double><<<nb, SB_THREADS, smem, st>>>(H, lambda, delta, P, npose, opts.damping_eps, ndamped, gWn, dH, dg, dlambda, dW);
+        lm_solve_bwd_kernel<double><<<nb, SB_THREADS, smem, st>>>(H, g, lambda, delta, P, npose, opts.damping_eps, ndamped, gWn, dH, dg, dlambda, dW);
     } else {
         e = cudaFuncSetAttribute(lm_solve_bwd_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) { set_error("lm_solve_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
-        lm_solve_bwd_kernel<float><<<nb, SB_THREADS, smem, st>>>(H, lambda, delta, P, npose, opts.damping_eps, ndamped, gWn, dH, dg, dlambda, dW);
+        lm_solve_bwd_kernel<float><<<nb, SB_THREADS, smem, st>>>(H, g, lambda, delta, P, npose, opts.damping_eps, ndamped, gWn, dH, dg, dlambda, dW);
     }
     BANET_CUDA_LAUNCH_CHECK("lm_solve_bwd_kernel launch");
     return BANET_OK;
@@ -550,14 +551,13 @@ int lm_solve_update_bwd(const float* H, const float* g, const float* lambda, con
                         const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
                         float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, cudaStream_t st)
 {
-    (void)g;
     BANET_REQUIRE(!opts.vmatrix_batch_scramble, BANET_ERR_UNSUPPORTED,
                   "lm_solve_update_bwd: the batch-interleaved VMatrix of bundlenet.py:45 is not differentiated (use vmatrix_batch_scramble=0)");
     const int P = 6 + K;
     BANET_REQUIRE(solve_bwd_supported(P), BANET_ERR_UNSUPPORTED, "lm_solve_update_bwd: P=%d does not fit shared memory", P);
     int rc = launch_pose_update_bwd(delta, nb, P, R, T, gRn, gTn, dg, dR, dT, st);       // ddelta[0:6] parked in dg
     if (rc) return rc;
-    return launch_solve_bwd(H, lambda, delta, nb, P, 6, opts, gWn, dH, dg, dlambda, dW, st);
+    return launch_solve_bwd(H, g, lambda, delta, nb, P, 6, lm_solve_uses_double(P), opts, gWn, dH, dg, dlambda, dW, st);
 }
 
 }  // namespace banet

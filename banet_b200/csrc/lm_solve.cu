@@ -238,6 +238,9 @@ int launch_pose_update(const float* delta, int nb, int P, const float* R, const 
     return BANET_OK;
 }
 
+// lm_solve_kernel<double> while its packed triangle fits 200 KB (P <= 223); its backward (lm_bwd.cu) factors in the same precision
+bool lm_solve_uses_double(int P) { return ((size_t)P * (P + 1) / 2 + 2 * (size_t)P) * sizeof(double) <= 200 * 1024; }
+
 int lm_solve_update(const float* H, const float* g, const float* lambda, int nb, int K, const banet_solve_opts_t& opts,
                     const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
                     float* delta, int32_t* status, int status_accumulate, cudaStream_t st)
@@ -245,7 +248,7 @@ int lm_solve_update(const float* H, const float* g, const float* lambda, int nb,
     const int P = 6 + K;
     const int ndamped = opts.undamped_last ? P - 1 : P;
     const size_t ntri = (size_t)P * (P + 1) / 2 + 2 * (size_t)P;
-    const bool use_double = ntri * sizeof(double) <= 200 * 1024;
+    const bool use_double = lm_solve_uses_double(P);
     const size_t smem = ntri * (use_double ? sizeof(double) : sizeof(float));
     BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_solve: P=%d does not fit shared memory", P);
     cudaError_t e;

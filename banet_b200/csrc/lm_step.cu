@@ -102,6 +102,10 @@ size_t lm_step_smem(int P, int C, bool use_double, bool full)
 
 bool lm_step_supported(int P, int C) { return lm_step_smem(P, C, false, false) <= 220 * 1024; }
 
+// storage: square double (P <= ~150), packed double (P <= ~200), packed float beyond; the dense window's backward (lm_window.cu) factors in
+// the precision this picks for its forward
+bool lm_step_uses_double(int P, int C) { return lm_step_smem(P, C, true, false) <= 200 * 1024; }
+
 // lambda_in != nullptr: used as is; else lambda = base * ||rbar||^(exp0 + MLP(rbar)) (MLP term 0 when mlp == nullptr).
 // In-place R/T/W (R_out == R ...) is fine: a pair's CTA reads before it writes.
 int lm_step(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K, const float* mlp, float base, const float* lambda_in,
@@ -110,9 +114,8 @@ int lm_step(const float* H, const float* g, const float* rbar_sum, int nb, int N
 {
     const int P = 6 + K;
     const int ndamped = opts.undamped_last ? P - 1 : P;
-    // storage: square double (P <= ~150), packed double (P <= ~200), packed float beyond
     const bool full = lm_step_smem(P, C, true, true) <= 200 * 1024;
-    const bool use_double = full || lm_step_smem(P, C, true, false) <= 200 * 1024;
+    const bool use_double = lm_step_uses_double(P, C);
     const size_t smem = lm_step_smem(P, C, use_double, full);
     BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_step: P=%d, C=%d do not fit shared memory", P, C);
     auto launch = [&](auto kern) -> int {

@@ -148,24 +148,25 @@ int lm_window_step(const float* H, const float* g, const float* rbar_sum, int nf
 size_t lm_window_step_bwd_workspace_floats(int nf, int K)
 {
     const size_t Pj = 6 * (size_t)nf + K;
-    return 2 * Pj * Pj + Pj;
+    return 2 * Pj * Pj + 2 * Pj;
 }
 
 // Backward of one window step (lambda given): with ddelta = [pose part from the per-frame SE(3) update backward | dW'], u = Ht_j^-1 ddelta
 // on the re-assembled damped system gives dHj = -u delta_j^T (+ the damping terms), dgj = u and dlambda (lm_solve_bwd_kernel, npose = 6 nf);
-// the assembly's adjoint maps (dHj, dgj) to the pairs.  dW = dW' (W' = W + delta_d).
+// the assembly's adjoint maps (dHj, dgj) to the pairs.  dW = dW' (W' = W + delta_d).  The solve backward factors in the precision lm_step
+// chose for the forward (lambda given), and the assembled gj goes with it: a window whose forward was skipped gets zero dH, dg, dlambda.
 int lm_window_step_bwd(const float* H, const float* g, const float* lambda, const float* delta_j, int nf, int K, const banet_solve_opts_t& opts,
                        const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
                        float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, float* ws, cudaStream_t st)
 {
     const int Pj = 6 * nf + K;
     BANET_REQUIRE(lm_window_supported(nf, K, 1), BANET_ERR_UNSUPPORTED, "lm_window_step_bwd: 6*%d+%d unknowns do not fit the solve kernel", nf, K);
-    float* Hj = ws; float* dHj = Hj + (size_t)Pj * Pj; float* dgj = dHj + (size_t)Pj * Pj;
-    window_assemble_kernel<<<64, 256, 0, st>>>(H, g, nullptr, nf, K, 0, Hj, dgj, nullptr, nullptr);      // gj lands in dgj, overwritten below
+    float* Hj = ws; float* dHj = Hj + (size_t)Pj * Pj; float* dgj = dHj + (size_t)Pj * Pj; float* gj = dgj + Pj;
+    window_assemble_kernel<<<64, 256, 0, st>>>(H, g, nullptr, nf, K, 0, Hj, gj, nullptr, nullptr);
     BANET_CUDA_LAUNCH_CHECK("window_assemble_kernel launch");
     int rc = launch_pose_update_bwd(delta_j, nf, 6, R, T, gRn, gTn, dgj, dR, dT, st);                   // ddelta[0:6 nf] -> dgj
     if (rc) return rc;
-    rc = launch_solve_bwd(Hj, lambda, delta_j, 1, Pj, 6 * nf, opts, gWn, dHj, dgj, dlambda, dW, st);
+    rc = launch_solve_bwd(Hj, gj, lambda, delta_j, 1, Pj, 6 * nf, lm_step_uses_double(Pj, 1), opts, gWn, dHj, dgj, dlambda, dW, st);
     if (rc) return rc;
     window_assemble_bwd_kernel<<<64, 256, 0, st>>>(dHj, dgj, nf, K, dH, dg);
     BANET_CUDA_LAUNCH_CHECK("window_assemble_bwd_kernel launch");

@@ -4,17 +4,21 @@ assembled window system (oracle.window_assemble), values and gradients, and the 
 import torch
 
 
-def window_arrow_solve(H, g, lam, damping_eps: float = 1e-5, undamped_last: bool = True):
+def window_arrow_solve(H, g, lam, damping_eps: float = 1e-5, undamped_last: bool = True, fp32_damping_diag: bool = False):
     """H [nf,P,P], g [nf,P,1] (one window's per-pair normal equations, P = 6 + K), lam scalar -> the window's step [6 nf + K, 1] (frame f's
     pose at 6f, the depth at 6 nf).  Damping as bundlenet.py:264-266 on the joint system: lam (diag + eps) on every pose diagonal and on the
-    frame-summed depth diagonal, except the last depth coefficient when undamped_last."""
+    frame-summed depth diagonal, except the last depth coefficient when undamped_last.  fp32_damping_diag: the summed depth diagonal is
+    rounded to float before it scales the damping, as the kernels do (the assembled joint matrix holds it in float)."""
     nf, P, _ = H.shape
     K = P - 6
     Hcc, Hcd, Hdd = H[:, :6, :6], H[:, :6, 6:], H[:, 6:, 6:]
     gc, gd = g[:, :6], g[:, 6:]
     Acc = Hcc + torch.diag_embed((torch.diagonal(Hcc, dim1=-2, dim2=-1) + damping_eps) * lam)        # damped 6x6 per frame
     Dsum = Hdd.sum(0)
-    ddamp = (torch.diagonal(Dsum) + damping_eps) * lam
+    ddiag = torch.diagonal(Dsum)
+    if fp32_damping_diag:
+        ddiag = ddiag + (ddiag.detach().float().to(H.dtype) - ddiag.detach())                       # rounded value, unit derivative
+    ddamp = (ddiag + damping_eps) * lam
     if undamped_last:
         ddamp = torch.cat([ddamp[:-1], torch.zeros(1, dtype=H.dtype)])
     L = torch.linalg.cholesky(Acc)                                                                   # Acc_f = L_f L_f^T
