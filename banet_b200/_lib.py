@@ -125,6 +125,9 @@ SIGNATURES = {
     "banet_lm_build_bwd": (C.c_int, [C.POINTER(BanetLevel)] + [c_float_p] * 6 + [C.c_int] + [c_float_p] * 7 + [c_stream]),
     "banet_lm_build_bwd_weighted": (C.c_int, [C.POINTER(BanetLevel)] + [c_float_p] * 6 + [C.c_int] + [c_float_p] * 8 + [c_stream]),
     "banet_lm_solve_update_bwd": (C.c_int, [c_float_p] * 4 + [C.c_int, C.c_int, C.POINTER(BanetSolveOpts)] + [c_float_p] * 5 + [c_float_p] * 6 + [c_stream]),
+    "banet_lm_step_bwd_workspace_bytes": (C.c_size_t, [C.c_int] * 3),
+    "banet_lm_step_bwd": (C.c_int, [c_float_p] * 3 + [C.c_int] * 4 + [c_float_p, C.c_float, c_float_p, c_float_p, C.POINTER(BanetSolveOpts)]
+                          + [c_float_p] * 5 + [c_float_p] * 8 + [C.c_void_p, C.c_size_t, c_stream]),
     "banet_grad_fixed_concat_bwd": (C.c_int, [c_float_p] + [C.c_int] * 5 + [c_float_p, c_stream]),
     "banet_resample_bwd": (C.c_int, [c_float_p, c_float_p, C.c_float] + [C.c_int] * 5 + [c_float_p, c_stream]),
     "banet_depth_compose_bwd": (C.c_int, [c_float_p] * 3 + [C.c_int] * 3 + [c_float_p, c_float_p, c_stream]),

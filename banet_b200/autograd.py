@@ -8,6 +8,8 @@ Two training paths:
     conv1, conv2, D, B, R, T, W and the lambda-MLP parameters (TF autodiff + the registered op gradient, bundlenet.py:79-82).
     `window_iteration_fused` is the same for the joint keyframe window (banet_lm_window_solve_update / _bwd after the per-pair build),
     `window_batch_iteration_fused` for a batch of windows (banet_lm_window_batch_solve_update / _bwd).
+    `lm_run` is a whole differentiable coarse-to-fine solve as ops.lm_run runs it (the same kernels and bits): per iteration the build and
+    the fused step banet_lm_step (lambda-MLP included), backward banet_lm_step_bwd -> banet_lm_build_bwd.
   * `iteration` (the reference's own split of labour, kept as the A/B baseline and for op-level drop-in use):
 
     reference:  TF graph ops (warp, resampler, Jacobians, damping, solve, update; TF autodiff)  +  native op
@@ -232,6 +234,88 @@ class _LMSolveUpdateFn(torch.autograd.Function):
         dH, dg, dlam, dR, dT, dW = ops.lm_solve_update_bwd(H, g, lam, delta, R, T, dRn.contiguous(), dTn.contiguous(),
                                                            None if dWn is None else dWn.contiguous(), ctx.eps, ctx.undamped_last)
         return dH, dg.reshape(g.shape), dlam.reshape(lam.shape), dR, dT, dW, None, None
+
+
+class _LMStepFn(torch.autograd.Function):
+    """(R', T', W') = banet_lm_step(H, g, rbar_sum, lambda-MLP or lambda, R, T, W): the lambda-MLP, damping, solve and update of one
+    iteration in one launch; backward = banet_lm_step_bwd, which re-runs the MLP and re-factors the system.  Saves H, g, rbar_sum, lambda,
+    delta, R, T and references to the MLP parameters: nothing per pixel, no MLP activation and no packed copy of the weights (they are packed
+    for each call).  mlp: the level's (filters, biases) x 5 flattened (gradients split back onto them), or none with lam [nb] given."""
+
+    @staticmethod
+    def forward(ctx, H, g, rbar_sum, lam, R, T, W, N, base, damping_eps, undamped_last, *mlp):
+        packed = ops.pack_mlp(list(zip(mlp[0::2], mlp[1::2]))) if mlp else None
+        Rn, Tn, Wn, delta, lout, status = ops.lm_step(H, g, rbar_sum, N, packed, base, R, T, W, lam=None if mlp else lam,
+                                                      damping_eps=damping_eps, undamped_last=undamped_last)
+        ctx.save_for_backward(H, g, rbar_sum, lout, delta, R, T, *mlp)
+        ctx.has_w = W is not None
+        ctx.N = int(N); ctx.base = float(base); ctx.eps = float(damping_eps); ctx.undamped_last = bool(undamped_last)
+        ctx.mark_non_differentiable(status)
+        if W is None:
+            return Rn, Tn, status
+        return Rn, Tn, Wn, status
+
+    @staticmethod
+    def backward(ctx, *grads):
+        H, g, rbar, lam, delta, R, T, *mlp = ctx.saved_tensors
+        nb, P = g.shape[0], H.shape[1]
+        dRn = grads[0] if grads[0] is not None else torch.zeros_like(R)
+        dTn = grads[1] if grads[1] is not None else torch.zeros_like(T)
+        dWn = None
+        if ctx.has_w:
+            dWn = grads[2] if grads[2] is not None else torch.zeros(nb, P - 6, 1, device=H.device)
+        packed = ops.pack_mlp(list(zip(mlp[0::2], mlp[1::2]))) if mlp else None
+        dH, dg, drb, dmlp, dlam, dR, dT, dW = ops.lm_step_bwd(H, g, rbar, ctx.N, packed, lam, delta, R, T, dRn.contiguous(), dTn.contiguous(),
+                                                              None if dWn is None else dWn.contiguous(), ctx.eps, ctx.undamped_last, ctx.base)
+        dparams = []
+        if mlp:
+            off = 0
+            for t in mlp:
+                dparams.append(dmlp[off:off + t.numel()].view(t.shape).to(t.dtype)); off += t.numel()
+        return (dH, dg.reshape(g.shape), drb, None if mlp else dlam, dR, dT, dW, None, None, None, None, *dparams)
+
+
+def lm_run(levels: Sequence[ops.Level], iters_per_level: int, R: Tensor, T: Tensor, W: Optional[Tensor],
+           mlp_params: Optional[Sequence[Optional[Sequence[Tuple[Tensor, Tensor]]]]] = None, lambda_fixed: Optional[float] = None,
+           l2_regularizer_base: Optional[float] = None, damping_eps: float = 1e-5, precision: int = -1, exact_sym: bool = False,
+           return_status: bool = False):
+    """Differentiable ops.lm_run: per level and iteration, the build (_LMBuildFn, the level's precision resolved as banet_lm_run resolves it)
+    and the fused step (_LMStepFn: lambda-MLP, damping, solve, update in one launch), W carried across levels.  The forward runs
+    ops.lm_run's kernels in its order and returns its bits.  Gradients reach every level's conv1, conv2, D, B and weight, R, T, W and each
+    level's lambda-MLP (filters, biases); intr and p are constants, as in iteration_fused.
+    mlp_params[l]: level l's [(filters [cin,cout], biases [cout])] x 5, used unless lambda_fixed is given (then lambda = lambda_fixed for every
+    pair).  l2_regularizer_base None: 1000 with a depth basis, 1 pose-only (ops.lm_run's default).  Where banet_lm_run would leave the fused
+    step for its three-kernel path ((K, C) beyond banet_lm_step's shared memory) this raises: it has no second path.
+    Returns (R', T', W') (, status [nb]: the bitwise or over the iterations, as ops.lm_run's)."""
+    from . import _lib
+    nb = R.shape[0]
+    K = 0 if W is None else W.shape[1]
+    if l2_regularizer_base is None:
+        l2_regularizer_base = 1000.0 if K > 0 else 1.0
+    status = torch.zeros(nb, device=R.device, dtype=torch.int32)
+    for li, lv in enumerate(levels):
+        Cl, Nl = lv.conv1.shape[2], lv.conv1.shape[1]
+        if not ops.lm_step_supported(nb, Cl, K):
+            raise _lib.BanetError(f"autograd.lm_run: level {li}: K={K}, C={Cl} do not fit the fused step (banet_lm_step), where banet_lm_run "
+                                  "takes its three-kernel path; this function has no second path")
+        if lambda_fixed is None:
+            if mlp_params is None or mlp_params[li] is None:
+                raise _lib.BanetError(f"autograd.lm_run: level {li} has no lambda-MLP parameters and lambda_fixed is None")
+            mlp, lam = [t for wb in mlp_params[li] for t in wb], None
+        else:
+            mlp, lam = [], torch.full((nb,), float(lambda_fixed), device=R.device, dtype=torch.float32)
+        for _ in range(iters_per_level):
+            H, g, rbar, _nvalid = _LMBuildFn.apply(lv.conv1, lv.conv2, lv.D, lv.B, R, T, W, lv.intr.detach(), lv.p.detach(), precision, exact_sym,
+                                                   lv.grid, lv.weight)
+            out = _LMStepFn.apply(H, g, rbar, lam, R, T, W, Nl, l2_regularizer_base, damping_eps, K > 0, *mlp)
+            if W is None:
+                R, T, st = out
+            else:
+                R, T, W, st = out
+            status = status | st
+    if return_status:
+        return R, T, W, status
+    return R, T, W
 
 
 class _WindowSolveUpdateFn(torch.autograd.Function):

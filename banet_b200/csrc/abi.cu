@@ -193,6 +193,34 @@ extern "C" int banet_lm_step(const float* H, const float* g, const float* rbar_s
                    R_out, T_out, W_out, delta, lambda_out, status, 0, (cudaStream_t)stream);
 }
 
+extern "C" size_t banet_lm_step_bwd_workspace_bytes(int nb, int C, int K)
+{
+    if (nb <= 0 || C <= 0 || K < 0 || !lm_step_supported(6 + K, C)) return 0;
+    return align_up((size_t)nb * lm_step_bwd_ws_floats(C) * sizeof(float), 256);
+}
+
+extern "C" int banet_lm_step_bwd(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K, const float* mlp_weights,
+                                 float base, const float* lambda, const float* delta, const banet_solve_opts_t* opts, const float* R, const float* T,
+                                 const float* dR_out, const float* dT_out, const float* dW_out, float* dH, float* dg, float* drbar_sum, float* dmlp,
+                                 float* dlambda, float* dR, float* dT, float* dW, void* ws, size_t ws_bytes, banet_stream_t stream)
+{
+    (void)base;                                                      // lambda = base ||rbar||^(2 + t) is given: its derivatives need no base
+    BANET_REQUIRE(H && g && lambda && delta && opts && R && T && dR_out && dT_out && dH && dg && dlambda && dR && dT && nb > 0 && K >= 0,
+                  BANET_ERR_BAD_ARG, "lm_step_bwd: bad argument");
+    BANET_REQUIRE(K == 0 || (dW_out && dW), BANET_ERR_BAD_ARG, "lm_step_bwd: K=%d but dW_out / dW is null", K);
+    BANET_REQUIRE(!mlp_weights || (rbar_sum && drbar_sum && dmlp && N > 0 && C > 0), BANET_ERR_BAD_ARG,
+                  "lm_step_bwd: the lambda-MLP needs rbar_sum, drbar_sum, dmlp, N > 0 and C > 0");
+    BANET_REQUIRE(!opts->vmatrix_batch_scramble, BANET_ERR_UNSUPPORTED, "lm_step_bwd: vmatrix_batch_scramble is not differentiated");
+    const int Cs = C > 0 ? C : 1;                                    // banet_lm_step's rule: the storage plan depends on C also with lambda given
+    BANET_REQUIRE(lm_step_supported(6 + K, Cs), BANET_ERR_UNSUPPORTED, "lm_step_bwd: K=%d, C=%d do not fit the fused step", K, Cs);
+    if (mlp_weights) {
+        const size_t need = banet_lm_step_bwd_workspace_bytes(nb, C, K);
+        BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_step_bwd: workspace %zu < %zu bytes", ws_bytes, need);
+    }
+    return lm_step_bwd(H, g, rbar_sum, nb, N, Cs, K, mlp_weights, lambda, delta, *opts, R, T, dR_out, dT_out, dW_out, dH, dg, drbar_sum, dmlp,
+                       dlambda, dR, dT, dW, reinterpret_cast<float*>(ws), (cudaStream_t)stream);
+}
+
 extern "C" int banet_lm_build_bwd_weighted(const banet_level_t* lv, const float* R, const float* T, const float* W,
                                            const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
                                            float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,

@@ -69,6 +69,12 @@ bool lm_step_uses_double(int P, int C);
 int lm_step(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K, const float* mlp, float base, const float* lambda_in,
             const StepMode& mode, const float* nvalid, const banet_solve_opts_t& opts, const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
             float* delta, float* lambda_out, int32_t* status, int status_accumulate, cudaStream_t st);
+// its backward (kStepBundleNet), in the forward's storage plan for (P, C); ws: nb * lm_step_bwd_ws_floats(C) floats when mlp != nullptr
+size_t lm_step_bwd_ws_floats(int C);
+int lm_step_bwd(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K, const float* mlp, const float* lambda,
+                const float* delta, const banet_solve_opts_t& opts, const float* R, const float* T, const float* gRn, const float* gTn,
+                const float* gWn, float* dH, float* dg, float* drbar_sum, float* dmlp, float* dlambda, float* dR, float* dT, float* dW,
+                float* ws, cudaStream_t st);
 
 int launch_pose_update(const float* delta, int nb, int P, const float* R, const float* T, float* R_out, float* T_out, cudaStream_t st);
 

@@ -20,6 +20,7 @@
 #include "common.cuh"
 #include "features.cuh"
 #include "lm_build.h"
+#include "lm_step.cuh"
 #include "pose_bwd.cuh"
 
 namespace banet {
@@ -415,6 +416,7 @@ __global__ void pose_update_bwd_kernel(const float* __restrict__ delta, int nb, 
 }
 
 constexpr int SB_THREADS = 1024;
+static_assert(SB_THREADS == STEP_THREADS, "solve_adjoint_outputs (lm_step.cuh) strides by STEP_THREADS");
 __host__ __device__ __forceinline__ int tri2(int i, int k) { return i * (i + 1) / 2 + k; }
 
 // u = Ht^-1 ddelta with the same Cholesky as lm_solve_kernel; dg (in: ddelta[0:npose] from pose_update_bwd_kernel, out: u).  npose = 6 for the
@@ -489,29 +491,8 @@ lm_solve_bwd_kernel(const float* __restrict__ H, const float* __restrict__ g, co
         }
     }
     __syncthreads();
-    const int flag = s_flag;
-    // dH = -u delta^T (1 + damp lambda on the diagonal), dg = u, dlambda = -sum_i u_i delta_i damp_i (H_ii + eps)
-    double part = 0.0;
-    for (int i = tid; i < P * P; i += SB_THREADS) {
-        const int rr = i / P, cc = i - rr * P;
-        float v = 0.f;
-        if (!flag) {
-            double t = -(double)uu[rr] * (double)r[cc];
-            if (rr == cc && rr < ndamped) { part += t * ((double)Hb[(size_t)rr * P + rr] + (double)eps); t *= 1.0 + (double)lam; }
-            v = (float)t;
-        }
-        dH[(size_t)b * P * P + i] = v;
-    }
-    for (int i = tid; i < P; i += SB_THREADS) dg[(size_t)b * P + i] = flag ? 0.f : (float)uu[i];
-    part += __shfl_xor_sync(0xffffffffu, part, 16); part += __shfl_xor_sync(0xffffffffu, part, 8); part += __shfl_xor_sync(0xffffffffu, part, 4);
-    part += __shfl_xor_sync(0xffffffffu, part, 2); part += __shfl_xor_sync(0xffffffffu, part, 1);
-    if ((tid & 31) == 0) s_dl[tid >> 5] = part;
-    __syncthreads();
-    if (tid == 0) {
-        double dl = 0.0;
-        for (int wq = 0; wq < SB_THREADS / 32; ++wq) dl += s_dl[wq];
-        dlambda[b] = flag ? 0.f : (float)dl;
-    }
+    const float dl = solve_adjoint_outputs<S>(uu, r, Hb, P, ndamped, eps, lam, s_flag, dH + (size_t)b * P * P, dg + (size_t)b * P, s_dl, tid);
+    if (tid == 0) dlambda[b] = dl;
 }
 
 int launch_pose_update_bwd(const float* delta, int nb, int P, const float* R, const float* T, const float* gRn, const float* gTn,

@@ -17,6 +17,7 @@
 // The reference's batch-interleaved VMatrix (vmatrix_batch_scramble, bundlenet.py:45) needs every pair's delta first: the host falls back to
 // the three-kernel path for that option.
 #include "lm_step.cuh"
+#include "pose_bwd.cuh"
 
 namespace banet {
 
@@ -94,6 +95,159 @@ lm_step_kernel(const float* __restrict__ H, const float* __restrict__ g, const f
     }
 }
 
+// Backward of lm_step_kernel in kStepBundleNet mode, one CTA per pair, in the forward's shared-memory layout and storage (S, FULL):
+//   1. the lambda-MLP forward again with step_lambda_mlp's code, every activation kept in the pair's workspace row (nothing extra is saved by
+//      the forward);
+//   2. the SE(3) update backward at the forward's step (pose_bwd.cuh): ddelta[0:6], dR, dT; dW = dW';
+//   3. the damped matrix factored as the forward did, with [ddelta[0:6] | dW'] as row P: u = Ht^-1 [ddelta | dW'];
+//   4. dH = -u delta^T ((1 + lambda) on the damped diagonal), dg = u, dlambda (solve_adjoint_outputs, shared with lm_solve_bwd_kernel);
+//   5. through lambda = base ||rbar||^(2 + t), t = tanh(z_5): dt = dlambda lambda ln||rbar||, d||rbar|| = dlambda lambda (2 + t) / ||rbar||,
+//      then the five layers backwards (warp per input row, fixed-order warp sums; selu' from the stored output a: scale if a > 0, else
+//      a + scale alpha), each layer's output delta stored next to its input activation; drbar_sum = drbar / N.
+// The skip is re-derived from H, g, lambda exactly as the forward decides it; a skipped pair gets zero dH, dg, dlambda, drbar_sum and a zero
+// workspace row (no MLP contribution) and passes dR', dT', dW' through (its delta is 0).
+template <typename S, bool FULL>
+__global__ void __launch_bounds__(STEP_THREADS)
+lm_step_bwd_kernel(const float* __restrict__ H, const float* __restrict__ g, const float* __restrict__ rbar_sum, int N, int C,
+                   const float* __restrict__ mlp, const float* __restrict__ lambda, const float* __restrict__ delta, int P, float eps, int ndamped,
+                   const float* __restrict__ R, const float* __restrict__ T, const float* __restrict__ gRn, const float* __restrict__ gTn,
+                   const float* __restrict__ gWn, float* __restrict__ dH, float* __restrict__ dg, float* __restrict__ drbar_sum,
+                   float* __restrict__ dlambda, float* __restrict__ dR, float* __restrict__ dT, float* __restrict__ dW, float* ws)
+{
+    extern __shared__ __align__(16) unsigned char smraw[];
+    S* A = reinterpret_cast<S*>(smraw);                              // the forward's layout (lm_step_kernel)
+    const int LD = (P + 1) | 1;
+    const size_t nA = FULL ? (size_t)(P + 1) * LD : (size_t)(P + 1) * (P + 2) / 2;
+    auto IX = [&](int i, int k) -> int { return FULL ? i * LD + k : i * (i + 1) / 2 + k; };
+    S* xs = A + nA;                                                  // [P] u
+    S* dinv = xs + P;                                                // [P] reciprocals of the Cholesky diagonal, then the forward's delta
+    S* dots = dinv + P;
+    float* mbuf = reinterpret_cast<float*>(dots + STEP_NB);          // MLP buffers as in the forward; the backward's deltas ping-pong in 2 x 4C
+    __shared__ int s_flag;
+    __shared__ float s_wpart[STEP_WARPS], s_lam, s_lam_unused, s_ddl[6], s_dn;
+    __shared__ double s_part[STEP_WARPS];
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, K = P - 6;
+    float* keep = mlp ? ws + (size_t)b * mlp_ws_stride(C) : nullptr;
+    const float invN = 1.0f / (float)N;
+    if (tid == 0) s_flag = 0;
+    __syncthreads();
+
+    // ---- 1. the forward's lambda-MLP, activations kept (lambda itself is the forward's, given) ---------------------------------------------
+    if (mlp) {
+        float part = 0.f;
+        for (int c = tid; c < C; c += STEP_THREADS) { const float r = rbar_sum[(size_t)b * C + c] * invN; mbuf[c] = r; keep[c] = r; part += r * r; }
+        step_lambda_mlp<true>(part, mbuf, C, mlp, 1.f, kStepBundleNet.lambda_exp0, s_wpart, &s_lam, &s_lam_unused, tid, keep);
+    }
+    const float lam = lambda[b];
+
+    // ---- 2. SE(3) update backward at the forward's step -----------------------------------------------------------------------------------
+    if (tid == 0) {
+        double dl[6];
+        for (int i = 0; i < 6; ++i) { dl[i] = delta[(size_t)b * P + i]; if (!isfinite(dl[i])) dl[i] = 0.0; }
+        pose_update_bwd_one(dl, R + (size_t)b * 9, T + (size_t)b * 3, gRn + (size_t)b * 9, gTn + (size_t)b * 3, s_ddl, dR + (size_t)b * 9,
+                            dT + (size_t)b * 3);
+    }
+    __syncthreads();
+
+    // ---- 3. the forward's damped matrix, right-hand side [ddelta | dW'] as row P ----------------------------------------------------------
+    const float* Hb = H + (size_t)b * P * P;
+    int bad = 0;
+    for (int i = warp; i < P; i += STEP_WARPS)
+        for (int k = lane; k <= i; k += 32) {
+            const float v = Hb[(size_t)i * P + k];
+            if (!isfinite(v)) bad = 1;
+            S sv = (S)v;
+            if (k == i && i < ndamped) sv += ((S)v + (S)eps) * (S)lam;
+            A[IX(i, k)] = sv;
+        }
+    for (int k = tid; k < P; k += STEP_THREADS) {
+        if (!isfinite(g[(size_t)b * P + k])) bad = 1;                // the forward skipped the step on a non-finite right-hand side
+        float v;
+        if (k < 6) v = s_ddl[k];
+        else { v = gWn[(size_t)b * K + k - 6]; dW[(size_t)b * K + k - 6] = v; }      // W' = W + delta_d
+        A[IX(P, k)] = (S)v;
+    }
+    if (!isfinite(lam)) bad = 1;
+    if (bad) atomicOr(&s_flag, 2);
+    __syncthreads();
+    step_cholesky_solve<S, FULL>(A, P, xs, dinv, dots, &s_flag, tid);
+
+    // ---- 4. dH, dg, dlambda ----------------------------------------------------------------------------------------------------------------
+    for (int i = tid; i < P; i += STEP_THREADS) dinv[i] = (S)delta[(size_t)b * P + i];
+    __syncthreads();
+    const int flag = s_flag;
+    const float dlam = solve_adjoint_outputs<S>(xs, dinv, Hb, P, ndamped, eps, lam, flag, dH + (size_t)b * P * P, dg + (size_t)b * P, s_part, tid);
+    if (tid == 0) dlambda[b] = dlam;
+    if (!mlp) return;
+    if (flag) {                                                      // skipped: no MLP contribution
+        for (size_t i = tid; i < mlp_ws_stride(C); i += STEP_THREADS) keep[i] = 0.f;
+        for (int c = tid; c < C; c += STEP_THREADS) drbar_sum[(size_t)b * C + c] = 0.f;
+        return;
+    }
+
+    // ---- 5. lambda = base ||rbar||^(2 + t) and the five layers backwards (bundlenet.py:244-253) ------------------------------------------
+    float* dout = mbuf; float* din = mbuf + 4 * C;
+    if (tid == 0) {
+        const double nrm = keep[mlp_norm_off(C)], t = keep[mlp_act_off(5, C)], L = (double)dlam * (double)lam;
+        double dt = 0.0, dn = 0.0;
+        if (nrm > 0.0) { dt = L * log(nrm); dn = L * (2.0 + t) / (nrm * nrm); }
+        s_dn = (float)dn;                                            // drbar_i gets dn * rbar_i (d||rbar|| / d rbar_i = rbar_i / ||rbar||)
+        dout[0] = (float)(dt * (1.0 - t * t));
+    }
+    __syncthreads();
+    const float selu_scale = 1.0507009873554804934193349852946f, selu_sa = 1.0507009873554804934193349852946f * 1.6732632423543772848170429916717f;
+    const int dims[6] = {C, 2 * C, 4 * C, 2 * C, C, 1};
+    size_t woff[5];
+    woff[0] = 0;
+    for (int l = 1; l < 5; ++l) woff[l] = woff[l - 1] + (size_t)dims[l - 1] * dims[l] + dims[l];
+    for (int l = 4; l >= 0; --l) {
+        const int cin = dims[l], cout = dims[l + 1];
+        const float* Wm = mlp + woff[l];
+        for (int j = tid; j < cout; j += STEP_THREADS) keep[mlp_delta_off(l, C) + j] = dout[j];
+        for (int i = warp; i < cin; i += STEP_WARPS) {                // da_i = sum_j W[i][j] delta_j: a warp per row, lanes over the row
+            float s = 0.f;
+            for (int j = lane; j < cout; j += 32) s = fmaf(__ldg(Wm + (size_t)i * cout + j), dout[j], s);
+            s = warp_sum(s);
+            if (lane == 0) {
+                if (l > 0) { const float a = keep[mlp_act_off(l, C) + i]; din[i] = s * (a > 0.f ? selu_scale : a + selu_sa); }
+                else drbar_sum[(size_t)b * C + i] = (s + s_dn * keep[i]) * invN;
+            }
+        }
+        __syncthreads();
+        float* tmp = dout; dout = din; din = tmp;
+    }
+}
+
+// dmlp = sum over pairs, in pair order, of each layer's outer product a_{l} delta_l^T (filters) and delta_l (biases): one thread per parameter,
+// no atomics (bit-reproducible, independent of what dmlp held).  Same packing as the weights: [W1, b1, ..., W5, b5].
+__global__ void lm_mlp_grad_kernel(const float* __restrict__ ws, int nb, int C, float* __restrict__ dmlp)
+{
+    const size_t n = (size_t)20 * C * C + (size_t)10 * C + 1;
+    const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= n) return;
+    const int dims[6] = {C, 2 * C, 4 * C, 2 * C, C, 1};
+    size_t off = 0;
+    int l = 0;
+    for (; l < 4; ++l) {
+        const size_t sz = (size_t)dims[l] * dims[l + 1] + dims[l + 1];
+        if (idx < off + sz) break;
+        off += sz;
+    }
+    const int cin = dims[l], cout = dims[l + 1];
+    const size_t r = idx - off, stride = mlp_ws_stride(C);
+    float s = 0.f;
+    if (r < (size_t)cin * cout) {
+        const int i = (int)(r / cout), j = (int)(r - (size_t)i * cout);
+        const float* a = ws + mlp_act_off(l, C) + i;
+        const float* d = ws + mlp_delta_off(l, C) + j;
+        for (int b = 0; b < nb; ++b) s = fmaf(a[(size_t)b * stride], d[(size_t)b * stride], s);
+    } else {
+        const float* d = ws + mlp_delta_off(l, C) + (r - (size_t)cin * cout);
+        for (int b = 0; b < nb; ++b) s += d[(size_t)b * stride];
+    }
+    dmlp[idx] = s;
+}
+
 size_t lm_step_smem(int P, int C, bool use_double, bool full)
 {
     const size_t nA = (full ? (size_t)(P + 1) * ((P + 1) | 1) : (size_t)(P + 1) * (P + 2) / 2) + 2 * (size_t)P + STEP_NB;
@@ -106,6 +260,20 @@ bool lm_step_supported(int P, int C) { return lm_step_smem(P, C, false, false) <
 // the precision this picks for its forward
 bool lm_step_uses_double(int P, int C) { return lm_step_smem(P, C, true, false) <= 200 * 1024; }
 
+// the storage of lm_step_kernel and of its backward, which must factor alike (the backward re-derives the forward's skip from its own
+// factorisation) and which need the same shared memory: one plan for both
+namespace {
+struct StepPlan { bool full, use_double; size_t smem; };
+StepPlan step_plan(int P, int C)
+{
+    StepPlan p;
+    p.full = lm_step_smem(P, C, true, true) <= 200 * 1024;
+    p.use_double = lm_step_uses_double(P, C);
+    p.smem = lm_step_smem(P, C, p.use_double, p.full);
+    return p;
+}
+}  // namespace
+
 // lambda_in != nullptr: used as is; else lambda = base * ||rbar||^(exp0 + MLP(rbar)) (MLP term 0 when mlp == nullptr).
 // In-place R/T/W (R_out == R ...) is fine: a pair's CTA reads before it writes.
 int lm_step(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K, const float* mlp, float base, const float* lambda_in,
@@ -114,9 +282,8 @@ int lm_step(const float* H, const float* g, const float* rbar_sum, int nb, int N
 {
     const int P = 6 + K;
     const int ndamped = opts.undamped_last ? P - 1 : P;
-    const bool full = lm_step_smem(P, C, true, true) <= 200 * 1024;
-    const bool use_double = lm_step_uses_double(P, C);
-    const size_t smem = lm_step_smem(P, C, use_double, full);
+    const StepPlan plan = step_plan(P, C);
+    const size_t smem = plan.smem;
     BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_step: P=%d, C=%d do not fit shared memory", P, C);
     auto launch = [&](auto kern) -> int {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -126,11 +293,45 @@ int lm_step(const float* H, const float* g, const float* rbar_sum, int nb, int N
         return BANET_OK;
     };
     int rc;
-    if (full) rc = launch(lm_step_kernel<double, true>);
-    else if (use_double) rc = launch(lm_step_kernel<double, false>);
+    if (plan.full) rc = launch(lm_step_kernel<double, true>);
+    else if (plan.use_double) rc = launch(lm_step_kernel<double, false>);
     else rc = launch(lm_step_kernel<float, false>);
     if (rc) return rc;
     BANET_CUDA_LAUNCH_CHECK("lm_step_kernel launch");
+    return BANET_OK;
+}
+
+size_t lm_step_bwd_ws_floats(int C) { return mlp_ws_stride(C); }
+
+// Backward of lm_step (kStepBundleNet).  mlp == nullptr: lambda was given and only dlambda carries its gradient (drbar_sum, dmlp, ws unused).
+int lm_step_bwd(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K, const float* mlp, const float* lambda,
+                const float* delta, const banet_solve_opts_t& opts, const float* R, const float* T, const float* gRn, const float* gTn,
+                const float* gWn, float* dH, float* dg, float* drbar_sum, float* dmlp, float* dlambda, float* dR, float* dT, float* dW,
+                float* ws, cudaStream_t st)
+{
+    const int P = 6 + K;
+    const int ndamped = opts.undamped_last ? P - 1 : P;
+    const StepPlan plan = step_plan(P, C);
+    const size_t smem = plan.smem;
+    BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_step_bwd: P=%d, C=%d do not fit shared memory", P, C);
+    auto launch = [&](auto kern) -> int {
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) { set_error("lm_step_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
+        kern<<<nb, STEP_THREADS, smem, st>>>(H, g, rbar_sum, N, C, mlp, lambda, delta, P, opts.damping_eps, ndamped, R, T, gRn, gTn, gWn,
+                                             dH, dg, drbar_sum, dlambda, dR, dT, dW, ws);
+        return BANET_OK;
+    };
+    int rc;
+    if (plan.full) rc = launch(lm_step_bwd_kernel<double, true>);
+    else if (plan.use_double) rc = launch(lm_step_bwd_kernel<double, false>);
+    else rc = launch(lm_step_bwd_kernel<float, false>);
+    if (rc) return rc;
+    BANET_CUDA_LAUNCH_CHECK("lm_step_bwd_kernel launch");
+    if (mlp) {
+        const size_t n = (size_t)20 * C * C + (size_t)10 * C + 1;
+        lm_mlp_grad_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ws, nb, C, dmlp);
+        BANET_CUDA_LAUNCH_CHECK("lm_mlp_grad_kernel launch");
+    }
     return BANET_OK;
 }
 

@@ -66,8 +66,17 @@ __device__ __forceinline__ void dense_layer(const float* __restrict__ in, const 
 
 // lambda = base * ||rbar||^(exp0 + MLP(rbar)) (bundlenet.py:243-253; MLP term 0 when mlp == nullptr).  On entry mbuf[0:C] holds rbar and `part`
 // is this thread's share of ||rbar||^2; mbuf: 2 x 4C floats + max(4C, 1024) floats of slice partials.  Thread 0 writes *lambda_out.
+// KEEP (the step's backward): the same arithmetic, and layer l's output activation also goes to keep + mlp_act_off(l + 1, C) and ||rbar||
+// to keep[mlp_norm_off(C)].  That is the per-pair workspace row of lm_step_bwd: activations a_0 = rbar (stored by the caller), a_1..a_5,
+// then each layer's output delta (the gradient of its pre-activation), then ||rbar||.
+__host__ __device__ __forceinline__ int mlp_act_off(int l, int C) { const int o[6] = {0, C, 3 * C, 7 * C, 9 * C, 10 * C}; return o[l]; }
+__host__ __device__ __forceinline__ int mlp_delta_off(int l, int C) { const int o[5] = {10 * C + 1, 12 * C + 1, 16 * C + 1, 18 * C + 1, 19 * C + 1}; return o[l]; }
+__host__ __device__ __forceinline__ int mlp_norm_off(int C) { return 19 * C + 2; }
+__host__ __device__ __forceinline__ size_t mlp_ws_stride(int C) { return ((size_t)19 * C + 3 + 3) & ~(size_t)3; }   // floats per pair, 16-B rows
+
+template <bool KEEP = false>
 __device__ __forceinline__ float step_lambda_mlp(float part, float* mbuf, int C, const float* __restrict__ mlp, float base, float exp0,
-                                                 float* s_wpart, float* s_lam, float* lambda_out, int tid)
+                                                 float* s_wpart, float* s_lam, float* lambda_out, int tid, float* keep = nullptr)
 {
     const int lane = tid & 31, warp = tid >> 5;
     float* bufA = mbuf; float* bufB = mbuf + 4 * C; float* acc = mbuf + 8 * C;
@@ -80,6 +89,7 @@ __device__ __forceinline__ float step_lambda_mlp(float part, float* mbuf, int C,
     for (int l = 0; l < (mlp ? 5 : 0); ++l) {
         const int cin = dims[l], cout = dims[l + 1];
         dense_layer(in, wp, wp + (size_t)cin * cout, cin, cout, l == 4, acc, out, tid);
+        if constexpr (KEEP) for (int j = tid; j < cout; j += STEP_THREADS) keep[mlp_act_off(l + 1, C) + j] = out[j];
         wp += (size_t)cin * cout + cout;
         float* tmp = in; in = out; out = tmp;
         __syncthreads();
@@ -89,6 +99,7 @@ __device__ __forceinline__ float step_lambda_mlp(float part, float* mbuf, int C,
         float norm2 = 0.f;
         for (int wq = 0; wq < STEP_WARPS; ++wq) norm2 += s_wpart[wq];               // fixed order
         *s_lam = base * powf(sqrtf(norm2), exp0 + (mlp ? in[0] : 0.f)); *lambda_out = *s_lam;
+        if constexpr (KEEP) keep[mlp_norm_off(C)] = sqrtf(norm2);
     }
     __syncthreads();
     return *s_lam;
@@ -222,6 +233,37 @@ __device__ __forceinline__ void step_cholesky_solve(S* A, int P, S* xs, S* dinv,
         }
         __syncthreads();
     }
+}
+
+// Adjoint of the damped solve delta = Ht^-1 g, Ht = H + diag(damp (diag H + eps)) lambda, given u = Ht^-1 ddelta (bundlenet.py:264-267):
+//   dH = -u delta^T with the factor (1 + lambda) on the damped diagonal, dg = u, dlambda = -sum_{i < ndamped} u_i delta_i (H_ii + eps).
+// u, dl (= delta) [P] in shared memory, Hb the pair's [P,P] H; flag != 0 (the forward skipped the step): every output 0.  All STEP_THREADS
+// threads call it; dlambda is summed in double in a fixed order (bit-reproducible) and returned in thread 0.
+template <typename S>
+__device__ __forceinline__ float solve_adjoint_outputs(const S* u, const S* dl, const float* __restrict__ Hb, int P, int ndamped, float eps,
+                                                       float lam, int flag, float* __restrict__ dHb, float* __restrict__ dgb, double* s_part,
+                                                       int tid)
+{
+    double part = 0.0;
+    for (int i = tid; i < P * P; i += STEP_THREADS) {
+        const int rr = i / P, cc = i - rr * P;
+        float v = 0.f;
+        if (!flag) {
+            double t = -(double)u[rr] * (double)dl[cc];
+            if (rr == cc && rr < ndamped) { part += t * ((double)Hb[(size_t)rr * P + rr] + (double)eps); t *= 1.0 + (double)lam; }
+            v = (float)t;
+        }
+        dHb[i] = v;
+    }
+    for (int i = tid; i < P; i += STEP_THREADS) dgb[i] = flag ? 0.f : (float)u[i];
+    part += __shfl_xor_sync(0xffffffffu, part, 16); part += __shfl_xor_sync(0xffffffffu, part, 8); part += __shfl_xor_sync(0xffffffffu, part, 4);
+    part += __shfl_xor_sync(0xffffffffu, part, 2); part += __shfl_xor_sync(0xffffffffu, part, 1);
+    if ((tid & 31) == 0) s_part[tid >> 5] = part;
+    __syncthreads();
+    double dlam = 0.0;
+    if (tid == 0)
+        for (int wq = 0; wq < STEP_WARPS; ++wq) dlam += s_part[wq];
+    return flag ? 0.f : (float)dlam;
 }
 
 // R' = exp(w) R, T' = V(w) t + exp(w) T in double (bundlenet.py:269-275) for one pair: dl = (w, t), Rb [3,3], Tb [3] -> Ro, To (may alias).

@@ -612,6 +612,46 @@ def lm_solve_update_bwd(H: Tensor, g: Tensor, lam: Tensor, delta: Tensor, R: Ten
     return dH, dg, dlam, dR, dT, dW
 
 
+def lm_step_bwd(H: Tensor, g: Tensor, rbar_sum: Optional[Tensor], N: int, mlp_packed: Optional[Tensor], lam: Tensor, delta: Tensor, R: Tensor,
+                T: Tensor, dRn: Tensor, dTn: Tensor, dWn: Optional[Tensor], damping_eps: float = 1e-5, undamped_last: Optional[bool] = None,
+                base: float = 1000.0, workspace: Optional[Tensor] = None):
+    """Backward of lm_step (banet_lm_step_bwd).  lam, delta: the lambda and delta lm_step returned; rbar_sum, N as given to lm_step (rbar_sum
+    also sets the storage plan when lambda was given, as in the forward).  -> dH [nb,P,P], dg [nb,P], drbar_sum [nb,C] (None without the MLP),
+    dmlp (packed like mlp_packed; None without it), dlambda [nb], dR, dT, dW.  workspace: a uint8 buffer to use when it is large enough."""
+    lib = load()
+    Hc = _chk(H, "H"); nb, P, _ = Hc.shape
+    K = P - 6
+    if undamped_last is None:
+        undamped_last = K > 0
+    gc = _chk(g.reshape(nb, P), "g", (nb, P)); lc = _chk(lam.reshape(nb), "lambda", (nb,)); dl = _chk(delta, "delta", (nb, P))
+    rb = None if rbar_sum is None else _chk(rbar_sum, "rbar_sum"); mp = None if mlp_packed is None else _chk(mlp_packed, "mlp_packed")
+    Cc = 1 if rb is None else rb.shape[1]
+    R = _chk(R, "R", (nb, 3, 3)); T = _chk(T, "T", (nb, 3, 1))
+    gR = _chk(dRn, "dR_out", (nb, 3, 3)); gT = _chk(dTn, "dT_out", (nb, 3, 1)); gW = None if K == 0 else _chk(dWn, "dW_out", (nb, K, 1))
+    dev = Hc.device
+    dH = torch.empty(nb, P, P, device=dev); dg = torch.empty(nb, P, device=dev); dlam = torch.empty(nb, device=dev)
+    dR = torch.empty(nb, 3, 3, device=dev); dT = torch.empty(nb, 3, 1, device=dev); dW = None if K == 0 else torch.empty(nb, K, 1, device=dev)
+    drb = None if mp is None else torch.empty(nb, Cc, device=dev)
+    dmlp = None if mp is None else torch.empty_like(mp)
+    ws = None
+    if mp is not None:
+        if mp.numel() != lib.banet_mlp_param_count(Cc):
+            raise _lib.BanetError(f"mlp_packed has {mp.numel()} params, expected {lib.banet_mlp_param_count(Cc)} for C={Cc}")
+        nbytes = lib.banet_lm_step_bwd_workspace_bytes(nb, Cc, K)
+        ws = workspace if workspace is not None and workspace.numel() >= nbytes else _ws(nbytes, dev)
+    opts = BanetSolveOpts(float(damping_eps), int(undamped_last), 0)
+    check(lib.banet_lm_step_bwd(Hc.data_ptr(), gc.data_ptr(), _ptr(rb), nb, int(N), Cc, K, _ptr(mp), float(base), lc.data_ptr(), dl.data_ptr(),
+                                C.byref(opts), R.data_ptr(), T.data_ptr(), gR.data_ptr(), gT.data_ptr(), _ptr(gW), dH.data_ptr(), dg.data_ptr(),
+                                _ptr(drb), _ptr(dmlp), dlam.data_ptr(), dR.data_ptr(), dT.data_ptr(), _ptr(dW), _ptr(ws),
+                                0 if ws is None else ws.numel(), _stream()), "banet_lm_step_bwd")
+    return dH, dg, drb, dmlp, dlam, dR, dT, dW
+
+
+def lm_step_supported(nb: int, C: int, K: int) -> bool:
+    """Whether banet_lm_step and its backward take K depth bases at MLP width C (C = 1 when lambda is given without rbar_sum)."""
+    return load().banet_lm_step_bwd_workspace_bytes(int(nb), int(C), int(K)) > 0
+
+
 def lm_window_solve_update_bwd(H: Tensor, g: Tensor, lam: Tensor, delta: Tensor, R: Tensor, T: Tensor, dRn: Tensor, dTn: Tensor, dWn: Tensor,
                                damping_eps: float = 1e-5, undamped_last: bool = True):
     """Backward of lm_window_solve_update (banet_lm_window_solve_update_bwd) -> dH [nf,P,P], dg [nf,P], dlambda [1], dR, dT, dW [K,1]."""

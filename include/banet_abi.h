@@ -226,6 +226,27 @@ int    banet_lm_solve_update_bwd(const float* H, const float* g, const float* la
                                  const float* dR_out, const float* dT_out, const float* dW_out,
                                  float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW,
                                  banet_stream_t stream);
+/* Backward of banet_lm_step (lambda-MLP + damping + solve + update in one launch): gradients of (R',T',W') [dR_out, dT_out, dW_out] ->
+ * dH [nb,P,P] (not symmetric, as banet_lm_build_bwd takes it), dg [nb,P], drbar_sum [nb,C], dmlp [banet_mlp_param_count(C)], dlambda [nb],
+ * dR, dT, dW; every output is overwritten (dmlp too: it is not accumulated).  The arguments up to mlp_weights and base are the forward's;
+ * lambda [nb] and delta [nb,P] are the lambda_out and delta the forward returned.  mlp_weights NULL: the forward was given lambda, dlambda
+ * carries its gradient, and rbar_sum, drbar_sum, dmlp and ws may be NULL.  With the MLP, dlambda is the gradient w.r.t. the lambda the MLP
+ * produced, and drbar_sum and dmlp carry it on through lambda = base * ||rbar||^(2 + MLP(rbar)) (rbar = rbar_sum / N).  dmlp is packed like
+ * mlp_weights and summed over the pairs in a fixed order: bit-reproducible, independent of what ws held.
+ * The kernel re-factors the damped system in the storage the forward used for this (P, C) (one plan for both) and re-derives the forward's
+ * skip from H, g and lambda: a skipped pair (status != 0, delta = 0) gets zero dH, dg, dlambda, drbar_sum, contributes nothing to dmlp and
+ * passes dR_out, dT_out, dW_out through; other pairs are not affected.  K = 0 is pose-only (opts->undamped_last as in the forward).
+ * Argument errors, reported before any CUDA call: a null pointer BANET_ERR_BAD_ARG; vmatrix_batch_scramble != 0 and a (K, C) that
+ * banet_lm_step rejects BANET_ERR_UNSUPPORTED (the same edge: the backward needs no more shared memory than the forward); ws smaller than
+ * banet_lm_step_bwd_workspace_bytes(nb, C, K) with the MLP BANET_ERR_WORKSPACE.  The workspace query returns 0 for a (K, C) that
+ * banet_lm_step rejects. */
+size_t banet_lm_step_bwd_workspace_bytes(int nb, int C, int K);
+int    banet_lm_step_bwd(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K,
+                         const float* mlp_weights, float base, const float* lambda, const float* delta,
+                         const banet_solve_opts_t* opts, const float* R, const float* T,
+                         const float* dR_out, const float* dT_out, const float* dW_out,
+                         float* dH, float* dg, float* drbar_sum, float* dmlp, float* dlambda,
+                         float* dR, float* dT, float* dW, void* ws, size_t ws_bytes, banet_stream_t stream);
 /* Backward of banet_grad_fixed_concat (transposed REFLECT stencil + the half swap): dconv2 [nb,h,w,3C] -> dF [nb,h,w,C]. */
 int    banet_grad_fixed_concat_bwd(const float* dconv2, int nb, int h, int w, int C, int swap_halves,
                                    float* dF, banet_stream_t stream);
