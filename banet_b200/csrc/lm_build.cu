@@ -17,6 +17,7 @@
 #include "common.cuh"
 #include "features.cuh"
 #include "lm_build.h"
+#include "point.cuh"
 
 namespace banet {
 
@@ -38,46 +39,6 @@ template <int KP> struct BuildSmem {
     static constexpr int off_cc = off_pose + 16;                        // [2][32]
     static constexpr int off_rb = off_cc + 64;                          // [BUILD_WARPS][C]
     static size_t bytes(int C) { return (size_t)(off_rb + BUILD_WARPS * C) * sizeof(float); }
-};
-
-template <int G> __device__ __forceinline__ void lds_group(const float* p, float* out);
-template <> __device__ __forceinline__ void lds_group<1>(const float* p, float* o) { o[0] = p[0]; }
-template <> __device__ __forceinline__ void lds_group<2>(const float* p, float* o) {
-    float2 v = *reinterpret_cast<const float2*>(p); o[0] = v.x; o[1] = v.y; }
-template <> __device__ __forceinline__ void lds_group<4>(const float* p, float* o) {
-    float4 v = *reinterpret_cast<const float4*>(p); o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w; }
-
-__device__ __forceinline__ int reflect_idx(int i, int n) {      // tf.pad REFLECT by one (bundlenet.py:97)
-    return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i);
-}
-
-// ---- S2 helper: accumulate one group of VEC channels of one pixel ------------------------------
-// TF: element type of the feature loads (float, or bf16 widened exactly on load); the |diff| sums in smem are always fp32
-template <int VEC, typename TF = float> struct ChanVec;
-template <> struct ChanVec<4> {
-    float v[4];
-    __device__ __forceinline__ void load(const float* p) { float4 t = __ldg(reinterpret_cast<const float4*>(p)); v[0]=t.x; v[1]=t.y; v[2]=t.z; v[3]=t.w; }
-    __device__ __forceinline__ void load_stream(const float* p) { float4 t = ld_stream_f4(p); v[0]=t.x; v[1]=t.y; v[2]=t.z; v[3]=t.w; }
-    __device__ __forceinline__ void load_smem(const float* p) { float4 t = *reinterpret_cast<const float4*>(p); v[0]=t.x; v[1]=t.y; v[2]=t.z; v[3]=t.w; }
-    __device__ __forceinline__ void store_smem(float* p) const { *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]); }
-};
-template <> struct ChanVec<1> {
-    float v[1];
-    __device__ __forceinline__ void load(const float* p) { v[0] = __ldg(p); }
-    __device__ __forceinline__ void load_stream(const float* p) { v[0] = ld_stream_f1(p); }
-    __device__ __forceinline__ void load_smem(const float* p) { v[0] = p[0]; }
-    __device__ __forceinline__ void store_smem(float* p) const { p[0] = v[0]; }
-};
-template <> struct ChanVec<4, bf16> {
-    float v[4];
-    __device__ __forceinline__ void set(uint2 t) { v[0] = bf16_lo(t.x); v[1] = bf16_hi(t.x); v[2] = bf16_lo(t.y); v[3] = bf16_hi(t.y); }
-    __device__ __forceinline__ void load(const bf16* p) { set(__ldg(reinterpret_cast<const uint2*>(p))); }
-    __device__ __forceinline__ void load_stream(const bf16* p) { set(ld_stream_bf4(p)); }
-};
-template <> struct ChanVec<1, bf16> {
-    float v[1];
-    __device__ __forceinline__ void load(const bf16* p) { v[0] = ldg_feat(p); }
-    __device__ __forceinline__ void load_stream(const bf16* p) { v[0] = ld_stream_bf1(p); }
 };
 
 // 4 consecutive basis entries of a read-once stream, widened (bf16: 8 B, 8-B aligned)
@@ -226,29 +187,12 @@ lm_build_kernel(const BuildParams prm)
                 const float* pp = prm.p + (size_t)b * 3 * N + n0 + n;
                 const float p0 = pp[0], p1 = pp[N], p2 = pp[2 * (size_t)N];
                 float Dt = prm.D[gi];
-                if constexpr (KP > 0) {
-                    float d0 = 0.f, d1 = 0.f, d2 = 0.f, d3 = 0.f;
-#pragma unroll 4
-                    for (int k = 0; k < KP; k += 4) {
-                        const float4 bv = *reinterpret_cast<const float4*>(Bs + n * LDB + k);
-                        const float4 wv = *reinterpret_cast<const float4*>(sW + k);
-                        d0 = fmaf(bv.x, wv.x, d0); d1 = fmaf(bv.y, wv.y, d1);
-                        d2 = fmaf(bv.z, wv.z, d2); d3 = fmaf(bv.w, wv.w, d3);
-                    }
-                    Dt += (d0 + d1) + (d2 + d3);
-                }
-                rx = sPose[0] * p0 + sPose[1] * p1 + sPose[2] * p2;
-                ry = sPose[3] * p0 + sPose[4] * p1 + sPose[5] * p2;
-                rz = sPose[6] * p0 + sPose[7] * p1 + sPose[8] * p2;
-                const float X = rx * Dt + sPose[9], Y = ry * Dt + sPose[10], Z = rz * Dt + sPose[11];
-                x = X / Z; y = Y / Z; iZ = 1.0f / Z;
-                const float u = sPose[12] * x + sPose[14], v = sPose[13] * y + sPose[15];
-                // reference mask: not(px<0 | px>w-1 | py<0 | py>h-1); non-finite projections are masked too
-                const bool ok = (u >= 0.f) && (u <= (float)(w - 1)) && (v >= 0.f) && (v <= (float)(h - 1)) && isfinite(iZ);
-                if (ok) {
+                if constexpr (KP > 0) Dt += basis_dot<KP>(Bs + n * LDB, sW);
+                const Projection pr(sPose, p0, p1, p2, Dt);
+                rx = pr.rx; ry = pr.ry; rz = pr.rz; x = pr.x; y = pr.y; iZ = pr.iZ;
+                if (pr.in_bounds(h, w)) {
                     mask = 1.f;
-                    const float fu = floorf(u), fv = floorf(v);
-                    x0 = (int)fu; y0 = (int)fv; dx = u - fu; dy = v - fv;
+                    tap_corner(pr.u, pr.v, x0, y0, dx, dy);
                 }
             }
             rec[R_X0 * TILE_PX + n] = __int_as_float(x0); rec[R_Y0 * TILE_PX + n] = __int_as_float(y0);
@@ -261,72 +205,25 @@ lm_build_kernel(const BuildParams prm)
         // ---- S2: feature gather, warp per pixel, lanes over channels (bundlenet.py:230-239) ------
         for (int i = 0; i < TILE_PX / BUILD_WARPS; ++i) {
             const int n = i * BUILD_WARPS + warp;
-            float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f;
+            PointMQ mq{0.f, 0.f, 0.f, 0.f, 0.f};
             if (rec[R_MASK * TILE_PX + n] != 0.f) {
-                const int x0 = __float_as_int(rec[R_X0 * TILE_PX + n]), y0 = __float_as_int(rec[R_Y0 * TILE_PX + n]);
-                const float dx = rec[R_DX * TILE_PX + n], dy = rec[R_DY * TILE_PX + n];
-                const int x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
-                const float w00 = (1.f - dx) * (1.f - dy), w01 = dx * (1.f - dy), w10 = (1.f - dx) * dy, w11 = dx * dy;
+                const Taps tp(__float_as_int(rec[R_X0 * TILE_PX + n]), __float_as_int(rec[R_Y0 * TILE_PX + n]), rec[R_DX * TILE_PX + n], rec[R_DY * TILE_PX + n], h, w);
                 const TF* img = static_cast<const TF*>(prm.conv2) + (size_t)b * h * w * c2;
-                const TF* t00 = img + ((size_t)y0 * w + x0) * c2;
-                const TF* t01 = img + ((size_t)y0 * w + x1) * c2;
-                const TF* t10 = img + ((size_t)y1 * w + x0) * c2;
-                const TF* t11 = img + ((size_t)y1 * w + x1) * c2;
                 const TF* c1 = static_cast<const TF*>(prm.conv1) + ((size_t)b * N + n0 + n) * C;
                 float* myRb = sRb + warp * C;
+                const TapGather<TF> tg(img, tp, h, w, C, c2);
                 for (int c = lane * VEC; c < C; c += 32 * VEC) {
-                    ChanVec<VEC, TF> f1, a00, a01, a10, a11;
-                    ChanVec<VEC> gx, gy;
+                    ChanVec<VEC, TF> f1;
                     f1.load_stream(c1 + c);
-                    a00.load(t00 + c); a01.load(t01 + c); a10.load(t10 + c); a11.load(t11 + c);
-                    if (!fly_grad) {
-                        ChanVec<VEC, TF> g00, g01, g10, g11;
-                        g00.load(t00 + C + c); g01.load(t01 + C + c); g10.load(t10 + C + c); g11.load(t11 + C + c);
-#pragma unroll
-                        for (int u = 0; u < VEC; ++u) gx.v[u] = w00 * g00.v[u] + w01 * g01.v[u] + w10 * g10.v[u] + w11 * g11.v[u];
-                        g00.load(t00 + 2 * C + c); g01.load(t01 + 2 * C + c); g10.load(t10 + 2 * C + c); g11.load(t11 + 2 * C + c);
-#pragma unroll
-                        for (int u = 0; u < VEC; ++u) gy.v[u] = w00 * g00.v[u] + w01 * g01.v[u] + w10 * g10.v[u] + w11 * g11.v[u];
-                    } else {
-                        // F2-only map: central differences with REFLECT-by-one borders (bundlenet.py:92-100) at each tap
-#pragma unroll
-                        for (int u = 0; u < VEC; ++u) { gx.v[u] = 0.f; gy.v[u] = 0.f; }
-                        const int xs[2] = {x0, x1}, ys[2] = {y0, y1};
-                        const float wt[4] = {w00, w01, w10, w11};
-#pragma unroll
-                        for (int tp = 0; tp < 4; ++tp) {
-                            const int xx = xs[tp & 1], yy = ys[tp >> 1];
-                            ChanVec<VEC, TF> e, wv, s, nn;
-                            e.load(img + ((size_t)yy * w + reflect_idx(xx + 1, w)) * c2 + c);
-                            wv.load(img + ((size_t)yy * w + reflect_idx(xx - 1, w)) * c2 + c);
-                            s.load(img + ((size_t)reflect_idx(yy + 1, h) * w + xx) * c2 + c);
-                            nn.load(img + ((size_t)reflect_idx(yy - 1, h) * w + xx) * c2 + c);
-#pragma unroll
-                            for (int u = 0; u < VEC; ++u) {
-                                gx.v[u] = fmaf(wt[tp], 0.5f * (e.v[u] - wv.v[u]), gx.v[u]);
-                                gy.v[u] = fmaf(wt[tp], 0.5f * (s.v[u] - nn.v[u]), gy.v[u]);
-                            }
-                        }
-                    }
-                    ChanVec<VEC> ra;
-                    ra.load_smem(myRb + c);
-#pragma unroll
-                    for (int u = 0; u < VEC; ++u) {
-                        const float f2 = w00 * a00.v[u] + w01 * a01.v[u] + w10 * a10.v[u] + w11 * a11.v[u];
-                        const float d = f1.v[u] - f2;
-                        m11 = fmaf(gx.v[u], gx.v[u], m11); m12 = fmaf(gx.v[u], gy.v[u], m12); m22 = fmaf(gy.v[u], gy.v[u], m22);
-                        q1 = fmaf(gx.v[u], d, q1); q2 = fmaf(gy.v[u], d, q2);
-                        ra.v[u] += fabsf(d);
-                    }
-                    ra.store_smem(myRb + c);
+                    tg.group<VEC>(f1, fly_grad, c, myRb, mq);
                 }
                 // point weight: scales M and q, i.e. every block of H and g; sum |diff| and nvalid stay unweighted (x * 1.0f is exact)
                 const float wn = prm.weight ? __ldg(prm.weight + (size_t)b * N + n0 + n) : 1.f;
-                m11 = warp_sum(m11) * wn; m12 = warp_sum(m12) * wn; m22 = warp_sum(m22) * wn; q1 = warp_sum(q1) * wn; q2 = warp_sum(q2) * wn;
+                mq.m11 = warp_sum(mq.m11) * wn; mq.m12 = warp_sum(mq.m12) * wn; mq.m22 = warp_sum(mq.m22) * wn; mq.q1 = warp_sum(mq.q1) * wn; mq.q2 = warp_sum(mq.q2) * wn;
             }
             if (lane == 0) {
-                rec[R_M11 * TILE_PX + n] = m11; rec[R_M12 * TILE_PX + n] = m12; rec[R_M22 * TILE_PX + n] = m22;
-                rec[R_Q1 * TILE_PX + n] = q1; rec[R_Q2 * TILE_PX + n] = q2;
+                rec[R_M11 * TILE_PX + n] = mq.m11; rec[R_M12 * TILE_PX + n] = mq.m12; rec[R_M22 * TILE_PX + n] = mq.m22;
+                rec[R_Q1 * TILE_PX + n] = mq.q1; rec[R_Q2 * TILE_PX + n] = mq.q2;
             }
         }
         __syncthreads();
@@ -337,31 +234,18 @@ lm_build_kernel(const BuildParams prm)
             float ext[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
             if (rec[R_MASK * TILE_PX + n] != 0.f) {
                 const float x = rec[R_X * TILE_PX + n], y = rec[R_Y * TILE_PX + n], iZ = rec[R_IZ * TILE_PX + n];
-                const float m11 = rec[R_M11 * TILE_PX + n], m12 = rec[R_M12 * TILE_PX + n], m22 = rec[R_M22 * TILE_PX + n];
-                const float q1 = rec[R_Q1 * TILE_PX + n], q2 = rec[R_Q2 * TILE_PX + n];
+                const PointMQ mq{rec[R_M11 * TILE_PX + n], rec[R_M12 * TILE_PX + n], rec[R_M22 * TILE_PX + n], rec[R_Q1 * TILE_PX + n], rec[R_Q2 * TILE_PX + n]};
                 const float fx = sPose[12], fy = sPose[13];
-                // CameraJacobianMatrix, negated (bundlenet.py:58-60)
-                const float a0[6] = {-fx * (x * y), -fx * (-1.f - x * x), -fx * y, -fx * (-iZ), 0.f, -fx * (x * iZ)};
-                const float a1[6] = {-fy * (1.f + y * y), -fy * (-(x * y)), -fy * (-x), 0.f, -fy * (-iZ), -fy * (y * iZ)};
-                float ux[6], uy[6];
+                float a0[6], a1[6], pt[27];
+                camera_jacobian(fx, fy, x, y, iZ, a0, a1);
+                pose_terms(a0, a1, mq, pt);
 #pragma unroll
-                for (int i = 0; i < 6; ++i) { ux[i] = m11 * a0[i] + m12 * a1[i]; uy[i] = m12 * a0[i] + m22 * a1[i]; }
-                int q = 0;
-#pragma unroll
-                for (int i = 0; i < 6; ++i)
-#pragma unroll
-                    for (int jj = i; jj < 6; ++jj) { cc[q] += a0[i] * ux[jj] + a1[i] * uy[jj]; ++q; }
-#pragma unroll
-                for (int i = 0; i < 6; ++i) cc[21 + i] += a0[i] * q1 + a1[i] * q2;
+                for (int q = 0; q < 27; ++q) cc[q] += pt[q];
                 cc[27] += 1.f;
                 if constexpr (KP > 0) {
-                    const float rx = rec[R_RX * TILE_PX + n], ry = rec[R_RY * TILE_PX + n], rz = rec[R_RZ * TILE_PX + n];
-                    const float jd0 = fx * ((rx - rz * x) * iZ), jd1 = fy * ((ry - rz * y) * iZ);   // DepthJacobianMatrix :69-70
-                    const float u0 = m11 * jd0 + m12 * jd1, u1 = m12 * jd0 + m22 * jd1;
-#pragma unroll
-                    for (int i = 0; i < 6; ++i) ext[i] = a0[i] * u0 + a1[i] * u1;
-                    ext[6] = jd0 * q1 + jd1 * q2;
-                    ext[7] = jd0 * u0 + jd1 * u1;
+                    float jd0, jd1;
+                    depth_jacobian(fx, fy, rec[R_RX * TILE_PX + n], rec[R_RY * TILE_PX + n], rec[R_RZ * TILE_PX + n], x, y, iZ, jd0, jd1);
+                    depth_terms(a0, a1, jd0, jd1, mq, ext);
                 }
             }
             if constexpr (KP > 0) {
@@ -414,22 +298,9 @@ lm_reduce_kernel(const BuildParams prm, int grid_build, float* __restrict__ H, f
     const int b = blockIdx.y, K = prm.K, C = prm.C, P = 6 + K;
     const SlotLayout L{K, C};
     const long long p0 = (long long)b * prm.tiles_per_pair, p1 = p0 + prm.tiles_per_pair;
-    // slots that hold a partial of pair b: one per CTA whose tile range intersects [p0,p1) (a contiguous CTA range)
-    __shared__ const float* s_slot[2 * kMaxSMs + 8];        // a pair can be spread over the whole grid (<= 2 CTAs per SM)
+    __shared__ const float* s_slot[kMaxSlots];
     __shared__ int s_n;
-    if (threadIdx.x == 0) {
-        int c0 = (int)((p0 * grid_build) / prm.total_tiles);
-        while (c0 + 1 < grid_build && part_begin(prm.total_tiles, grid_build, c0 + 1) <= p0) ++c0;
-        int n = 0;
-        for (int c = c0; c < grid_build && n < 2 * kMaxSMs + 8; ++c) {
-            const long long tb = part_begin(prm.total_tiles, grid_build, c), te = part_begin(prm.total_tiles, grid_build, c + 1);
-            if (tb >= p1) break;
-            if (tb >= te || te <= p0) continue;
-            const int span = b - (int)(tb / prm.tiles_per_pair);
-            s_slot[n++] = prm.partials + ((size_t)c * prm.max_span + span) * prm.slot_floats;
-        }
-        s_n = n;
-    }
+    if (threadIdx.x == 0) s_n = find_slots(prm, grid_build, prm.tiles_per_pair, b, p0, p1, s_slot);
     __syncthreads();
     const int nslot = s_n;
     const int nel = L.off_rbar() + C;
@@ -475,16 +346,6 @@ int launch_lm_reduce(const BuildParams& prm, int grid_build, float* H, float* g,
 }
 
 // ---- host side ------------------------------------------------------------------------------------
-static int padded_K(int K) {
-    if (K == 0) return 0;
-    if (K <= 16) return 16;
-    if (K <= 32) return 32;
-    if (K <= 64) return 64;
-    if (K <= 128) return 128;
-    if (K <= 256) return 256;
-    return -1;
-}
-
 int build_plan(const banet_level_t* lv, int num_sms, BuildPlan* plan)
 {
     const int KP = padded_K(lv->K);

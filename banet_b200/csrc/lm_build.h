@@ -33,6 +33,16 @@ struct BuildPlan {
 int num_sms();
 
 // fp32 SIMT path (lm_build.cu)
+// padded basis width of the fp32 SIMT kernels: 0 without a basis, -1 for K > 256 (not supported)
+static inline int padded_K(int K) {
+    if (K == 0) return 0;
+    if (K <= 16) return 16;
+    if (K <= 32) return 32;
+    if (K <= 64) return 64;
+    if (K <= 128) return 128;
+    if (K <= 256) return 256;
+    return -1;
+}
 int build_plan(const banet_level_t* lv, int num_sms, BuildPlan* plan);
 int lm_build_simt(const banet_level_t* lv, const BuildPlan& plan, const float* R, const float* T, const float* W,
                   float* H, float* g, float* rbar_sum, float* nvalid, void* ws, cudaStream_t st);

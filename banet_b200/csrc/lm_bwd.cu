@@ -22,6 +22,7 @@
 #include "lm_build.h"
 #include "lm_step.cuh"
 #include "pose_bwd.cuh"
+#include "point.cuh"
 
 namespace banet {
 
@@ -44,52 +45,12 @@ struct BwdParams {
     long long total_tiles;
 };
 
-__device__ __forceinline__ float sgnf(float v) { return v > 0.f ? 1.f : (v < 0.f ? -1.f : 0.f); }
-__device__ __forceinline__ int reflect1(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }     // tf.pad REFLECT by one
-
 // conv2 layouts of the build backward.  F2-only: the gradient channels are the forward's on-the-fly stencil at each tap,
 //   gx_tau = 1/2 (F[y, rho(x+1)] - F[y, rho(x-1)]),  gy_tau = 1/2 (F[rho(y+1), x] - F[rho(y-1), x]),
 // so its adjoint scatters w_tau df into the tap and +-1/2 w_tau dgx, +-1/2 w_tau dgy into the tap's four stencil neighbours (20 addresses;
 // the atomics keep texels that the reflect and the clamp make coincide correct).  Summing an interior point's 20 contributions into its 12
 // distinct texels first (12 atomics) was slower on an H100 at every measured size (DESIGN.md §4), so every point takes the plain scatter.
 constexpr int BWD_3C = 0, BWD_F2 = 1;
-
-// Pixel coordinates of the four taps (bit 0: x0 / x1, bit 1: y0 / y1) and of their stencil neighbours in an F2-only map.
-struct FlyTaps {
-    int cx[2], ex[2], wx[2], cy[2], sy[2], ny[2];
-    __device__ __forceinline__ FlyTaps(int x0, int x1, int y0, int y1, int h, int w) {
-        cx[0] = x0; cx[1] = x1; cy[0] = y0; cy[1] = y1;
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            ex[i] = reflect1(cx[i] + 1, w); wx[i] = reflect1(cx[i] - 1, w);
-            sy[i] = reflect1(cy[i] + 1, h); ny[i] = reflect1(cy[i] - 1, h);
-        }
-    }
-    // channel c of the tap values t, the tap x-gradients g and y-gradients k
-    template <typename TF>
-    __device__ __forceinline__ void load(const TF* img, int w, int C, int c, float t[4], float g[4], float k[4]) const {
-#pragma unroll
-        for (int tp = 0; tp < 4; ++tp) {
-            const int xx = cx[tp & 1];
-            const size_t row = (size_t)cy[tp >> 1] * w;
-            t[tp] = ldg_feat(img + (row + xx) * C + c);
-            g[tp] = 0.5f * (ldg_feat(img + (row + ex[tp & 1]) * C + c) - ldg_feat(img + (row + wx[tp & 1]) * C + c));
-            k[tp] = 0.5f * (ldg_feat(img + ((size_t)sy[tp >> 1] * w + xx) * C + c) - ldg_feat(img + ((size_t)ny[tp >> 1] * w + xx) * C + c));
-        }
-    }
-    // the adjoint of load for one channel: df on the values, dgx / dgy on the gradients, each tap weighted by wt
-    __device__ __forceinline__ void scatter(float* dimg, int w, int C, int c, const float wt[4], float df, float dgx, float dgy) const {
-#pragma unroll
-        for (int tp = 0; tp < 4; ++tp) {
-            const int xx = cx[tp & 1];
-            const size_t row = (size_t)cy[tp >> 1] * w;
-            const float hx = 0.5f * wt[tp] * dgx, hy = 0.5f * wt[tp] * dgy;
-            atomicAdd(dimg + (row + xx) * C + c, wt[tp] * df);
-            atomicAdd(dimg + (row + ex[tp & 1]) * C + c, hx); atomicAdd(dimg + (row + wx[tp & 1]) * C + c, -hx);
-            atomicAdd(dimg + ((size_t)sy[tp >> 1] * w + xx) * C + c, hy); atomicAdd(dimg + ((size_t)ny[tp >> 1] * w + xx) * C + c, -hy);
-        }
-    }
-};
 
 // smem layout (floats): S_dd [K][K] | S_cd [6][K] | S_dc [K][6] | S_cc [36] | ghat [P] | W [K] | pose [16] | rhat [C]
 // TF: feature element type (float or bf16, widened on load); dconv1 / dconv2 are fp32 for both.  TB: the same for the basis; dB is fp32.
@@ -161,7 +122,7 @@ lm_build_bwd_kernel(const BwdParams prm)
             __syncthreads();
             cur_b = b;
         }
-        const float fx = sPose[12], fy = sPose[13], ox = sPose[14], oy = sPose[15];
+        const float fx = sPose[12], fy = sPose[13];
         const TF* img = static_cast<const TF*>(prm.conv2) + (size_t)b * h * w * C3;
         float* dimg = prm.dconv2 + (size_t)b * h * w * C3;
 
@@ -181,51 +142,23 @@ lm_build_bwd_kernel(const BwdParams prm)
             const float* pp = prm.p + (size_t)b * 3 * N + n;
             const float p0 = __ldg(pp), p1 = __ldg(pp + N), p2 = __ldg(pp + 2 * (size_t)N);
             const float Dt = __ldg(prm.D + gi) + bw;                                     // bundlenet.py:208
-            const float rx = sPose[0] * p0 + sPose[1] * p1 + sPose[2] * p2;
-            const float ry = sPose[3] * p0 + sPose[4] * p1 + sPose[5] * p2;
-            const float rz = sPose[6] * p0 + sPose[7] * p1 + sPose[8] * p2;
-            const float X = rx * Dt + sPose[9], Y = ry * Dt + sPose[10], Z = rz * Dt + sPose[11];
-            const float x = X / Z, y = Y / Z, iZ = 1.0f / Z;
-            const float u = fx * x + ox, v = fy * y + oy;
-            const bool ok = (u >= 0.f) && (u <= (float)(w - 1)) && (v >= 0.f) && (v <= (float)(h - 1)) && isfinite(iZ);
+            const Projection pr(sPose, p0, p1, p2, Dt);
             float* dc1 = prm.dconv1 + gi * C;
-            if (!ok) {                                   // masked pixel: no gradient at all (mask is piecewise constant)
+            if (!pr.in_bounds(h, w)) {                   // masked pixel: no gradient at all (mask is piecewise constant)
                 for (int c = lane; c < C; c += 32) dc1[c] = 0.f;
 #pragma unroll
                 for (int i = 0; i < BWD_KL; ++i) { const int k = lane + 32 * i; if (k < K) prm.dB[gi * K + k] = 0.f; }
                 if (lane == 0) { prm.dD[gi] = 0.f; if (prm.dweight) prm.dweight[gi] = 0.f; }
                 continue;
             }
-            const float fu = floorf(u), fv = floorf(v);
-            const int x0 = (int)fu, y0 = (int)fv, x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
-            const float dx = u - fu, dy = v - fv;
-            const float w00 = (1.f - dx) * (1.f - dy), w01 = dx * (1.f - dy), w10 = (1.f - dx) * dy, w11 = dx * dy;
-            const size_t o00 = ((size_t)y0 * w + x0) * C3, o01 = ((size_t)y0 * w + x1) * C3, o10 = ((size_t)y1 * w + x0) * C3, o11 = ((size_t)y1 * w + x1) * C3;
+            const Taps tp = taps_at(pr.u, pr.v, h, w);
             const TF* c1 = static_cast<const TF*>(prm.conv1) + gi * C;
             // ---- pass 1: M = G^T G, q = G^T d (lanes over channels) ----------------------------------------------------------------
-            float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f;
-            for (int c = lane; c < C; c += 32) {
-                float f2, gx, gy;
-                if constexpr (FLY) {
-                    const FlyTaps fly(x0, x1, y0, y1, h, w);
-                    float t[4], g[4], k[4];
-                    fly.load(img, w, C, c, t, g, k);
-                    f2 = w00 * t[0] + w01 * t[1] + w10 * t[2] + w11 * t[3];
-                    gx = w00 * g[0] + w01 * g[1] + w10 * g[2] + w11 * g[3];
-                    gy = w00 * k[0] + w01 * k[1] + w10 * k[2] + w11 * k[3];
-                } else {
-                    f2 = w00 * ldg_feat(img + o00 + c) + w01 * ldg_feat(img + o01 + c) + w10 * ldg_feat(img + o10 + c) + w11 * ldg_feat(img + o11 + c);
-                    gx = w00 * ldg_feat(img + o00 + C + c) + w01 * ldg_feat(img + o01 + C + c) + w10 * ldg_feat(img + o10 + C + c) + w11 * ldg_feat(img + o11 + C + c);
-                    gy = w00 * ldg_feat(img + o00 + 2 * C + c) + w01 * ldg_feat(img + o01 + 2 * C + c) + w10 * ldg_feat(img + o10 + 2 * C + c) + w11 * ldg_feat(img + o11 + 2 * C + c);
-                }
-                const float d = ldg_feat(c1 + c) - f2;
-                m11 = fmaf(gx, gx, m11); m12 = fmaf(gx, gy, m12); m22 = fmaf(gy, gy, m22); q1 = fmaf(gx, d, q1); q2 = fmaf(gy, d, q2);
-            }
-            m11 = warp_sum(m11); m12 = warp_sum(m12); m22 = warp_sum(m22); q1 = warp_sum(q1); q2 = warp_sum(q2);
+            PointMQ mq = point_mq<FLY>(img, c1, tp, h, w, C, lane);
             // ---- Jacobians (bundlenet.py:49-74) ------------------------------------------------------------------------------------
-            const float a0[6] = {-fx * (x * y), -fx * (-1.f - x * x), -fx * y, -fx * (-iZ), 0.f, -fx * (x * iZ)};
-            const float a1[6] = {-fy * (1.f + y * y), -fy * (-(x * y)), -fy * (-x), 0.f, -fy * (-iZ), -fy * (y * iZ)};
-            const float jd0 = fx * ((rx - rz * x) * iZ), jd1 = fy * ((ry - rz * y) * iZ);
+            float a0[6], a1[6], jd0, jd1;
+            camera_jacobian(fx, fy, pr.x, pr.y, pr.iZ, a0, a1);
+            depth_jacobian(fx, fy, pr.rx, pr.ry, pr.rz, pr.x, pr.y, pr.iZ, jd0, jd1);
             // ---- K-dimensional contractions -----------------------------------------------------------------------------------------
             float e[BWD_KL];
             float alpha[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, beta[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, eta = 0.f, gamma = 0.f;
@@ -258,99 +191,34 @@ lm_build_bwd_kernel(const BwdParams prm)
 #pragma unroll
                 for (int m = 0; m < 6; ++m) { alpha[m] = warp_sum(alpha[m]); beta[m] = warp_sum(beta[m]); }
             }
-            // ---- 2 x (6+1) algebra (every lane, redundantly) --------------------------------------------------------------------------
-            float Yc0[6], Yc1[6];
-#pragma unroll
-            for (int i = 0; i < 6; ++i) {
-                float s0 = jd0 * beta[i], s1 = jd1 * beta[i];
-#pragma unroll
-                for (int m = 0; m < 6; ++m) { s0 = fmaf(a0[m], Scc[m * 6 + i], s0); s1 = fmaf(a1[m], Scc[m * 6 + i], s1); }
-                Yc0[i] = s0; Yc1[i] = s1;
-            }
-            float fb0 = 0.f, fb1 = 0.f, z0 = jd0 * eta, z1 = jd1 * eta;
-#pragma unroll
-            for (int m = 0; m < 6; ++m) { fb0 = fmaf(a0[m], alpha[m], fb0); fb1 = fmaf(a1[m], alpha[m], fb1); z0 = fmaf(a0[m], sg[m], z0); z1 = fmaf(a1[m], sg[m], z1); }
-            const float yb0 = fb0 + jd0 * gamma, yb1 = fb1 + jd1 * gamma;
-            float Q00 = yb0 * jd0, Q01 = yb0 * jd1, Q10 = yb1 * jd0, Q11 = yb1 * jd1;
-#pragma unroll
-            for (int i = 0; i < 6; ++i) { Q00 = fmaf(Yc0[i], a0[i], Q00); Q01 = fmaf(Yc0[i], a1[i], Q01); Q10 = fmaf(Yc1[i], a0[i], Q10); Q11 = fmaf(Yc1[i], a1[i], Q11); }
-            // ---- point weight: dw = <Ghat, H_n> + <ghat, g_n> = 1/2 <M, Q> + q.z (H_n = J^T M J is symmetric, so this is exact for both
-            //      S conventions).  Every adjoint that comes from Ghat, ghat is point n's times w_n: scaling M, q carries it to dJ and db,
-            //      scaling Q, z to dG and dd; the rhat sign(d) path is not weighted.  Unweighted: w_n = 1 and x * 1.0f is exact.
-            const float wn = prm.weight ? __ldg(prm.weight + gi) : 1.f;
-            if (prm.dweight && lane == 0) prm.dweight[gi] = 0.5f * (m11 * Q00 + m12 * (Q01 + Q10) + m22 * Q11) + (q1 * z0 + q2 * z1);
-            m11 *= wn; m12 *= wn; m22 *= wn; q1 *= wn; q2 *= wn;
-            Q00 *= wn; Q01 *= wn; Q10 *= wn; Q11 *= wn; z0 *= wn; z1 *= wn;
-            float dJ0[6], dJ1[6];
-#pragma unroll
-            for (int i = 0; i < 6; ++i) { dJ0[i] = m11 * Yc0[i] + m12 * Yc1[i] + q1 * sg[i]; dJ1[i] = m12 * Yc0[i] + m22 * Yc1[i] + q2 * sg[i]; }
-            const float dj0 = m11 * yb0 + m12 * yb1 + q1 * eta, dj1 = m12 * yb0 + m22 * yb1 + q2 * eta;
-            const float u0 = m11 * jd0 + m12 * jd1, u1 = m12 * jd0 + m22 * jd1;
-            const float sN = jd0 * u0 + jd1 * u1, tN = jd0 * q1 + jd1 * q2;
-            float vN[6];
-#pragma unroll
-            for (int i = 0; i < 6; ++i) vN[i] = a0[i] * u0 + a1[i] * u1;
+            // ---- 2 x (6+1) algebra (every lane, redundantly), the point weight, dJ and the depth terms of db --------------------------
+            PointAdjoint ad(a0, a1, jd0, jd1, Scc, sg, alpha, beta, eta, gamma);
+            const float dw = ad.weigh(prm.weight ? __ldg(prm.weight + gi) : 1.f, mq);
+            if (prm.dweight && lane == 0) prm.dweight[gi] = dw;
+            float dJ0[6], dJ1[6], dj0, dj1, vN[8];                 // depth terms of db: vN (6), then tN, sN
+            jacobian_adjoint(mq, ad, sg, eta, dJ0, dJ1, dj0, dj1);
+            depth_terms(a0, a1, jd0, jd1, mq, vN);
+            const float tN = vN[6], sN = vN[7];
             // ---- pass 2: dd, dG per channel -> dconv1, scatter into dconv2, coordinate gradient ------------------------------------------
-            float du = 0.f, dv = 0.f;
-            for (int c = lane; c < C; c += 32) {
-                float t00, t01, t10, t11, g00, g01, g10, g11, k00, k01, k10, k11;
-                if constexpr (FLY) {
-                    const FlyTaps fly(x0, x1, y0, y1, h, w);
-                    float t[4], g[4], k[4];
-                    fly.load(img, w, C, c, t, g, k);
-                    t00 = t[0]; t01 = t[1]; t10 = t[2]; t11 = t[3]; g00 = g[0]; g01 = g[1]; g10 = g[2]; g11 = g[3]; k00 = k[0]; k01 = k[1]; k10 = k[2]; k11 = k[3];
-                } else {
-                    t00 = ldg_feat(img + o00 + c); t01 = ldg_feat(img + o01 + c); t10 = ldg_feat(img + o10 + c); t11 = ldg_feat(img + o11 + c);
-                    g00 = ldg_feat(img + o00 + C + c); g01 = ldg_feat(img + o01 + C + c); g10 = ldg_feat(img + o10 + C + c); g11 = ldg_feat(img + o11 + C + c);
-                    k00 = ldg_feat(img + o00 + 2 * C + c); k01 = ldg_feat(img + o01 + 2 * C + c); k10 = ldg_feat(img + o10 + 2 * C + c); k11 = ldg_feat(img + o11 + 2 * C + c);
-                }
-                const float f2 = w00 * t00 + w01 * t01 + w10 * t10 + w11 * t11;
-                const float gx = w00 * g00 + w01 * g01 + w10 * g10 + w11 * g11;
-                const float gy = w00 * k00 + w01 * k01 + w10 * k10 + w11 * k11;
-                const float d = ldg_feat(c1 + c) - f2;
-                const float dd = gx * z0 + gy * z1 + sRh[c] * sgnf(d);
-                const float dgx = gx * Q00 + gy * Q10 + d * z0, dgy = gx * Q01 + gy * Q11 + d * z1;
-                dc1[c] = dd;
-                const float df = -dd;
-                if constexpr (FLY) {
-                    const float wt[4] = {w00, w01, w10, w11};
-                    const FlyTaps fly(x0, x1, y0, y1, h, w);
-                    fly.scatter(dimg, w, C, c, wt, df, dgx, dgy);
-                } else {
-                    atomicAdd(dimg + o00 + c, w00 * df); atomicAdd(dimg + o01 + c, w01 * df); atomicAdd(dimg + o10 + c, w10 * df); atomicAdd(dimg + o11 + c, w11 * df);
-                    atomicAdd(dimg + o00 + C + c, w00 * dgx); atomicAdd(dimg + o01 + C + c, w01 * dgx); atomicAdd(dimg + o10 + C + c, w10 * dgx); atomicAdd(dimg + o11 + C + c, w11 * dgx);
-                    atomicAdd(dimg + o00 + 2 * C + c, w00 * dgy); atomicAdd(dimg + o01 + 2 * C + c, w01 * dgy); atomicAdd(dimg + o10 + 2 * C + c, w10 * dgy); atomicAdd(dimg + o11 + 2 * C + c, w11 * dgy);
-                }
-                du += df * ((1.f - dy) * (t01 - t00) + dy * (t11 - t10)) + dgx * ((1.f - dy) * (g01 - g00) + dy * (g11 - g10)) + dgy * ((1.f - dy) * (k01 - k00) + dy * (k11 - k10));
-                dv += df * ((1.f - dx) * (t10 - t00) + dx * (t11 - t01)) + dgx * ((1.f - dx) * (g10 - g00) + dx * (g11 - g01)) + dgy * ((1.f - dx) * (k10 - k00) + dx * (k11 - k01));
-            }
-            du = warp_sum(du); dv = warp_sum(dv);
+            float du, dv;
+            channel_adjoint<FLY>(img, dimg, c1, sRh, tp, h, w, C, lane, ad, [&](int c, float dd) { dc1[c] = dd; }, du, dv);
             // ---- geometry backward ----------------------------------------------------------------------------------------------------
-            float gxx = fx * du, gyy = fy * dv, giZ = 0.f;                      // u = fx x + ox, v = fy y + oy
-            gxx += -fx * (dJ0[0] * y - 2.f * x * dJ0[1] + dJ0[5] * iZ) - fy * (-dJ1[1] * y - dJ1[2]);
-            gyy += -fx * (dJ0[0] * x + dJ0[2]) - fy * (2.f * y * dJ1[0] - dJ1[1] * x + dJ1[5] * iZ);
-            giZ += -fx * (-dJ0[3] + dJ0[5] * x) - fy * (-dJ1[4] + dJ1[5] * y);
-            float grx = dj0 * fx * iZ, gry = dj1 * fy * iZ, grz = -dj0 * fx * x * iZ - dj1 * fy * y * iZ;
-            gxx += -dj0 * fx * rz * iZ; gyy += -dj1 * fy * rz * iZ;
-            giZ += dj0 * fx * (rx - rz * x) + dj1 * fy * (ry - rz * y);
-            const float gX = gxx * iZ, gY = gyy * iZ, gZ = -iZ * (gxx * x + gyy * y) - iZ * iZ * giZ;
-            const float gDt = rx * gX + ry * gY + rz * gZ;
-            grx += Dt * gX; gry += Dt * gY; grz += Dt * gZ;
-            accT[0] += gX; accT[1] += gY; accT[2] += gZ;
-            accR[0] += grx * p0; accR[1] += grx * p1; accR[2] += grx * p2;
-            accR[3] += gry * p0; accR[4] += gry * p1; accR[5] += gry * p2;
-            accR[6] += grz * p0; accR[7] += grz * p1; accR[8] += grz * p2;
-            if (lane == 0) prm.dD[gi] = gDt;
+            const GeomGrad gg(pr, fx, fy, Dt, du, dv, dJ0, dJ1, dj0, dj1);
+            accT[0] += gg.gX; accT[1] += gg.gY; accT[2] += gg.gZ;
+            accR[0] += gg.grx * p0; accR[1] += gg.grx * p1; accR[2] += gg.grx * p2;
+            accR[3] += gg.gry * p0; accR[4] += gg.gry * p1; accR[5] += gg.gry * p2;
+            accR[6] += gg.grz * p0; accR[7] += gg.grz * p1; accR[8] += gg.grz * p2;
+            if (lane == 0) prm.dD[gi] = gg.gDt;
             // ---- dB row, dW ---------------------------------------------------------------------------------------------------------
 #pragma unroll
             for (int i = 0; i < BWD_KL; ++i) {
                 const int k = lane + 32 * i;
                 if (k < K) {
-                    float db = sN * e[i] + tN * sg[6 + k] + gDt * sW[k];
+                    float db = sN * e[i] + tN * sg[6 + k] + gg.gDt * sW[k];
 #pragma unroll
                     for (int m = 0; m < 6; ++m) db = fmaf(vN[m], Scd[m * K + k], db);
                     prm.dB[gi * K + k] = db;
-                    accW[i] = fmaf(gDt, bl[i], accW[i]);
+                    accW[i] = fmaf(gg.gDt, bl[i], accW[i]);
                 }
             }
         }

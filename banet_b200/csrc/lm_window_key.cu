@@ -27,10 +27,11 @@
 // its channel reduction, so every weighted quantity (H_cc, g_c, v_f, t_f, s_f and with s_f the window's depth block) follows; sum |d| and
 // nvalid stay unweighted.  The backward stores dw = 1/2 <M, Q> + q.z per (frame, point) and scales that point's adjoints by w.
 //
-// The per-point code (geometry, gather, Jacobians, the chain rule through the sampler) is that of lm_build.cu / lm_bwd.cu, restated here
-// for a keyframe given once; the existing kernels are left as they are.
+// The per-point code (geometry, gather, Jacobians, the chain rule through the sampler) is point.cuh's, shared with lm_build_kernel and
+// lm_build_bwd_kernel; this file holds what differs for a keyframe given once: the tile and frame loops, the slot layout and the commits.
 #include "common.cuh"
 #include "lm_build.h"
+#include "point.cuh"
 
 namespace banet {
 namespace {
@@ -75,28 +76,6 @@ template <int KP> struct KeySmem {
     static size_t bytes(int C) { return (size_t)(off_rb + KT_WARPS * C) * sizeof(float); }
 };
 
-template <int G> __device__ __forceinline__ void lds_g(const float* p, float* out);
-template <> __device__ __forceinline__ void lds_g<1>(const float* p, float* o) { o[0] = p[0]; }
-template <> __device__ __forceinline__ void lds_g<2>(const float* p, float* o) { float2 v = *reinterpret_cast<const float2*>(p); o[0] = v.x; o[1] = v.y; }
-template <> __device__ __forceinline__ void lds_g<4>(const float* p, float* o) {
-    float4 v = *reinterpret_cast<const float4*>(p); o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w; }
-
-__device__ __forceinline__ int reflect1(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }     // tf.pad REFLECT by one
-
-template <int VEC> struct Vec;
-template <> struct Vec<4> {
-    float v[4];
-    __device__ __forceinline__ void load(const float* p) { float4 t = __ldg(reinterpret_cast<const float4*>(p)); v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w; }
-    __device__ __forceinline__ void load_smem(const float* p) { float4 t = *reinterpret_cast<const float4*>(p); v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w; }
-    __device__ __forceinline__ void store_smem(float* p) const { *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]); }
-};
-template <> struct Vec<1> {
-    float v[1];
-    __device__ __forceinline__ void load(const float* p) { v[0] = __ldg(p); }
-    __device__ __forceinline__ void load_smem(const float* p) { v[0] = p[0]; }
-    __device__ __forceinline__ void store_smem(float* p) const { p[0] = v[0]; }
-};
-
 template <int KP, int VEC>
 __global__ void __launch_bounds__(KT_THREADS, (KP >= 128) ? 1 : 2)
 keyframe_build_kernel(const KeyParams prm)
@@ -113,7 +92,7 @@ keyframe_build_kernel(const KeyParams prm)
     constexpr int LDB = SM::LDB;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int N = prm.N, C = prm.C, K = prm.K, h = prm.h, w = prm.w, c2 = prm.c2, nf = prm.nf;
-    const bool fly_grad = (c2 == C);
+    const bool fly = (c2 == C);
 
     // register tile of H_dd as in lm_build_kernel (K > 128: one 128 x 128 block of its lower triangle per launch)
     constexpr int KB = (KP > 128) ? 128 : KP;
@@ -187,15 +166,7 @@ keyframe_build_kernel(const KeyParams prm)
                 const float* pp = prm.p + (size_t)wi * 3 * N + n0 + n;
                 p0 = pp[0]; p1 = pp[N]; p2 = pp[2 * (size_t)N];
                 Dt = prm.D[(size_t)wi * N + n0 + n];
-                float d0 = 0.f, d1 = 0.f, d2 = 0.f, d3 = 0.f;
-#pragma unroll 4
-                for (int k = 0; k < KP; k += 4) {
-                    const float4 bv = *reinterpret_cast<const float4*>(Bs + n * LDB + k);
-                    const float4 wv = *reinterpret_cast<const float4*>(sW + k);
-                    d0 = fmaf(bv.x, wv.x, d0); d1 = fmaf(bv.y, wv.y, d1);
-                    d2 = fmaf(bv.z, wv.z, d2); d3 = fmaf(bv.w, wv.w, d3);
-                }
-                Dt += (d0 + d1) + (d2 + d3);
+                Dt += basis_dot<KP>(Bs + n * LDB, sW);
             }
             rec[R_P0 * KT_PX + n] = p0; rec[R_P1 * KT_PX + n] = p1; rec[R_P2 * KT_PX + n] = p2; rec[R_DT * KT_PX + n] = Dt;
             rec[R_SSUM * KT_PX + n] = 0.f; rec[R_ANY * KT_PX + n] = 0.f;
@@ -218,17 +189,11 @@ keyframe_build_kernel(const KeyParams prm)
                 int x0 = 0, y0 = 0;
                 if (n < cnt) {
                     const float p0 = rec[R_P0 * KT_PX + n], p1 = rec[R_P1 * KT_PX + n], p2 = rec[R_P2 * KT_PX + n], Dt = rec[R_DT * KT_PX + n];
-                    rx = sPose[0] * p0 + sPose[1] * p1 + sPose[2] * p2;
-                    ry = sPose[3] * p0 + sPose[4] * p1 + sPose[5] * p2;
-                    rz = sPose[6] * p0 + sPose[7] * p1 + sPose[8] * p2;
-                    const float X = rx * Dt + sPose[9], Y = ry * Dt + sPose[10], Z = rz * Dt + sPose[11];
-                    x = X / Z; y = Y / Z; iZ = 1.0f / Z;
-                    const float u = sPose[12] * x + sPose[14], v = sPose[13] * y + sPose[15];
-                    const bool ok = (u >= 0.f) && (u <= (float)(w - 1)) && (v >= 0.f) && (v <= (float)(h - 1)) && isfinite(iZ);
-                    if (ok) {
+                    const Projection pr(sPose, p0, p1, p2, Dt);
+                    rx = pr.rx; ry = pr.ry; rz = pr.rz; x = pr.x; y = pr.y; iZ = pr.iZ;
+                    if (pr.in_bounds(h, w)) {
                         mask = 1.f;
-                        const float fu = floorf(u), fv = floorf(v);
-                        x0 = (int)fu; y0 = (int)fv; dx = u - fu; dy = v - fv;
+                        tap_corner(pr.u, pr.v, x0, y0, dx, dy);
                     }
                 }
                 rec[R_X0 * KT_PX + n] = __int_as_float(x0); rec[R_Y0 * KT_PX + n] = __int_as_float(y0);
@@ -240,73 +205,26 @@ keyframe_build_kernel(const KeyParams prm)
             // S2: feature gather, warp per point, lanes over channels (bundlenet.py:230-239)
             for (int i = 0; i < KT_PX / KT_WARPS; ++i) {
                 const int n = i * KT_WARPS + warp;
-                float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f;
+                PointMQ mq{0.f, 0.f, 0.f, 0.f, 0.f};
                 const bool valid = rec[R_MASK * KT_PX + n] != 0.f;
                 if (valid) {
-                    const int x0 = __float_as_int(rec[R_X0 * KT_PX + n]), y0 = __float_as_int(rec[R_Y0 * KT_PX + n]);
-                    const float dx = rec[R_DX * KT_PX + n], dy = rec[R_DY * KT_PX + n];
-                    const int x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
-                    const float w00 = (1.f - dx) * (1.f - dy), w01 = dx * (1.f - dy), w10 = (1.f - dx) * dy, w11 = dx * dy;
-                    const float* img = prm.conv2 + (size_t)b * h * w * c2;
-                    const float* t00 = img + ((size_t)y0 * w + x0) * c2;
-                    const float* t01 = img + ((size_t)y0 * w + x1) * c2;
-                    const float* t10 = img + ((size_t)y1 * w + x0) * c2;
-                    const float* t11 = img + ((size_t)y1 * w + x1) * c2;
+                    const Taps tp(__float_as_int(rec[R_X0 * KT_PX + n]), __float_as_int(rec[R_Y0 * KT_PX + n]), rec[R_DX * KT_PX + n], rec[R_DY * KT_PX + n], h, w);
+                    const TapGather<float> tg(prm.conv2 + (size_t)b * h * w * c2, tp, h, w, C, c2);
                     const float* c1 = prm.conv1 + ((size_t)wi * N + n0 + n) * C;      // the keyframe's features, re-read by every frame (L1 / L2)
                     float* myRb = sRb + warp * C;
                     for (int c = lane * VEC; c < C; c += 32 * VEC) {
-                        Vec<VEC> f1, a00, a01, a10, a11, gx, gy;
+                        ChanVec<VEC> f1;
                         f1.load(c1 + c);
-                        a00.load(t00 + c); a01.load(t01 + c); a10.load(t10 + c); a11.load(t11 + c);
-                        if (!fly_grad) {
-                            Vec<VEC> g00, g01, g10, g11;
-                            g00.load(t00 + C + c); g01.load(t01 + C + c); g10.load(t10 + C + c); g11.load(t11 + C + c);
-#pragma unroll
-                            for (int u = 0; u < VEC; ++u) gx.v[u] = w00 * g00.v[u] + w01 * g01.v[u] + w10 * g10.v[u] + w11 * g11.v[u];
-                            g00.load(t00 + 2 * C + c); g01.load(t01 + 2 * C + c); g10.load(t10 + 2 * C + c); g11.load(t11 + 2 * C + c);
-#pragma unroll
-                            for (int u = 0; u < VEC; ++u) gy.v[u] = w00 * g00.v[u] + w01 * g01.v[u] + w10 * g10.v[u] + w11 * g11.v[u];
-                        } else {
-                            // F2-only map: central differences with REFLECT-by-one borders (bundlenet.py:92-100) at each tap
-#pragma unroll
-                            for (int u = 0; u < VEC; ++u) { gx.v[u] = 0.f; gy.v[u] = 0.f; }
-                            const int xs[2] = {x0, x1}, ys[2] = {y0, y1};
-                            const float wt[4] = {w00, w01, w10, w11};
-#pragma unroll
-                            for (int tp = 0; tp < 4; ++tp) {
-                                const int xx = xs[tp & 1], yy = ys[tp >> 1];
-                                Vec<VEC> e, wv, s, nn;
-                                e.load(img + ((size_t)yy * w + reflect1(xx + 1, w)) * c2 + c);
-                                wv.load(img + ((size_t)yy * w + reflect1(xx - 1, w)) * c2 + c);
-                                s.load(img + ((size_t)reflect1(yy + 1, h) * w + xx) * c2 + c);
-                                nn.load(img + ((size_t)reflect1(yy - 1, h) * w + xx) * c2 + c);
-#pragma unroll
-                                for (int u = 0; u < VEC; ++u) {
-                                    gx.v[u] = fmaf(wt[tp], 0.5f * (e.v[u] - wv.v[u]), gx.v[u]);
-                                    gy.v[u] = fmaf(wt[tp], 0.5f * (s.v[u] - nn.v[u]), gy.v[u]);
-                                }
-                            }
-                        }
-                        Vec<VEC> ra;
-                        ra.load_smem(myRb + c);
-#pragma unroll
-                        for (int u = 0; u < VEC; ++u) {
-                            const float f2 = w00 * a00.v[u] + w01 * a01.v[u] + w10 * a10.v[u] + w11 * a11.v[u];
-                            const float d = f1.v[u] - f2;
-                            m11 = fmaf(gx.v[u], gx.v[u], m11); m12 = fmaf(gx.v[u], gy.v[u], m12); m22 = fmaf(gy.v[u], gy.v[u], m22);
-                            q1 = fmaf(gx.v[u], d, q1); q2 = fmaf(gy.v[u], d, q2);
-                            ra.v[u] += fabsf(d);
-                        }
-                        ra.store_smem(myRb + c);
+                        tg.group<VEC>(f1, fly, c, myRb, mq);
                     }
-                    m11 = warp_sum(m11); m12 = warp_sum(m12); m22 = warp_sum(m22); q1 = warp_sum(q1); q2 = warp_sum(q2);
+                    mq.m11 = warp_sum(mq.m11); mq.m12 = warp_sum(mq.m12); mq.m22 = warp_sum(mq.m22); mq.q1 = warp_sum(mq.q1); mq.q2 = warp_sum(mq.q2);
                 }
                 if (lane == 0) {
                     // point weight of (frame f, point n): scales M and q, and through them every weighted quantity of S3 (H_cc, g_c, v_f,
                     // t_f, s_f); sum |d|, nvalid and R_ANY stay unweighted.  Unweighted: x * 1.0f is exact
                     const float wn = (prm.weight && valid) ? __ldg(prm.weight + (size_t)b * N + n0 + n) : 1.f;
-                    rec[R_M11 * KT_PX + n] = m11 * wn; rec[R_M12 * KT_PX + n] = m12 * wn; rec[R_M22 * KT_PX + n] = m22 * wn;
-                    rec[R_Q1 * KT_PX + n] = q1 * wn; rec[R_Q2 * KT_PX + n] = q2 * wn;
+                    rec[R_M11 * KT_PX + n] = mq.m11 * wn; rec[R_M12 * KT_PX + n] = mq.m12 * wn; rec[R_M22 * KT_PX + n] = mq.m22 * wn;
+                    rec[R_Q1 * KT_PX + n] = mq.q1 * wn; rec[R_Q2 * KT_PX + n] = mq.q2 * wn;
                 }
             }
             __syncthreads();
@@ -319,29 +237,14 @@ keyframe_build_kernel(const KeyParams prm)
                 for (int q = 0; q < 28; ++q) cc[q] = 0.f;
                 if (rec[R_MASK * KT_PX + n] != 0.f) {
                     const float x = rec[R_X * KT_PX + n], y = rec[R_Y * KT_PX + n], iZ = rec[R_IZ * KT_PX + n];
-                    const float m11 = rec[R_M11 * KT_PX + n], m12 = rec[R_M12 * KT_PX + n], m22 = rec[R_M22 * KT_PX + n];
-                    const float q1 = rec[R_Q1 * KT_PX + n], q2 = rec[R_Q2 * KT_PX + n];
+                    const PointMQ mq{rec[R_M11 * KT_PX + n], rec[R_M12 * KT_PX + n], rec[R_M22 * KT_PX + n], rec[R_Q1 * KT_PX + n], rec[R_Q2 * KT_PX + n]};
                     const float fx = sPose[12], fy = sPose[13];
-                    const float a0[6] = {-fx * (x * y), -fx * (-1.f - x * x), -fx * y, -fx * (-iZ), 0.f, -fx * (x * iZ)};
-                    const float a1[6] = {-fy * (1.f + y * y), -fy * (-(x * y)), -fy * (-x), 0.f, -fy * (-iZ), -fy * (y * iZ)};
-                    float ux[6], uy[6];
-#pragma unroll
-                    for (int i = 0; i < 6; ++i) { ux[i] = m11 * a0[i] + m12 * a1[i]; uy[i] = m12 * a0[i] + m22 * a1[i]; }
-                    int q = 0;
-#pragma unroll
-                    for (int i = 0; i < 6; ++i)
-#pragma unroll
-                        for (int jj = i; jj < 6; ++jj) { cc[q] = a0[i] * ux[jj] + a1[i] * uy[jj]; ++q; }
-#pragma unroll
-                    for (int i = 0; i < 6; ++i) cc[21 + i] = a0[i] * q1 + a1[i] * q2;
+                    float a0[6], a1[6], jd0, jd1;
+                    camera_jacobian(fx, fy, x, y, iZ, a0, a1);
+                    pose_terms(a0, a1, mq, cc);
                     cc[27] = 1.f;
-                    const float rx = rec[R_RX * KT_PX + n], ry = rec[R_RY * KT_PX + n], rz = rec[R_RZ * KT_PX + n];
-                    const float jd0 = fx * ((rx - rz * x) * iZ), jd1 = fy * ((ry - rz * y) * iZ);    // DepthJacobianMatrix :69-70
-                    const float u0 = m11 * jd0 + m12 * jd1, u1 = m12 * jd0 + m22 * jd1;
-#pragma unroll
-                    for (int i = 0; i < 6; ++i) ext[i] = a0[i] * u0 + a1[i] * u1;
-                    ext[6] = jd0 * q1 + jd1 * q2;
-                    ext[7] = jd0 * u0 + jd1 * u1;
+                    depth_jacobian(fx, fy, rec[R_RX * KT_PX + n], rec[R_RY * KT_PX + n], rec[R_RZ * KT_PX + n], x, y, iZ, jd0, jd1);
+                    depth_terms(a0, a1, jd0, jd1, mq, ext);
                     rec[R_SSUM * KT_PX + n] += ext[7];
                     rec[R_ANY * KT_PX + n] = 1.f;
                 }
@@ -397,8 +300,8 @@ keyframe_build_kernel(const KeyParams prm)
             float a[T], cv[T];
 #pragma unroll
             for (int gq = 0; gq < NG; ++gq) {
-                lds_g<G>(Bs + n * LDB + ki0 + gq * 16 * G + G * ti, a + gq * G);
-                lds_g<G>(Bs + n * LDB + kj0 + gq * 16 * G + G * tj, cv + gq * G);
+                lds_group<G>(Bs + n * LDB + ki0 + gq * 16 * G + G * ti, a + gq * G);
+                lds_group<G>(Bs + n * LDB + kj0 + gq * 16 * G + G * tj, cv + gq * G);
             }
 #pragma unroll
             for (int e = 0; e < T; ++e) {
@@ -420,22 +323,9 @@ keyframe_reduce_kernel(const KeyParams prm, int grid_build, float* __restrict__ 
     const int wi = blockIdx.y, K = prm.K, C = prm.C, nf = prm.nf, P = 6 + K;
     const KeySlot L{K, C};
     const long long p0 = (long long)wi * prm.tiles_per_win, p1 = p0 + prm.tiles_per_win;
-    __shared__ const float* s_slot[2 * kMaxSMs + 8];
+    __shared__ const float* s_slot[kMaxSlots];
     __shared__ int s_n;
-    if (threadIdx.x == 0) {
-        int c0 = (int)((p0 * grid_build) / prm.total_tiles);
-        while (c0 + 1 < grid_build && part_begin(prm.total_tiles, grid_build, c0 + 1) <= p0) ++c0;
-        while (c0 > 0 && part_begin(prm.total_tiles, grid_build, c0) > p0) --c0;
-        int n = 0;
-        for (int c = c0; c < grid_build && n < 2 * kMaxSMs + 8; ++c) {
-            const long long tb = part_begin(prm.total_tiles, grid_build, c), te = part_begin(prm.total_tiles, grid_build, c + 1);
-            if (tb >= p1) break;
-            if (tb >= te || te <= p0) continue;
-            const int span = wi - (int)(tb / prm.tiles_per_win);
-            s_slot[n++] = prm.partials + ((size_t)c * prm.max_span + span) * prm.slot_floats;
-        }
-        s_n = n;
-    }
+    if (threadIdx.x == 0) s_n = find_slots(prm, grid_build, prm.tiles_per_win, wi, p0, p1, s_slot);
     __syncthreads();
     const int nslot = s_n;
     const int FF = 7 * K + 28 + C;                                    // used floats of a frame's part of the slot
@@ -483,8 +373,6 @@ keyframe_reduce_kernel(const KeyParams prm, int grid_build, float* __restrict__ 
     }
 }
 
-int padded_key_K(int K) { return K <= 16 ? 16 : K <= 32 ? 32 : K <= 64 ? 64 : K <= 128 ? 128 : K <= 256 ? 256 : -1; }
-
 template <int KP, int VEC>
 int launch_key_build(const KeyParams& prm, int grid, cudaStream_t st)
 {
@@ -514,8 +402,6 @@ struct KeyBwdParams {
     int exact_sym, nfc, tiles_per_win;
     long long total_tiles;
 };
-
-__device__ __forceinline__ float sgn(float v) { return v > 0.f ? 1.f : (v < 0.f ? -1.f : 0.f); }
 
 // shared memory (floats): S_dd [K][K] | W [K] | dconv1 row per warp [KB_WARPS][C] | per frame of the chunk (nfc of them, stride key_bwd_frame_floats):
 //   S_cd [6][K] | S_dc [K][6] | S_cc [36] | ghat [P] | pose [16] | rhat [C] | dR, dT per warp [KB_WARPS][12]
@@ -629,38 +515,19 @@ keyframe_build_bwd_kernel(const KeyBwdParams prm)
                         float* Fr = sFr + fl * FS;
                         const float *Scd = Fr, *Sdc = Scd + 6 * K, *Scc = Sdc + 6 * K, *sg = Scc + 36, *sPose = sg + P, *sRh = sPose + 16;
                         float* sRT = Fr + 13 * K + 58 + C + warp * 12;
-                        const float fx = sPose[12], fy = sPose[13], ox = sPose[14], oy = sPose[15];
-                        const float rx = sPose[0] * p0 + sPose[1] * p1 + sPose[2] * p2;
-                        const float ry = sPose[3] * p0 + sPose[4] * p1 + sPose[5] * p2;
-                        const float rz = sPose[6] * p0 + sPose[7] * p1 + sPose[8] * p2;
-                        const float X = rx * Dt + sPose[9], Y = ry * Dt + sPose[10], Z = rz * Dt + sPose[11];
-                        const float x = X / Z, y = Y / Z, iZ = 1.0f / Z;
-                        const float u = fx * x + ox, v = fy * y + oy;
-                        const bool ok = (u >= 0.f) && (u <= (float)(w - 1)) && (v >= 0.f) && (v <= (float)(h - 1)) && isfinite(iZ);
-                        if (!ok) {                                           // masked in this frame: no gradient through it
+                        const float fx = sPose[12], fy = sPose[13];
+                        const Projection pr(sPose, p0, p1, p2, Dt);
+                        if (!pr.in_bounds(h, w)) {                           // masked in this frame: no gradient through it
                             if (prm.dweight && lane == 0) prm.dweight[b * N + n] = 0.f;
                             continue;
                         }
-                        const float fu = floorf(u), fv = floorf(v);
-                        const int x0 = (int)fu, y0 = (int)fv, x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
-                        const float dx = u - fu, dy = v - fv;
-                        const float w00 = (1.f - dx) * (1.f - dy), w01 = dx * (1.f - dy), w10 = (1.f - dx) * dy, w11 = dx * dy;
+                        const Taps tp = taps_at(pr.u, pr.v, h, w);
                         const float* img = prm.conv2 + b * h * w * C3;
                         float* dimg = prm.dconv2 + b * h * w * C3;
-                        const size_t o00 = ((size_t)y0 * w + x0) * C3, o01 = ((size_t)y0 * w + x1) * C3, o10 = ((size_t)y1 * w + x0) * C3, o11 = ((size_t)y1 * w + x1) * C3;
-                        // pass 1: M = G^T G, q = G^T d
-                        float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f;
-                        for (int c = lane; c < C; c += 32) {
-                            const float f2 = w00 * __ldg(img + o00 + c) + w01 * __ldg(img + o01 + c) + w10 * __ldg(img + o10 + c) + w11 * __ldg(img + o11 + c);
-                            const float gx = w00 * __ldg(img + o00 + C + c) + w01 * __ldg(img + o01 + C + c) + w10 * __ldg(img + o10 + C + c) + w11 * __ldg(img + o11 + C + c);
-                            const float gy = w00 * __ldg(img + o00 + 2 * C + c) + w01 * __ldg(img + o01 + 2 * C + c) + w10 * __ldg(img + o10 + 2 * C + c) + w11 * __ldg(img + o11 + 2 * C + c);
-                            const float d = __ldg(c1 + c) - f2;
-                            m11 = fmaf(gx, gx, m11); m12 = fmaf(gx, gy, m12); m22 = fmaf(gy, gy, m22); q1 = fmaf(gx, d, q1); q2 = fmaf(gy, d, q2);
-                        }
-                        m11 = warp_sum(m11); m12 = warp_sum(m12); m22 = warp_sum(m22); q1 = warp_sum(q1); q2 = warp_sum(q2);
-                        const float a0[6] = {-fx * (x * y), -fx * (-1.f - x * x), -fx * y, -fx * (-iZ), 0.f, -fx * (x * iZ)};
-                        const float a1[6] = {-fy * (1.f + y * y), -fy * (-(x * y)), -fy * (-x), 0.f, -fy * (-iZ), -fy * (y * iZ)};
-                        const float jd0 = fx * ((rx - rz * x) * iZ), jd1 = fy * ((ry - rz * y) * iZ);
+                        PointMQ mq = point_mq<false>(img, c1, tp, h, w, C, lane);              // pass 1: M = G^T G, q = G^T d
+                        float a0[6], a1[6], jd0, jd1;
+                        camera_jacobian(fx, fy, pr.x, pr.y, pr.iZ, a0, a1);
+                        depth_jacobian(fx, fy, pr.rx, pr.ry, pr.rz, pr.x, pr.y, pr.iZ, jd0, jd1);
                         // O(K) contractions with this frame's S_cd, S_dc, ghat_d
                         float alpha[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, beta[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, eta = 0.f;
 #pragma unroll
@@ -675,87 +542,36 @@ keyframe_build_bwd_kernel(const KeyBwdParams prm)
                         eta = warp_sum(eta);
 #pragma unroll
                         for (int m = 0; m < 6; ++m) { alpha[m] = warp_sum(alpha[m]); beta[m] = warp_sum(beta[m]); }
-                        // 2 x (6+1) algebra (every lane, redundantly)
-                        float Yc0[6], Yc1[6];
-#pragma unroll
-                        for (int i = 0; i < 6; ++i) {
-                            float s0 = jd0 * beta[i], s1 = jd1 * beta[i];
-#pragma unroll
-                            for (int m = 0; m < 6; ++m) { s0 = fmaf(a0[m], Scc[m * 6 + i], s0); s1 = fmaf(a1[m], Scc[m * 6 + i], s1); }
-                            Yc0[i] = s0; Yc1[i] = s1;
-                        }
-                        float fb0 = 0.f, fb1 = 0.f, z0 = jd0 * eta, z1 = jd1 * eta;
-#pragma unroll
-                        for (int m = 0; m < 6; ++m) { fb0 = fmaf(a0[m], alpha[m], fb0); fb1 = fmaf(a1[m], alpha[m], fb1); z0 = fmaf(a0[m], sg[m], z0); z1 = fmaf(a1[m], sg[m], z1); }
-                        const float yb0 = fb0 + jd0 * gamma, yb1 = fb1 + jd1 * gamma;
-                        float Q00 = yb0 * jd0, Q01 = yb0 * jd1, Q10 = yb1 * jd0, Q11 = yb1 * jd1;
-#pragma unroll
-                        for (int i = 0; i < 6; ++i) { Q00 = fmaf(Yc0[i], a0[i], Q00); Q01 = fmaf(Yc0[i], a1[i], Q01); Q10 = fmaf(Yc1[i], a0[i], Q10); Q11 = fmaf(Yc1[i], a1[i], Q11); }
-                        // ---- point weight of (frame f, point n), as in lm_build_bwd_kernel: dw = 1/2 <M, Q> + q.z, one writer, no atomics.
-                        //      Q holds gamma = b^T S_dd b from frame 0's depth block, so dw is the adjoint of the window-reduced forward (this
-                        //      point's depth contribution lands in frame 0's block).  Then M, q, Q, z carry w to dJ, dj, db, dd, dG; the
-                        //      rhat sign(d) path is not weighted.  Unweighted: w = 1 and x * 1.0f is exact.
-                        const float wn = prm.weight ? __ldg(prm.weight + b * N + n) : 1.f;
-                        if (prm.dweight && lane == 0) prm.dweight[b * N + n] = 0.5f * (m11 * Q00 + m12 * (Q01 + Q10) + m22 * Q11) + (q1 * z0 + q2 * z1);
-                        m11 *= wn; m12 *= wn; m22 *= wn; q1 *= wn; q2 *= wn;
-                        Q00 *= wn; Q01 *= wn; Q10 *= wn; Q11 *= wn; z0 *= wn; z1 *= wn;
-                        float dJ0[6], dJ1[6];
-#pragma unroll
-                        for (int i = 0; i < 6; ++i) { dJ0[i] = m11 * Yc0[i] + m12 * Yc1[i] + q1 * sg[i]; dJ1[i] = m12 * Yc0[i] + m22 * Yc1[i] + q2 * sg[i]; }
-                        const float dj0 = m11 * yb0 + m12 * yb1 + q1 * eta, dj1 = m12 * yb0 + m22 * yb1 + q2 * eta;
-                        const float u0 = m11 * jd0 + m12 * jd1, u1 = m12 * jd0 + m22 * jd1;
-                        const float sN = jd0 * u0 + jd1 * u1, tN = jd0 * q1 + jd1 * q2;
-                        float vN[6];
-#pragma unroll
-                        for (int i = 0; i < 6; ++i) vN[i] = a0[i] * u0 + a1[i] * u1;
+                        // 2 x (6+1) algebra (every lane, redundantly).  Point weight of (frame f, point n), as in lm_build_bwd_kernel: Q holds
+                        // gamma = b^T S_dd b from frame 0's depth block, so dw is the adjoint of the window-reduced forward (this point's depth
+                        // contribution lands in frame 0's block).
+                        PointAdjoint ad(a0, a1, jd0, jd1, Scc, sg, alpha, beta, eta, gamma);
+                        const float dw = ad.weigh(prm.weight ? __ldg(prm.weight + b * N + n) : 1.f, mq);
+                        if (prm.dweight && lane == 0) prm.dweight[b * N + n] = dw;
+                        float dJ0[6], dJ1[6], dj0, dj1, vN[8];                 // depth terms of db: vN (6), then tN, sN
+                        jacobian_adjoint(mq, ad, sg, eta, dJ0, dJ1, dj0, dj1);
+                        depth_terms(a0, a1, jd0, jd1, mq, vN);
+                        const float tN = vN[6], sN = vN[7];
                         // pass 2: dd, dG per channel -> dconv1 (summed over the frames), dconv2 (atomics), the coordinate gradient
-                        float du = 0.f, dv = 0.f;
-                        for (int c = lane; c < C; c += 32) {
-                            const float t00 = __ldg(img + o00 + c), t01 = __ldg(img + o01 + c), t10 = __ldg(img + o10 + c), t11 = __ldg(img + o11 + c);
-                            const float g00 = __ldg(img + o00 + C + c), g01 = __ldg(img + o01 + C + c), g10 = __ldg(img + o10 + C + c), g11 = __ldg(img + o11 + C + c);
-                            const float k00 = __ldg(img + o00 + 2 * C + c), k01 = __ldg(img + o01 + 2 * C + c), k10 = __ldg(img + o10 + 2 * C + c), k11 = __ldg(img + o11 + 2 * C + c);
-                            const float f2 = w00 * t00 + w01 * t01 + w10 * t10 + w11 * t11;
-                            const float gx = w00 * g00 + w01 * g01 + w10 * g10 + w11 * g11;
-                            const float gy = w00 * k00 + w01 * k01 + w10 * k10 + w11 * k11;
-                            const float d = __ldg(c1 + c) - f2;
-                            const float dd = gx * z0 + gy * z1 + sRh[c] * sgn(d);
-                            const float dgx = gx * Q00 + gy * Q10 + d * z0, dgy = gx * Q01 + gy * Q11 + d * z1;
-                            myDc1[c] += dd;
-                            const float df = -dd;
-                            atomicAdd(dimg + o00 + c, w00 * df); atomicAdd(dimg + o01 + c, w01 * df); atomicAdd(dimg + o10 + c, w10 * df); atomicAdd(dimg + o11 + c, w11 * df);
-                            atomicAdd(dimg + o00 + C + c, w00 * dgx); atomicAdd(dimg + o01 + C + c, w01 * dgx); atomicAdd(dimg + o10 + C + c, w10 * dgx); atomicAdd(dimg + o11 + C + c, w11 * dgx);
-                            atomicAdd(dimg + o00 + 2 * C + c, w00 * dgy); atomicAdd(dimg + o01 + 2 * C + c, w01 * dgy); atomicAdd(dimg + o10 + 2 * C + c, w10 * dgy); atomicAdd(dimg + o11 + 2 * C + c, w11 * dgy);
-                            du += df * ((1.f - dy) * (t01 - t00) + dy * (t11 - t10)) + dgx * ((1.f - dy) * (g01 - g00) + dy * (g11 - g10)) + dgy * ((1.f - dy) * (k01 - k00) + dy * (k11 - k10));
-                            dv += df * ((1.f - dx) * (t10 - t00) + dx * (t11 - t01)) + dgx * ((1.f - dx) * (g10 - g00) + dx * (g11 - g01)) + dgy * ((1.f - dx) * (k10 - k00) + dx * (k11 - k01));
-                        }
-                        du = warp_sum(du); dv = warp_sum(dv);
-                        // geometry backward
-                        float gxx = fx * du, gyy = fy * dv, giZ = 0.f;
-                        gxx += -fx * (dJ0[0] * y - 2.f * x * dJ0[1] + dJ0[5] * iZ) - fy * (-dJ1[1] * y - dJ1[2]);
-                        gyy += -fx * (dJ0[0] * x + dJ0[2]) - fy * (2.f * y * dJ1[0] - dJ1[1] * x + dJ1[5] * iZ);
-                        giZ += -fx * (-dJ0[3] + dJ0[5] * x) - fy * (-dJ1[4] + dJ1[5] * y);
-                        float grx = dj0 * fx * iZ, gry = dj1 * fy * iZ, grz = -dj0 * fx * x * iZ - dj1 * fy * y * iZ;
-                        gxx += -dj0 * fx * rz * iZ; gyy += -dj1 * fy * rz * iZ;
-                        giZ += dj0 * fx * (rx - rz * x) + dj1 * fy * (ry - rz * y);
-                        const float gX = gxx * iZ, gY = gyy * iZ, gZ = -iZ * (gxx * x + gyy * y) - iZ * iZ * giZ;
-                        const float gDt = rx * gX + ry * gY + rz * gZ;
-                        grx += Dt * gX; gry += Dt * gY; grz += Dt * gZ;
+                        float du, dv;
+                        channel_adjoint<false>(img, dimg, c1, sRh, tp, h, w, C, lane, ad, [&](int c, float dd) { myDc1[c] += dd; }, du, dv);
+                        const GeomGrad gg(pr, fx, fy, Dt, du, dv, dJ0, dJ1, dj0, dj1);
                         if (lane == 0) {
-                            sRT[0] += grx * p0; sRT[1] += grx * p1; sRT[2] += grx * p2;
-                            sRT[3] += gry * p0; sRT[4] += gry * p1; sRT[5] += gry * p2;
-                            sRT[6] += grz * p0; sRT[7] += grz * p1; sRT[8] += grz * p2;
-                            sRT[9] += gX; sRT[10] += gY; sRT[11] += gZ;
+                            sRT[0] += gg.grx * p0; sRT[1] += gg.grx * p1; sRT[2] += gg.grx * p2;
+                            sRT[3] += gg.gry * p0; sRT[4] += gg.gry * p1; sRT[5] += gg.gry * p2;
+                            sRT[6] += gg.grz * p0; sRT[7] += gg.grz * p1; sRT[8] += gg.grz * p2;
+                            sRT[9] += gg.gX; sRT[10] += gg.gY; sRT[11] += gg.gZ;
                         }
-                        dDacc += gDt;
+                        dDacc += gg.gDt;
 #pragma unroll
                         for (int i = 0; i < KL; ++i) {
                             const int k = lane + 32 * i;
                             if (k < K) {
-                                float d1 = sN * e[i] + tN * sg[6 + k] + gDt * sW[k];
+                                float d1 = sN * e[i] + tN * sg[6 + k] + gg.gDt * sW[k];
 #pragma unroll
                                 for (int m = 0; m < 6; ++m) d1 = fmaf(vN[m], Scd[m * K + k], d1);
                                 db[i] += d1;
-                                accW[i] = fmaf(gDt, bl[i], accW[i]);
+                                accW[i] = fmaf(gg.gDt, bl[i], accW[i]);
                             }
                         }
                     }
@@ -791,7 +607,7 @@ keyframe_build_bwd_kernel(const KeyBwdParams prm)
 // ------------------------------------------------------------------------------------------------------------------------------------
 int keyframe_plan(const banet_keyframe_level_t* lv, int num_sms, KeyframePlan* plan)
 {
-    const int KP = padded_key_K(lv->K);
+    const int KP = padded_K(lv->K);
     BANET_REQUIRE(lv->K >= 1 && KP > 0, BANET_ERR_UNSUPPORTED, "keyframe build (fp32 SIMT): K=%d > 256 not supported", lv->K);
     BANET_REQUIRE(lv->C <= 2048, BANET_ERR_UNSUPPORTED, "keyframe build: C=%d > 2048", lv->C);
     plan->KP = KP;

@@ -3,6 +3,7 @@
 #include "common.cuh"
 #include "features.cuh"
 #include "lm_build.h"
+#include "point.cuh"
 
 namespace banet {
 
@@ -23,8 +24,6 @@ __global__ void compute_coordinates_kernel(const float* __restrict__ points, con
     float* pb = p + (size_t)b * 3 * N;
     pb[n] = x; pb[(size_t)N + n] = y; pb[2 * (size_t)N + n] = z;
 }
-
-__device__ __forceinline__ int reflect1(int i, int n) { return i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i); }
 
 // grad_fixed + concat (+ half swap): bundlenet.py:92-100, 386-389.  One thread per (texel, 4 channels).
 template <int VEC>
