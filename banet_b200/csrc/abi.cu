@@ -211,14 +211,13 @@ extern "C" int banet_lm_step_bwd(const float* H, const float* g, const float* rb
     BANET_REQUIRE(!mlp_weights || (rbar_sum && drbar_sum && dmlp && N > 0 && C > 0), BANET_ERR_BAD_ARG,
                   "lm_step_bwd: the lambda-MLP needs rbar_sum, drbar_sum, dmlp, N > 0 and C > 0");
     BANET_REQUIRE(!opts->vmatrix_batch_scramble, BANET_ERR_UNSUPPORTED, "lm_step_bwd: vmatrix_batch_scramble is not differentiated");
-    const int Cs = C > 0 ? C : 1;                                    // banet_lm_step's rule: the storage plan depends on C also with lambda given
-    BANET_REQUIRE(lm_step_supported(6 + K, Cs), BANET_ERR_UNSUPPORTED, "lm_step_bwd: K=%d, C=%d do not fit the fused step", K, Cs);
+    BANET_REQUIRE(lm_step_supported(6 + K, mlp_weights ? C : 0), BANET_ERR_UNSUPPORTED, "lm_step_bwd: K=%d, C=%d do not fit the fused step", K, C);
     if (mlp_weights) {
         const size_t need = banet_lm_step_bwd_workspace_bytes(nb, C, K);
         BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_step_bwd: workspace %zu < %zu bytes", ws_bytes, need);
     }
-    return lm_step_bwd(H, g, rbar_sum, nb, N, Cs, K, mlp_weights, lambda, delta, *opts, R, T, dR_out, dT_out, dW_out, dH, dg, drbar_sum, dmlp,
-                       dlambda, dR, dT, dW, reinterpret_cast<float*>(ws), (cudaStream_t)stream);
+    return lm_step_bwd(H, g, rbar_sum, nb, N, C, K, mlp_weights, lambda, delta, *opts, R, T, dR_out, dT_out, dW_out, 6, nullptr, dH, dg, drbar_sum,
+                       dmlp, dlambda, dR, dT, dW, reinterpret_cast<float*>(ws), (cudaStream_t)stream);
 }
 
 extern "C" int banet_lm_build_bwd_weighted(const banet_level_t* lv, const float* R, const float* T, const float* W,
@@ -302,6 +301,9 @@ extern "C" int banet_lm_run(const banet_level_t* levels, int nlevels, int iters_
         BANET_REQUIRE(levels[l].nb == nb && levels[l].K == K, BANET_ERR_BAD_ARG, "lm_run: nb/K must agree across levels");
         BANET_REQUIRE((mlp_weights && mlp_weights[l]) || lambda_fixed >= 0.f, BANET_ERR_BAD_ARG,
                       "lm_run: level %d has no lambda-MLP weights and lambda_fixed < 0", l);
+        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
+        BANET_REQUIRE(lm_step_supported(6 + K, use_mlp ? levels[l].C : 0), BANET_ERR_UNSUPPORTED, "lm_run: K=%d, C=%d do not fit the step kernel",
+                      K, levels[l].C);
     }
     BANET_REQUIRE(K == 0 || W, BANET_ERR_BAD_ARG, "lm_run: K=%d but W is null", K);
     RunCarve c;
@@ -329,18 +331,11 @@ extern "C" int banet_lm_run(const banet_level_t* levels, int nlevels, int iters_
         for (int it = 0; it < iters_per_level; ++it) {
             rc = build_dispatch(lv, res, plan, R, T, W, H, g, rbar, nvalid, base + c.build, st);
             if (rc) return rc;
-            const int P = 6 + K;
-            if (!opts->vmatrix_batch_scramble && lm_step_supported(P, lv->C)) {      // one launch: lambda-MLP + damping + Cholesky + update
-                rc = lm_step(H, g, rbar, nb, lv->N, lv->C, K, use_mlp ? mlp_weights[l] : nullptr, l2_regularizer_base, use_mlp ? nullptr : lam,
-                             kStepBundleNet, nullptr, *opts, R, T, W, R, T, W, delta, lam, status, 1, st);
-                if (rc) return rc;
-                continue;
-            }
-            if (use_mlp) {
-                rc = lm_lambda(rbar, nb, lv->N, lv->C, mlp_weights[l], l2_regularizer_base, lam, st);
-                if (rc) return rc;
-            }
-            rc = lm_solve_update(H, g, lam, nb, K, *opts, R, T, W, R, T, W, delta, status, 1, st);
+            // one launch: lambda-MLP + damping + Cholesky + update; the batch-interleaved VMatrix updates R, T after every pair's step
+            const bool scramble = opts->vmatrix_batch_scramble != 0;
+            rc = lm_step(H, g, rbar, nb, lv->N, lv->C, K, use_mlp ? mlp_weights[l] : nullptr, l2_regularizer_base, use_mlp ? nullptr : lam,
+                         kStepBundleNet, nullptr, *opts, R, T, W, scramble ? nullptr : R, T, W, delta, lam, status, 1, st);
+            if (!rc && scramble) rc = launch_pose_update(delta, nb, 6 + K, 1, R, T, R, T, st);
             if (rc) return rc;
         }
     }
@@ -451,8 +446,7 @@ extern "C" int banet_lm_window_solve_update_bwd(const float* H, const float* g, 
                   "lm_window_solve_update_bwd: null pointer");
     BANET_REQUIRE(nf > 0 && K > 0 && !opts->vmatrix_batch_scramble, BANET_ERR_BAD_ARG,
                   "lm_window_solve_update_bwd: needs nf > 0, a depth basis (K > 0) and vmatrix_batch_scramble = 0 (nf=%d K=%d)", nf, K);
-    BANET_REQUIRE(lm_window_supported(nf, K, 1) && solve_bwd_supported(6 * nf + K), BANET_ERR_UNSUPPORTED,
-                  "lm_window_solve_update_bwd: 6*%d+%d unknowns do not fit the solve kernels", nf, K);
+    BANET_REQUIRE(lm_window_supported(nf, K, 0), BANET_ERR_UNSUPPORTED, "lm_window_solve_update_bwd: 6*%d+%d unknowns do not fit the solve kernel", nf, K);
     const size_t need = banet_lm_window_solve_update_bwd_workspace_bytes(nf, K);
     BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_window_solve_update_bwd: workspace %zu < %zu bytes", ws_bytes, need);
     return lm_window_step_bwd(H, g, lambda, delta, nf, K, *opts, R, T, dR_out, dT_out, dW_out, dH, dg, dlambda, dR, dT, dW,

@@ -64,29 +64,30 @@ int plan_for(const banet_level_t* lv, int resolved, BuildPlan* plan);
 int build_dispatch(const banet_level_t* lv, int resolved, const BuildPlan& plan, const float* R, const float* T, const float* W,
                    float* H, float* g, float* rbar_sum, float* nvalid, void* ws, cudaStream_t st);
 
-// lambda MLP / solve / update (lm_solve.cu)
-int lm_lambda(const float* rbar_sum, int nb, int N, int C, const float* mlp, float base, float* lambda_out, cudaStream_t st);
-bool lm_solve_uses_double(int P);
-int lm_solve_update(const float* H, const float* g, const float* lambda, int nb, int K, const banet_solve_opts_t& opts,
-                    const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
-                    float* delta, int32_t* status, int status_accumulate, cudaStream_t st);
-
 // fused lambda-MLP + damping + blocked Cholesky + update, one launch (lm_step.cu); mlp == nullptr: lambda_in is used as is
 struct StepMode { float lambda_exp0; int rbar_per_valid, use_vmatrix, clamp_theta; };
 constexpr StepMode kStepBundleNet = {2.0f, 0, 1, 1};          // bundlenet.py:241-276
-bool lm_step_supported(int P, int C);
-bool lm_step_uses_double(int P, int C);
+bool lm_step_supported(int P, int Cm);                        // Cm: the lambda-MLP width, 0 when lambda is given
 int lm_step(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K, const float* mlp, float base, const float* lambda_in,
             const StepMode& mode, const float* nvalid, const banet_solve_opts_t& opts, const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
             float* delta, float* lambda_out, int32_t* status, int status_accumulate, cudaStream_t st);
-// its backward (kStepBundleNet), in the forward's storage plan for (P, C); ws: nb * lm_step_bwd_ws_floats(C) floats when mlp != nullptr
+// its backward (kStepBundleNet), in the forward's storage plan; ws: nb * lm_step_bwd_ws_floats(C) floats when mlp != nullptr.  ddelta_pose
+// != nullptr: the first npose unknowns are poses whose update backward the caller ran (ddelta_pose [nb, npose]; dR, dT untouched); else npose = 6
 size_t lm_step_bwd_ws_floats(int C);
 int lm_step_bwd(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K, const float* mlp, const float* lambda,
                 const float* delta, const banet_solve_opts_t& opts, const float* R, const float* T, const float* gRn, const float* gTn,
-                const float* gWn, float* dH, float* dg, float* drbar_sum, float* dmlp, float* dlambda, float* dR, float* dT, float* dW,
-                float* ws, cudaStream_t st);
-
-int launch_pose_update(const float* delta, int nb, int P, const float* R, const float* T, float* R_out, float* T_out, cudaStream_t st);
+                const float* gWn, int npose, const float* ddelta_pose, float* dH, float* dg, float* drbar_sum, float* dmlp, float* dlambda,
+                float* dR, float* dT, float* dW, float* ws, cudaStream_t st);
+// the step's pieces on their own: lambda (banet_lm_lambda), the step with lambda given and its backward (banet_lm_solve_update(_bwd)), and
+// the SE(3) update of nb poses from their steps delta [nb, P] (scramble: vmatrix_batch_scramble)
+int lm_lambda(const float* rbar_sum, int nb, int N, int C, const float* mlp, float base, float* lambda_out, cudaStream_t st);
+int lm_solve_update(const float* H, const float* g, const float* lambda, int nb, int K, const banet_solve_opts_t& opts,
+                    const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
+                    float* delta, int32_t* status, int status_accumulate, cudaStream_t st);
+int lm_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int K, const banet_solve_opts_t& opts,
+                        const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
+                        float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, cudaStream_t st);
+int launch_pose_update(const float* delta, int nb, int P, int scramble, const float* R, const float* T, float* R_out, float* T_out, cudaStream_t st);
 
 // joint step of a keyframe window: nf pairs sharing one W (lm_window.cu); ws: lm_window_step_workspace_floats floats
 bool lm_window_supported(int nf, int K, int C);
@@ -139,16 +140,8 @@ int lm_track_legacy(const banet_level_t* levels, int nlevels, const int* level_i
 // backward of one iteration (lm_bwd.cu)
 int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dH, const float* dg, const float* drbar,
                  int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, float* dweight, cudaStream_t st);
-int lm_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int K, const banet_solve_opts_t& opts,
-                        const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
-                        float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, cudaStream_t st);
-// its two stages: the SE(3) update backward (ddelta[0:6] of pair b -> ddelta + b * P), and u = Ht^-1 [ddelta[0:npose] | dW'] with dH, dg = u,
-// dlambda, dW = dW' (pairs of P unknowns, the first npose of them poses).  g [nb,P] is the forward's right-hand side (a non-finite entry
-// skipped the step); use_double: the precision the forward factored in (lm_solve_uses_double / lm_step_uses_double)
+// the SE(3) update backward of nb poses (ddelta[0:6] of pose b -> ddelta + b * P)
 int launch_pose_update_bwd(const float* delta, int nb, int P, const float* R, const float* T, const float* gRn, const float* gTn,
                            float* ddelta, float* dR, float* dT, cudaStream_t st);
-bool solve_bwd_supported(int P);
-int launch_solve_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int P, int npose, bool use_double,
-                     const banet_solve_opts_t& opts, const float* gWn, float* dH, float* dg, float* dlambda, float* dW, cudaStream_t st);
 
 }  // namespace banet

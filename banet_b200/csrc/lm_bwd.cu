@@ -14,13 +14,11 @@
 //   then the chain rule through the sampler (features: atomics into dconv2; coordinates: tap differences), the projection, the
 //   warp (dR, dT), and the depth update (dD, dB, dW).  With point weights (H = sum w_n H_n, g = sum w_n g_n) the Ghat / ghat adjoints of
 //   pixel n are scaled by w_n and dw_n = 1/2 <M, Q> + q.z, stored by its one writer.
-// lm_solve_update_bwd_kernel: delta = Ht^-1 g, Ht = H + diag(damp (diag H + eps)) lambda  ->  u = Ht^-1 ddelta, dg = u, dHt = -u delta^T,
-//   dH = dHt (1 + damp lambda on the diagonal), dlambda = sum_i dHt_ii damp_i (H_ii + eps); ddelta from the SE(3) update by forward-mode
-//   dual numbers over the same expressions as pose_update_kernel (lm_solve.cu).
+// pose_update_bwd_kernel: the SE(3) update's backward, thread per pair, for the dense keyframe window (lm_window.cu); the solve's backward is
+//   lm_step_bwd_kernel (lm_step.cu).
 #include "common.cuh"
 #include "features.cuh"
 #include "lm_build.h"
-#include "lm_step.cuh"
 #include "pose_bwd.cuh"
 #include "point.cuh"
 
@@ -268,7 +266,7 @@ int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const 
 }
 
 // ------------------------------------------------------------------------------------------------------------------------------------
-// solve + update backward
+// SE(3) update backward
 // ------------------------------------------------------------------------------------------------------------------------------------
 // SE(3) update backward, thread per pair, double (R' = exp(w) R, T' = V(w) t + exp(w) T; bundlenet.py:269-275): writes
 // ddelta[0:6] (into `ddelta`, row stride P), dR, dT.
@@ -283,130 +281,12 @@ __global__ void pose_update_bwd_kernel(const float* __restrict__ delta, int nb, 
     pose_update_bwd_one(dl, R + (size_t)b * 9, T + (size_t)b * 3, gRn + (size_t)b * 9, gTn + (size_t)b * 3, ddelta + (size_t)b * P, dR + (size_t)b * 9, dT + (size_t)b * 3);
 }
 
-constexpr int SB_THREADS = 1024;
-static_assert(SB_THREADS == STEP_THREADS, "solve_adjoint_outputs (lm_step.cuh) strides by STEP_THREADS");
-__host__ __device__ __forceinline__ int tri2(int i, int k) { return i * (i + 1) / 2 + k; }
-
-// u = Ht^-1 ddelta with the same Cholesky as lm_solve_kernel; dg (in: ddelta[0:npose] from pose_update_bwd_kernel, out: u).  npose = 6 for the
-// pairs of the 2-view iteration, 6 nf for the one system of a keyframe window; the remaining P - npose entries of ddelta are dW'.
-template <typename S>
-__global__ void __launch_bounds__(SB_THREADS)
-lm_solve_bwd_kernel(const float* __restrict__ H, const float* __restrict__ g, const float* __restrict__ lambda, const float* __restrict__ delta, int P,
-                    int npose, float eps, int ndamped, const float* __restrict__ gWn, float* __restrict__ dH, float* __restrict__ dg,
-                    float* __restrict__ dlambda, float* __restrict__ dW)
-{
-    extern __shared__ __align__(16) unsigned char smraw[];
-    S* A = reinterpret_cast<S*>(smraw);                 // packed lower triangle of the damped matrix -> its Cholesky factor
-    S* r = A + (size_t)P * (P + 1) / 2;                 // delta (the saved forward solution)
-    S* uu = r + P;                                      // ddelta -> u
-    S* dgq = uu + P;                                    // sqrt of the pivots
-    __shared__ int s_flag;
-    __shared__ double s_dl[SB_THREADS / 32];            // per-warp partial sums of dlambda, added in a fixed order: bit-reproducible
-    const int b = blockIdx.x, tid = threadIdx.x, K = P - npose;
-    const float* Hb = H + (size_t)b * P * P;
-    const float lam = lambda[b];
-    if (tid == 0) s_flag = 0;
-    __syncthreads();
-    int bad = 0;
-    for (int i = tid / 32; i < P; i += SB_THREADS / 32)
-        for (int k = tid % 32; k <= i; k += 32) {
-            const float v = Hb[(size_t)i * P + k];
-            if (!isfinite(v)) bad = 1;
-            S sv = (S)v;
-            if (k == i && i < ndamped) sv += ((S)v + (S)eps) * (S)lam;
-            A[tri2(i, k)] = sv;
-        }
-    for (int i = tid; i < P; i += SB_THREADS) {
-        if (!isfinite(g[(size_t)b * P + i])) bad = 1;          // the forward skipped the step on a non-finite right-hand side too
-        r[i] = (S)delta[(size_t)b * P + i];
-        if (i < npose) uu[i] = (S)dg[(size_t)b * P + i];
-        else { const float v = gWn[(size_t)b * K + i - npose]; uu[i] = (S)v; dW[(size_t)b * K + i - npose] = v; }       // W' = W + delta_d
-    }
-    if (!isfinite(lam)) bad = 1;
-    if (bad) atomicOr(&s_flag, 2);
-    const int ta = tid >> 5, tb = tid & 31;
-    S inv_prev = (S)1;
-    for (int j = 0; j < P; ++j) {                       // same right-looking Cholesky as lm_solve_kernel
-        __syncthreads();
-        if (j > 0) for (int i = j + tid; i < P; i += SB_THREADS) A[tri2(i, j - 1)] *= inv_prev;
-        S d = A[tri2(j, j)];
-        if (!(d > (S)0)) { if (tid == 0) atomicOr(&s_flag, 1); d = (S)1; }
-        const S invd = (S)1 / d;
-        inv_prev = (S)1 / sqrt(d);
-        for (int i = j + 1 + ta; i < P; i += 32) {
-            const S ci = A[tri2(i, j)] * invd;
-            for (int k = j + 1 + tb; k <= i; k += 32) A[tri2(i, k)] -= ci * A[tri2(k, j)];
-        }
-        if (tid == 0) dgq[j] = sqrt(d);
-    }
-    __syncthreads();
-    if (tid < 32) {                                     // warp 0: L y = ddelta, L^T u = y
-        const int lane = tid;
-        S* x = uu;
-        for (int j = 0; j < P; ++j) {
-            __syncwarp();
-            const S yj = x[j] / dgq[j];
-            __syncwarp();
-            if (lane == 0) x[j] = yj;
-            for (int i = j + 1 + lane; i < P; i += 32) x[i] -= A[tri2(i, j)] * yj;
-        }
-        for (int j = P - 1; j >= 0; --j) {
-            __syncwarp();
-            const S xj = x[j] / dgq[j];
-            __syncwarp();
-            if (lane == 0) x[j] = xj;
-            for (int i = lane; i < j; i += 32) x[i] -= A[tri2(j, i)] * xj;
-        }
-    }
-    __syncthreads();
-    const float dl = solve_adjoint_outputs<S>(uu, r, Hb, P, ndamped, eps, lam, s_flag, dH + (size_t)b * P * P, dg + (size_t)b * P, s_dl, tid);
-    if (tid == 0) dlambda[b] = dl;
-}
-
 int launch_pose_update_bwd(const float* delta, int nb, int P, const float* R, const float* T, const float* gRn, const float* gTn,
                            float* ddelta, float* dR, float* dT, cudaStream_t st)
 {
     pose_update_bwd_kernel<<<(nb + 63) / 64, 64, 0, st>>>(delta, nb, P, R, T, gRn, gTn, ddelta, dR, dT);
     BANET_CUDA_LAUNCH_CHECK("pose_update_bwd_kernel launch");
     return BANET_OK;
-}
-
-// packed lower triangle + 3 vectors in shared memory, in the precision of the forward's factorisation: the backward re-derives the forward's
-// skip decision from its own factorisation, so the two must factor alike.  Double needs 205 160 B at the largest pair system (P = 223).
-static size_t solve_bwd_floats(int P) { return (size_t)P * (P + 1) / 2 + 3 * (size_t)P; }
-bool solve_bwd_supported(int P) { return solve_bwd_floats(P) * sizeof(float) <= 220 * 1024; }
-
-int launch_solve_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int P, int npose, bool use_double,
-                     const banet_solve_opts_t& opts, const float* gWn, float* dH, float* dg, float* dlambda, float* dW, cudaStream_t st)
-{
-    const int ndamped = opts.undamped_last ? P - 1 : P;
-    const size_t smem = solve_bwd_floats(P) * (use_double ? sizeof(double) : sizeof(float));
-    BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_solve_bwd: P=%d does not fit shared memory", P);
-    cudaError_t e;
-    if (use_double) {
-        e = cudaFuncSetAttribute(lm_solve_bwd_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { set_error("lm_solve_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
-        lm_solve_bwd_kernel<double><<<nb, SB_THREADS, smem, st>>>(H, g, lambda, delta, P, npose, opts.damping_eps, ndamped, gWn, dH, dg, dlambda, dW);
-    } else {
-        e = cudaFuncSetAttribute(lm_solve_bwd_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { set_error("lm_solve_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
-        lm_solve_bwd_kernel<float><<<nb, SB_THREADS, smem, st>>>(H, g, lambda, delta, P, npose, opts.damping_eps, ndamped, gWn, dH, dg, dlambda, dW);
-    }
-    BANET_CUDA_LAUNCH_CHECK("lm_solve_bwd_kernel launch");
-    return BANET_OK;
-}
-
-int lm_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int K, const banet_solve_opts_t& opts,
-                        const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
-                        float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, cudaStream_t st)
-{
-    BANET_REQUIRE(!opts.vmatrix_batch_scramble, BANET_ERR_UNSUPPORTED,
-                  "lm_solve_update_bwd: the batch-interleaved VMatrix of bundlenet.py:45 is not differentiated (use vmatrix_batch_scramble=0)");
-    const int P = 6 + K;
-    BANET_REQUIRE(solve_bwd_supported(P), BANET_ERR_UNSUPPORTED, "lm_solve_update_bwd: P=%d does not fit shared memory", P);
-    int rc = launch_pose_update_bwd(delta, nb, P, R, T, gRn, gTn, dg, dR, dT, st);       // ddelta[0:6] parked in dg
-    if (rc) return rc;
-    return launch_solve_bwd(H, g, lambda, delta, nb, P, 6, lm_solve_uses_double(P), opts, gWn, dH, dg, dlambda, dW, st);
 }
 
 }  // namespace banet

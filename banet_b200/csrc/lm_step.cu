@@ -1,21 +1,20 @@
 // One kernel for everything of an LM iteration that is not the normal-equation build: lambda-MLP, damping, blocked Cholesky with the
-// right-hand side carried as an extra row, blocked back substitution, SE(3) / depth-coefficient update.
-//
-// Replaces, per iteration, lm_lambda_kernel + lm_solve_kernel + pose_update_kernel (lm_solve.cu; reference bundlenet.py:241-253, 264-276):
-// those are three launches of nb CTAs whose run time is pure dependent latency (measured round 1: 64 + 215..258 + 5 us, about 11 % of a cfg2
-// solve).  Here: one launch, one CTA (1024 threads) per pair:
+// right-hand side carried as an extra row, blocked back substitution, SE(3) / depth-coefficient update.  One launch, one CTA (1024 threads)
+// per pair:
 //   1. rbar = rbar_sum / N, ||rbar||; 5 dense layers C->2C->4C->2C->C->1 (selu x4, tanh): warps take (32 outputs x an input slice) tasks,
 //      lanes over consecutive outputs (coalesced 128-B weight rows, 8 rows in flight per lane), slices combined through shared memory;
 //      lambda = base * ||rbar||^(2 + tanh(.))                                                            (bundlenet.py:243-253)
-//   2. packed lower triangle of H (+ damping on the diagonal) and g as row P of the same packed array, in S = double (P <= 200) or float;
+//   2. lower triangle of H (+ damping on the diagonal) and g as row P of the same array, in S = double (square to P = 157, packed to 222) or
+//      float (packed, to 332), in the storage the MLP's buffers used (lm_step.cuh);
 //   3. right-looking Cholesky in panels of 4 columns: one thread per row of the panel (the block's own rows, the rows below, and row P = the
 //      right-hand side, so that forward substitution comes for free); every row owner factors the 4x4 diagonal block redundantly IN REGISTERS and
 //      solves its own row against it (a single thread factoring through shared memory was 37 % of the first version's run time, measured);
 //      warp-per-row trailing update; 3 block barriers per panel instead of one per column;
 //   4. back substitution L^T x = y panel by panel (4 warps form the 4 dot products of a panel, thread 0 solves the 4x4 triangle in registers);
 //   5. delta, W' = W + delta_d, status; R' = exp(w) R, T' = V(w) t + exp(w) T in double by thread 0 (per-pair VMatrix).
-// The reference's batch-interleaved VMatrix (vmatrix_batch_scramble, bundlenet.py:45) needs every pair's delta first: the host falls back to
-// the three-kernel path for that option.
+// The same kernel is the pair solve with lambda given (banet_lm_solve_update) and, with its backward, the dense keyframe window's solve.  The
+// reference's batch-interleaved VMatrix (vmatrix_batch_scramble, bundlenet.py:45) needs every pair's delta first: the step then leaves R, T
+// alone (R_out == nullptr) and pose_update_kernel follows.  banet_lm_lambda is step 1 on its own (step_lambda_kernel).
 #include "lm_step.cuh"
 #include "pose_bwd.cuh"
 
@@ -35,12 +34,11 @@ lm_step_kernel(const float* __restrict__ H, const float* __restrict__ g, const f
     // consecutive rows are bank-conflict free for 64-bit words; the packed triangle's varying row offsets were 2..4-way conflicted); else packed.
     S* A = reinterpret_cast<S*>(smraw);
     const int LD = (P + 1) | 1;
-    const size_t nA = FULL ? (size_t)(P + 1) * LD : (size_t)(P + 1) * (P + 2) / 2;
     auto IX = [&](int i, int k) -> int { return FULL ? i * LD + k : i * (i + 1) / 2 + k; };
-    S* xs = A + nA;                                                  // [P] solution
+    float* mbuf = reinterpret_cast<float*>(smraw);                   // MLP buffers (A's storage): 2 x 4C floats + max(4C, 1024) floats of slice partials
+    S* xs = reinterpret_cast<S*>(smraw + step_vectors_offset(P, FULL, sizeof(S), lambda_in ? 0 : C));   // [P] solution
     S* dinv = xs + P;                                                // [P] reciprocals of the Cholesky diagonal
     S* dots = dinv + P;                                              // [STEP_NB]
-    float* mbuf = reinterpret_cast<float*>(dots + STEP_NB);          // MLP buffers: 2 x 4C floats + max(4C, 1024) floats of slice partials
     __shared__ int s_flag;
     __shared__ float s_wpart[STEP_WARPS], s_lam;
     const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, K = P - 6;
@@ -57,7 +55,7 @@ lm_step_kernel(const float* __restrict__ H, const float* __restrict__ g, const f
         lam = step_lambda_mlp(part, mbuf, C, mlp, base, mode.lambda_exp0, s_wpart, &s_lam, lambda_out + b, tid);
     } else {
         lam = lambda_in[b];
-        if (tid == 0) lambda_out[b] = lam;
+        if (tid == 0 && lambda_out) lambda_out[b] = lam;
     }
 
     // ---- 2. load (+ damping, bundlenet.py:264-266 / :181-182) -------------------------------------------------------------------------------
@@ -89,6 +87,7 @@ lm_step_kernel(const float* __restrict__ H, const float* __restrict__ g, const f
     }
     if (tid == 0) {
         status[b] = status_accumulate ? (status[b] | flag) : flag;
+        if (!R_out) return;                                          // the caller updates R, T (vmatrix_batch_scramble)
         double dl[6];
         for (int i = 0; i < 6; ++i) { float dv = flag ? 0.f : (float)xs[i]; if (!isfinite(dv)) dv = 0.f; dl[i] = (double)dv; }
         se3_update(dl, mode, R + (size_t)b * 9, T + (size_t)b * 3, R_out + (size_t)b * 9, T_out + (size_t)b * 3);
@@ -100,33 +99,36 @@ lm_step_kernel(const float* __restrict__ H, const float* __restrict__ g, const f
 //      the forward);
 //   2. the SE(3) update backward at the forward's step (pose_bwd.cuh): ddelta[0:6], dR, dT; dW = dW';
 //   3. the damped matrix factored as the forward did, with [ddelta[0:6] | dW'] as row P: u = Ht^-1 [ddelta | dW'];
-//   4. dH = -u delta^T ((1 + lambda) on the damped diagonal), dg = u, dlambda (solve_adjoint_outputs, shared with lm_solve_bwd_kernel);
+//   4. dH = -u delta^T ((1 + lambda) on the damped diagonal), dg = u, dlambda (solve_adjoint_outputs);
 //   5. through lambda = base ||rbar||^(2 + t), t = tanh(z_5): dt = dlambda lambda ln||rbar||, d||rbar|| = dlambda lambda (2 + t) / ||rbar||,
 //      then the five layers backwards (warp per input row, fixed-order warp sums; selu' from the stored output a: scale if a > 0, else
-//      a + scale alpha), each layer's output delta stored next to its input activation; drbar_sum = drbar / N.
+//      a + scale alpha), each layer's output delta stored next to its input activation; drbar_sum = drbar / N.  The MLP's buffers share A's
+//      storage: step 4 reads u, delta and the global H, not A.
 // The skip is re-derived from H, g, lambda exactly as the forward decides it; a skipped pair gets zero dH, dg, dlambda, drbar_sum and a zero
 // workspace row (no MLP contribution) and passes dR', dT', dW' through (its delta is 0).
+// ddelta_pose != nullptr (the dense keyframe window, lambda given): the first npose unknowns are poses whose update backward the caller ran;
+// their rows of the right-hand side come from ddelta_pose [nb, npose] (it may be dg: it is read before dg is written), step 2 is skipped and
+// dR, dT are not written.  Else npose = 6.
 template <typename S, bool FULL>
 __global__ void __launch_bounds__(STEP_THREADS)
 lm_step_bwd_kernel(const float* __restrict__ H, const float* __restrict__ g, const float* __restrict__ rbar_sum, int N, int C,
-                   const float* __restrict__ mlp, const float* __restrict__ lambda, const float* __restrict__ delta, int P, float eps, int ndamped,
-                   const float* __restrict__ R, const float* __restrict__ T, const float* __restrict__ gRn, const float* __restrict__ gTn,
-                   const float* __restrict__ gWn, float* __restrict__ dH, float* __restrict__ dg, float* __restrict__ drbar_sum,
+                   const float* __restrict__ mlp, const float* __restrict__ lambda, const float* __restrict__ delta, int P, int npose, float eps,
+                   int ndamped, const float* __restrict__ R, const float* __restrict__ T, const float* __restrict__ gRn, const float* __restrict__ gTn,
+                   const float* __restrict__ gWn, const float* ddelta_pose, float* __restrict__ dH, float* dg, float* __restrict__ drbar_sum,
                    float* __restrict__ dlambda, float* __restrict__ dR, float* __restrict__ dT, float* __restrict__ dW, float* ws)
 {
     extern __shared__ __align__(16) unsigned char smraw[];
     S* A = reinterpret_cast<S*>(smraw);                              // the forward's layout (lm_step_kernel)
     const int LD = (P + 1) | 1;
-    const size_t nA = FULL ? (size_t)(P + 1) * LD : (size_t)(P + 1) * (P + 2) / 2;
     auto IX = [&](int i, int k) -> int { return FULL ? i * LD + k : i * (i + 1) / 2 + k; };
-    S* xs = A + nA;                                                  // [P] u
+    float* mbuf = reinterpret_cast<float*>(smraw);                   // MLP buffers as in the forward; the backward's deltas ping-pong in 2 x 4C
+    S* xs = reinterpret_cast<S*>(smraw + step_vectors_offset(P, FULL, sizeof(S), mlp ? C : 0));   // [P] u
     S* dinv = xs + P;                                                // [P] reciprocals of the Cholesky diagonal, then the forward's delta
     S* dots = dinv + P;
-    float* mbuf = reinterpret_cast<float*>(dots + STEP_NB);          // MLP buffers as in the forward; the backward's deltas ping-pong in 2 x 4C
     __shared__ int s_flag;
     __shared__ float s_wpart[STEP_WARPS], s_lam, s_lam_unused, s_ddl[6], s_dn;
     __shared__ double s_part[STEP_WARPS];
-    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, K = P - 6;
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, K = P - npose;
     float* keep = mlp ? ws + (size_t)b * mlp_ws_stride(C) : nullptr;
     const float invN = 1.0f / (float)N;
     if (tid == 0) s_flag = 0;
@@ -141,7 +143,7 @@ lm_step_bwd_kernel(const float* __restrict__ H, const float* __restrict__ g, con
     const float lam = lambda[b];
 
     // ---- 2. SE(3) update backward at the forward's step -----------------------------------------------------------------------------------
-    if (tid == 0) {
+    if (tid == 0 && !ddelta_pose) {
         double dl[6];
         for (int i = 0; i < 6; ++i) { dl[i] = delta[(size_t)b * P + i]; if (!isfinite(dl[i])) dl[i] = 0.0; }
         pose_update_bwd_one(dl, R + (size_t)b * 9, T + (size_t)b * 3, gRn + (size_t)b * 9, gTn + (size_t)b * 3, s_ddl, dR + (size_t)b * 9,
@@ -163,8 +165,8 @@ lm_step_bwd_kernel(const float* __restrict__ H, const float* __restrict__ g, con
     for (int k = tid; k < P; k += STEP_THREADS) {
         if (!isfinite(g[(size_t)b * P + k])) bad = 1;                // the forward skipped the step on a non-finite right-hand side
         float v;
-        if (k < 6) v = s_ddl[k];
-        else { v = gWn[(size_t)b * K + k - 6]; dW[(size_t)b * K + k - 6] = v; }      // W' = W + delta_d
+        if (k < npose) v = ddelta_pose ? ddelta_pose[(size_t)b * npose + k] : s_ddl[k];
+        else { v = gWn[(size_t)b * K + k - npose]; dW[(size_t)b * K + k - npose] = v; }      // W' = W + delta_d
         A[IX(P, k)] = (S)v;
     }
     if (!isfinite(lam)) bad = 1;
@@ -248,41 +250,73 @@ __global__ void lm_mlp_grad_kernel(const float* __restrict__ ws, int nb, int C, 
     dmlp[idx] = s;
 }
 
-size_t lm_step_smem(int P, int C, bool use_double, bool full)
+// R' = exp(w) R, T' = V(w) t + exp(w) T for nb pairs from their steps delta [nb, P], thread per pair (in place is fine: a thread reads its pair
+// before it writes).  scramble: V is built from the batch-interleaved skew matrices of bundlenet.py:45 (vmatrix_batch_scramble), which need
+// every pair's step first.
+__global__ void pose_update_kernel(const float* __restrict__ delta, int nb, int P, int scramble, const float* R, const float* T, float* R_out,
+                                   float* T_out)
 {
-    const size_t nA = (full ? (size_t)(P + 1) * ((P + 1) | 1) : (size_t)(P + 1) * (P + 2) / 2) + 2 * (size_t)P + STEP_NB;
-    return nA * (use_double ? sizeof(double) : sizeof(float)) + ((size_t)8 * C + (4 * C > 1024 ? 4 * C : 1024)) * sizeof(float);
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nb) return;
+    double dl[6], sk[9];
+    for (int i = 0; i < 6; ++i) dl[i] = delta[(size_t)b * P + i];
+    if (scramble) {
+        // literal bundlenet.py:45: tf.stack([...9 x [nb,1,1]...]) on axis 0, then reshape [-1,3,3]: flat[e*nb + b'] = skew entry e of pair
+        // b'; matrix b takes flat[b*9 .. b*9+8]
+        for (int q = 0; q < 9; ++q) {
+            const int f = b * 9 + q, e = f / nb, bp = f - e * nb;
+            const float* d2 = delta + (size_t)bp * P;
+            const double ax = d2[0], ay = d2[1], az = d2[2];
+            const double ent[9] = {0, -az, ay, az, 0, -ax, -ay, ax, 0};
+            sk[q] = ent[e];
+        }
+    }
+    const StepMode mode = kStepBundleNet;
+    se3_update(dl, mode, R + (size_t)b * 9, T + (size_t)b * 3, R_out + (size_t)b * 9, T_out + (size_t)b * 3, scramble ? sk : nullptr);
 }
 
-bool lm_step_supported(int P, int C) { return lm_step_smem(P, C, false, false) <= 220 * 1024; }
+// banet_lm_lambda: step 1 of lm_step_kernel on its own (the same code, so the same lambda bit for bit), one CTA per pair
+__global__ void __launch_bounds__(STEP_THREADS)
+step_lambda_kernel(const float* __restrict__ rbar_sum, int N, int C, const float* __restrict__ mlp, float base, float* __restrict__ lambda_out)
+{
+    extern __shared__ __align__(16) unsigned char smraw[];
+    float* mbuf = reinterpret_cast<float*>(smraw);
+    __shared__ float s_wpart[STEP_WARPS], s_lam;
+    const int b = blockIdx.x, tid = threadIdx.x;
+    const float invN = 1.0f / (float)N;
+    float part = 0.f;
+    for (int c = tid; c < C; c += STEP_THREADS) { const float r = rbar_sum[(size_t)b * C + c] * invN; mbuf[c] = r; part += r * r; }
+    step_lambda_mlp(part, mbuf, C, mlp, base, kStepBundleNet.lambda_exp0, s_wpart, &s_lam, lambda_out + b, tid);
+}
 
-// storage: square double (P <= ~150), packed double (P <= ~200), packed float beyond; the dense window's backward (lm_window.cu) factors in
-// the precision this picks for its forward
-bool lm_step_uses_double(int P, int C) { return lm_step_smem(P, C, true, false) <= 200 * 1024; }
-
-// the storage of lm_step_kernel and of its backward, which must factor alike (the backward re-derives the forward's skip from its own
-// factorisation) and which need the same shared memory: one plan for both
+// The storage of lm_step_kernel and of its backward, which must factor alike (the backward re-derives the forward's skip from its own
+// factorisation): square double (P <= 157), packed double (P <= 222), packed float (P <= 332), from the matrix and the vectors alone.  smem
+// adds the MLP's buffers where they outgrow the matrix (lm_step.cuh); Cm: the MLP width, 0 when lambda is given.
 namespace {
 struct StepPlan { bool full, use_double; size_t smem; };
-StepPlan step_plan(int P, int C)
+size_t step_solve_bytes(int P, bool dbl, bool full) { return (step_matrix_elems(P, full) + 2 * (size_t)P + STEP_NB) * (dbl ? sizeof(double) : sizeof(float)); }
+StepPlan step_plan(int P, int Cm)
 {
     StepPlan p;
-    p.full = lm_step_smem(P, C, true, true) <= 200 * 1024;
-    p.use_double = lm_step_uses_double(P, C);
-    p.smem = lm_step_smem(P, C, p.use_double, p.full);
+    p.full = step_solve_bytes(P, true, true) <= 200 * 1024;
+    p.use_double = p.full || step_solve_bytes(P, true, false) <= 200 * 1024;
+    const size_t elem = p.use_double ? sizeof(double) : sizeof(float);
+    p.smem = step_vectors_offset(P, p.full, elem, Cm) + (2 * (size_t)P + STEP_NB) * elem;
     return p;
 }
 }  // namespace
 
-// lambda_in != nullptr: used as is; else lambda = base * ||rbar||^(exp0 + MLP(rbar)) (MLP term 0 when mlp == nullptr).
-// In-place R/T/W (R_out == R ...) is fine: a pair's CTA reads before it writes.
+bool lm_step_supported(int P, int Cm) { return step_plan(P, Cm).smem <= 220 * 1024; }
+
+// lambda_in != nullptr: used as is (lambda_out, optional, receives it); else lambda = base * ||rbar||^(exp0 + MLP(rbar)) (MLP term 0 when
+// mlp == nullptr).  R_out == nullptr: R, T are not updated.  In-place R/T/W (R_out == R ...) is fine: a pair's CTA reads before it writes.
 int lm_step(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K, const float* mlp, float base, const float* lambda_in,
             const StepMode& mode, const float* nvalid, const banet_solve_opts_t& opts, const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
             float* delta, float* lambda_out, int32_t* status, int status_accumulate, cudaStream_t st)
 {
     const int P = 6 + K;
     const int ndamped = opts.undamped_last ? P - 1 : P;
-    const StepPlan plan = step_plan(P, C);
+    const StepPlan plan = step_plan(P, lambda_in ? 0 : C);
     const size_t smem = plan.smem;
     BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_step: P=%d, C=%d do not fit shared memory", P, C);
     auto launch = [&](auto kern) -> int {
@@ -301,24 +335,55 @@ int lm_step(const float* H, const float* g, const float* rbar_sum, int nb, int N
     return BANET_OK;
 }
 
+int launch_pose_update(const float* delta, int nb, int P, int scramble, const float* R, const float* T, float* R_out, float* T_out, cudaStream_t st)
+{
+    pose_update_kernel<<<(nb + 127) / 128, 128, 0, st>>>(delta, nb, P, scramble, R, T, R_out, T_out);
+    BANET_CUDA_LAUNCH_CHECK("pose_update_kernel launch");
+    return BANET_OK;
+}
+
+// lm_step with lambda given; with vmatrix_batch_scramble the step leaves R, T alone and pose_update_kernel updates them from every pair's step
+int lm_solve_update(const float* H, const float* g, const float* lambda, int nb, int K, const banet_solve_opts_t& opts,
+                    const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
+                    float* delta, int32_t* status, int status_accumulate, cudaStream_t st)
+{
+    const bool scramble = opts.vmatrix_batch_scramble != 0;
+    int rc = lm_step(H, g, nullptr, nb, 1, 0, K, nullptr, 1.f, lambda, kStepBundleNet, nullptr, opts, R, T, W, scramble ? nullptr : R_out, T_out,
+                     W_out, delta, nullptr, status, status_accumulate, st);
+    if (rc || !scramble) return rc;
+    return launch_pose_update(delta, nb, 6 + K, 1, R, T, R_out, T_out, st);
+}
+
+int lm_lambda(const float* rbar_sum, int nb, int N, int C, const float* mlp, float base, float* lambda_out, cudaStream_t st)
+{
+    const size_t smem = mlp_smem_bytes(C);
+    BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_lambda: C=%d too large", C);
+    cudaError_t e = cudaFuncSetAttribute(step_lambda_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { set_error("lm_lambda smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
+    step_lambda_kernel<<<nb, STEP_THREADS, smem, st>>>(rbar_sum, N, C, mlp, base, lambda_out);
+    BANET_CUDA_LAUNCH_CHECK("step_lambda_kernel launch");
+    return BANET_OK;
+}
+
 size_t lm_step_bwd_ws_floats(int C) { return mlp_ws_stride(C); }
 
 // Backward of lm_step (kStepBundleNet).  mlp == nullptr: lambda was given and only dlambda carries its gradient (drbar_sum, dmlp, ws unused).
+// ddelta_pose != nullptr: the first npose of the P = 6 + K unknowns are poses, their update backward done by the caller (lm_step_bwd_kernel).
 int lm_step_bwd(const float* H, const float* g, const float* rbar_sum, int nb, int N, int C, int K, const float* mlp, const float* lambda,
                 const float* delta, const banet_solve_opts_t& opts, const float* R, const float* T, const float* gRn, const float* gTn,
-                const float* gWn, float* dH, float* dg, float* drbar_sum, float* dmlp, float* dlambda, float* dR, float* dT, float* dW,
-                float* ws, cudaStream_t st)
+                const float* gWn, int npose, const float* ddelta_pose, float* dH, float* dg, float* drbar_sum, float* dmlp, float* dlambda,
+                float* dR, float* dT, float* dW, float* ws, cudaStream_t st)
 {
     const int P = 6 + K;
     const int ndamped = opts.undamped_last ? P - 1 : P;
-    const StepPlan plan = step_plan(P, C);
+    const StepPlan plan = step_plan(P, mlp ? C : 0);
     const size_t smem = plan.smem;
     BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_step_bwd: P=%d, C=%d do not fit shared memory", P, C);
     auto launch = [&](auto kern) -> int {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) { set_error("lm_step_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
-        kern<<<nb, STEP_THREADS, smem, st>>>(H, g, rbar_sum, N, C, mlp, lambda, delta, P, opts.damping_eps, ndamped, R, T, gRn, gTn, gWn,
-                                             dH, dg, drbar_sum, dlambda, dR, dT, dW, ws);
+        kern<<<nb, STEP_THREADS, smem, st>>>(H, g, rbar_sum, N, C, mlp, lambda, delta, P, npose, opts.damping_eps, ndamped, R, T, gRn, gTn, gWn,
+                                             ddelta_pose, dH, dg, drbar_sum, dlambda, dR, dT, dW, ws);
         return BANET_OK;
     };
     int rc;
@@ -333,6 +398,17 @@ int lm_step_bwd(const float* H, const float* g, const float* rbar_sum, int nb, i
         BANET_CUDA_LAUNCH_CHECK("lm_mlp_grad_kernel launch");
     }
     return BANET_OK;
+}
+
+// lm_step_bwd with lambda given
+int lm_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int K, const banet_solve_opts_t& opts,
+                        const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
+                        float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, cudaStream_t st)
+{
+    BANET_REQUIRE(!opts.vmatrix_batch_scramble, BANET_ERR_UNSUPPORTED,
+                  "lm_solve_update_bwd: the batch-interleaved VMatrix of bundlenet.py:45 is not differentiated (use vmatrix_batch_scramble=0)");
+    return lm_step_bwd(H, g, nullptr, nb, 1, 0, K, nullptr, lambda, delta, opts, R, T, gRn, gTn, gWn, 6, nullptr, dH, dg, nullptr, nullptr, dlambda,
+                       dR, dT, dW, nullptr, st);
 }
 
 }  // namespace banet

@@ -12,6 +12,19 @@ constexpr int STEP_THREADS = 1024;
 constexpr int STEP_WARPS = STEP_THREADS / 32;
 constexpr int STEP_NB = 4;                       // Cholesky panel width (the panel owners keep the NB x NB block in registers: 1024 threads leave 64 registers each)
 
+// Dynamic shared memory of a damped step (lm_step_kernel, lm_step_bwd_kernel, the arrow's kernels): [ union(A, MLP buffers) | vectors ].
+// A is the matrix of n unknowns with the right-hand side as row n (square with row pitch (n + 1) | 1, or packed), at offset 0.  The
+// lambda-MLP's buffers (step_lambda_mlp) share A's storage: the MLP finishes, with a block barrier, before A is loaded, and the step's
+// backward reuses them only after the factor is dead.  So the storage variant depends on the matrix and the vectors alone, and the MLP width
+// Cm (0 when lambda is given) only on whether the whole fits.
+__host__ __device__ __forceinline__ size_t mlp_smem_bytes(int Cm) { return Cm > 0 ? ((size_t)8 * Cm + (4 * Cm > 1024 ? 4 * Cm : 1024)) * sizeof(float) : 0; }
+__host__ __device__ __forceinline__ size_t step_matrix_elems(int n, bool full) { return full ? (size_t)(n + 1) * ((n + 1) | 1) : (size_t)(n + 1) * (n + 2) / 2; }
+__host__ __device__ __forceinline__ size_t step_vectors_offset(int n, bool full, size_t elem, int Cm)
+{
+    const size_t a = step_matrix_elems(n, full) * elem, m = mlp_smem_bytes(Cm);
+    return a > m ? a : m;
+}
+
 __device__ __forceinline__ float selu_s(float x) {
     const float alpha = 1.6732632423543772848170429916717f, scale = 1.0507009873554804934193349852946f;
     return scale * (x > 0.f ? x : alpha * expm1f(x));
@@ -267,7 +280,9 @@ __device__ __forceinline__ float solve_adjoint_outputs(const S* u, const S* dl, 
 }
 
 // R' = exp(w) R, T' = V(w) t + exp(w) T in double (bundlenet.py:269-275) for one pair: dl = (w, t), Rb [3,3], Tb [3] -> Ro, To (may alias).
-__device__ __forceinline__ void se3_update(const double* dl, const StepMode& mode, const float* Rb, const float* Tb, float* Ro, float* To)
+// skew: the skew matrix V is built from, when it is not the pair's own [w]x (the batch-interleaved one of bundlenet.py:45).
+__device__ __forceinline__ void se3_update(const double* dl, const StepMode& mode, const float* Rb, const float* Tb, float* Ro, float* To,
+                                           const double* skew = nullptr)
 {
     const double wx = dl[0], wy = dl[1], wz = dl[2], tx = dl[3], ty = dl[4], tz = dl[5];
     const double th_raw = sqrt(wx * wx + wy * wy + wz * wz);
@@ -279,7 +294,8 @@ __device__ __forceinline__ void se3_update(const double* dl, const StepMode& mod
     double ca, cb;                                               // VMatrix (bundlenet.py:39-46), series below 1e-4
     if (th_raw < 1e-4) { ca = 0.5 - th_raw * th_raw / 24.0; cb = 1.0 / 6.0 - th_raw * th_raw / 120.0; }
     else { ca = (1.0 - cos(th_raw)) / (th_raw * th_raw); cb = (th_raw - sin(th_raw)) / (th_raw * th_raw * th_raw); }
-    const double sk[9] = {0, -wz, wy, wz, 0, -wx, -wy, wx, 0};
+    const double own[9] = {0, -wz, wy, wz, 0, -wx, -wy, wx, 0};
+    const double* sk = skew ? skew : own;
     double V[9];
     for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) {
         const double sk2 = sk[i * 3] * sk[j] + sk[i * 3 + 1] * sk[3 + j] + sk[i * 3 + 2] * sk[6 + j];

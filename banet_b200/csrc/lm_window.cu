@@ -14,7 +14,7 @@
 // updated with its own 6 entries (:269-275), W with the shared K.  The solve is the fused lm_step kernel on the one (6 nf + K) system.
 //
 // Training: lm_window_step with lambda given is banet_lm_window_solve_update; lm_window_step_bwd is its backward: the per-frame SE(3) update
-// backward, the solve backward of lm_bwd.cu on the re-assembled system (its first 6 nf unknowns are poses), and the adjoint of the assembly.
+// backward, lm_step's backward on the re-assembled system (its first 6 nf unknowns are poses), and the adjoint of the assembly.
 #include "common.cuh"
 #include "lm_build.h"
 
@@ -142,7 +142,7 @@ int lm_window_step(const float* H, const float* g, const float* rbar_sum, int nf
         cudaError_t e = cudaMemcpyAsync(lambda_out, lam, sizeof(float), cudaMemcpyDeviceToDevice, st);
         if (e != cudaSuccess) { set_error("lm_window_step: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
     }
-    return launch_pose_update(delta_j, nf, 6, R, T, R_out, T_out, st);        // frame f's six entries are delta_j[6f, 6f+6)
+    return launch_pose_update(delta_j, nf, 6, 0, R, T, R_out, T_out, st);        // frame f's six entries are delta_j[6f, 6f+6)
 }
 
 size_t lm_window_step_bwd_workspace_floats(int nf, int K)
@@ -152,9 +152,9 @@ size_t lm_window_step_bwd_workspace_floats(int nf, int K)
 }
 
 // Backward of one window step (lambda given): with ddelta = [pose part from the per-frame SE(3) update backward | dW'], u = Ht_j^-1 ddelta
-// on the re-assembled damped system gives dHj = -u delta_j^T (+ the damping terms), dgj = u and dlambda (lm_solve_bwd_kernel, npose = 6 nf);
-// the assembly's adjoint maps (dHj, dgj) to the pairs.  dW = dW' (W' = W + delta_d).  The solve backward factors in the precision lm_step
-// chose for the forward (lambda given), and the assembled gj goes with it: a window whose forward was skipped gets zero dH, dg, dlambda.
+// on the re-assembled damped system gives dHj = -u delta_j^T (+ the damping terms), dgj = u and dlambda (lm_step_bwd, npose = 6 nf);
+// the assembly's adjoint maps (dHj, dgj) to the pairs.  dW = dW' (W' = W + delta_d).  lm_step_bwd factors with the forward's kernel code and
+// storage, and the assembled gj goes with it: a window whose forward was skipped gets zero dH, dg, dlambda.
 int lm_window_step_bwd(const float* H, const float* g, const float* lambda, const float* delta_j, int nf, int K, const banet_solve_opts_t& opts,
                        const float* R, const float* T, const float* gRn, const float* gTn, const float* gWn,
                        float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, float* ws, cudaStream_t st)
@@ -166,7 +166,8 @@ int lm_window_step_bwd(const float* H, const float* g, const float* lambda, cons
     BANET_CUDA_LAUNCH_CHECK("window_assemble_kernel launch");
     int rc = launch_pose_update_bwd(delta_j, nf, 6, R, T, gRn, gTn, dgj, dR, dT, st);                   // ddelta[0:6 nf] -> dgj
     if (rc) return rc;
-    rc = launch_solve_bwd(Hj, gj, lambda, delta_j, 1, Pj, 6 * nf, lm_step_uses_double(Pj, 1), opts, gWn, dHj, dgj, dlambda, dW, st);
+    rc = lm_step_bwd(Hj, gj, nullptr, 1, 1, 0, Pj - 6, nullptr, lambda, delta_j, opts, nullptr, nullptr, nullptr, nullptr, gWn, 6 * nf, dgj, dHj, dgj,
+                     nullptr, nullptr, dlambda, nullptr, nullptr, dW, nullptr, st);
     if (rc) return rc;
     window_assemble_bwd_kernel<<<64, 256, 0, st>>>(dHj, dgj, nf, K, dH, dg);
     BANET_CUDA_LAUNCH_CHECK("window_assemble_bwd_kernel launch");

@@ -11,7 +11,8 @@
 //   D. per frame, warp per frame:     x_f = Ht_cc,f^-1 (r_f - Hcd_f x_d)
 //
 // Only S (and one frame's Y) lives in shared memory: nothing limits nf but the workspace, which holds each frame's L_f, z_f and x_f
-// (ARROW_FRAME_DOUBLES doubles).  S is double while it fits shared memory (square, then packed, as lm_step chooses for its own matrix), else float.
+// (ARROW_FRAME_DOUBLES doubles).  S is double while it fits shared memory (square to K = 154, then packed to 215, by lm_step's rule for its
+// own matrix), else float (to K = 256); the lambda-MLP's buffers share S's storage (lm_step.cuh).
 // No atomics: every sum over frames runs in frame order inside one thread, so the step is bit-reproducible and independent of the workspace's
 // previous contents.
 //
@@ -46,14 +47,9 @@ struct ArrowParams {
     double* fws;                             // [nw, nf, ARROW_FRAME_DOUBLES]
 };
 
-// Shared memory of one window: S's lower triangle + right-hand-side row (square or packed) | x_d [K] | 1/diag [K] | dots [STEP_NB] |
-// Y_f [6][K] | sum_f diag Hdd_f [K]  (all S) | lambda-MLP buffers (floats; forward with the MLP only)
-size_t arrow_smem(int K, int C, bool use_double, bool full)
-{
-    const size_t nA = full ? (size_t)(K + 1) * ((K + 1) | 1) : (size_t)(K + 1) * (K + 2) / 2;
-    const size_t mlp = C > 0 ? ((size_t)8 * C + (4 * C > 1024 ? 4 * C : 1024)) * sizeof(float) : 0;
-    return (nA + 9 * (size_t)K + STEP_NB) * (use_double ? sizeof(double) : sizeof(float)) + mlp;
-}
+// Shared memory of one window: union(S's lower triangle + right-hand-side row (square or packed), lambda-MLP buffers (forward with the MLP
+// only)) | x_d [K] | 1/diag [K] | dots [STEP_NB] | Y_f [6][K] | sum_f diag Hdd_f [K]  (all S but the MLP's floats)
+constexpr int arrow_vector_elems(int K) { return 9 * K + STEP_NB; }
 
 // Phases A-D above for window w with right-hand side r: pose part rhs_pose[(w nf + f) P + m] (row stride P), depth part rhs_d0 [K] (or 0)
 // plus, per frame, rhs_d_frames[(w nf + f) P + 6 + k] (or nothing).  check_rhs: non-finite right-hand sides set status bit 2; bad_in != 0
@@ -234,9 +230,9 @@ window_arrow_step_kernel(const ArrowParams p)
     extern __shared__ __align__(16) unsigned char smraw[];
     const int K = p.K, nf = p.nf, Pj = 6 * nf + K;
     S* A = reinterpret_cast<S*>(smraw);
-    const size_t nA = FULL ? (size_t)(K + 1) * ((K + 1) | 1) : (size_t)(K + 1) * (K + 2) / 2;
-    S* xs = A + nA; S* dinv = xs + K; S* dots = dinv + K; S* Y = dots + STEP_NB; S* dsum = Y + 6 * K;
-    float* mbuf = reinterpret_cast<float*>(dsum + K);
+    float* mbuf = reinterpret_cast<float*>(smraw);
+    S* xs = reinterpret_cast<S*>(smraw + step_vectors_offset(K, FULL, sizeof(S), p.lambda_in ? 0 : p.C));
+    S* dinv = xs + K; S* dots = dinv + K; S* Y = dots + STEP_NB; S* dsum = Y + 6 * K;
     __shared__ int s_flag;
     __shared__ float s_wpart[STEP_WARPS], s_lam;
     const int w = blockIdx.x, tid = threadIdx.x;
@@ -290,8 +286,8 @@ window_arrow_step_bwd_kernel(const ArrowParams p)
     extern __shared__ __align__(16) unsigned char smraw[];
     const int K = p.K, nf = p.nf, P = 6 + K, Pj = 6 * nf + K;
     S* A = reinterpret_cast<S*>(smraw);
-    const size_t nA = FULL ? (size_t)(K + 1) * ((K + 1) | 1) : (size_t)(K + 1) * (K + 2) / 2;
-    S* xs = A + nA; S* dinv = xs + K; S* dots = dinv + K; S* Y = dots + STEP_NB; S* dsum = Y + 6 * K;
+    S* xs = reinterpret_cast<S*>(smraw + step_matrix_elems(K, FULL) * sizeof(S));
+    S* dinv = xs + K; S* dots = dinv + K; S* Y = dots + STEP_NB; S* dsum = Y + 6 * K;
     __shared__ int s_flag;
     __shared__ double s_dl[STEP_WARPS];
     const int w = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -355,14 +351,17 @@ window_arrow_step_bwd_kernel(const ArrowParams p)
     }
 }
 
-// smem size and kernel variant for K unknowns of depth and C MLP channels (0: lambda given), the choice lm_step makes for its own matrix
+// kernel variant for K unknowns of depth, from the matrix and the vectors alone (the rule lm_step applies to its own matrix), and smem with
+// the buffers of an MLP of width Cm (0: lambda given)
 struct ArrowPlan { bool use_double, full; size_t smem; };
-ArrowPlan arrow_plan(int K, int C)
+ArrowPlan arrow_plan(int K, int Cm)
 {
+    auto bytes = [&](bool dbl, bool full) { return (step_matrix_elems(K, full) + arrow_vector_elems(K)) * (dbl ? sizeof(double) : sizeof(float)); };
     ArrowPlan pl;
-    pl.full = arrow_smem(K, C, true, true) <= 200 * 1024;
-    pl.use_double = pl.full || arrow_smem(K, C, true, false) <= 200 * 1024;
-    pl.smem = arrow_smem(K, C, pl.use_double, pl.full);
+    pl.full = bytes(true, true) <= 200 * 1024;
+    pl.use_double = pl.full || bytes(true, false) <= 200 * 1024;
+    const size_t elem = pl.use_double ? sizeof(double) : sizeof(float);
+    pl.smem = step_vectors_offset(K, pl.full, elem, Cm) + arrow_vector_elems(K) * elem;
     return pl;
 }
 

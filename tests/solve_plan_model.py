@@ -1,77 +1,55 @@
 """CPU restatement of how the damped-solve kernels choose their shared-memory storage (no GPU, no library).
 
-Each solver keeps its matrix in shared memory and picks, by size, square fp64 (FULL), packed fp64 or packed fp32 storage, or rejects the
-size with BANET_ERR_UNSUPPORTED (-4).  The rules below restate lm_step_smem / lm_step (lm_step.cu), arrow_smem / arrow_plan
-(lm_window_batch.cu), lm_solve_uses_double / lm_solve_update (lm_solve.cu) and solve_bwd_floats / launch_solve_bwd (lm_bwd.cu).
-tests/test_solve_edges.py ties the rejection edges to the built library and runs every variant on the GPU at the sizes generated here.
+There are two solvers, each keeping its matrix in shared memory: lm_step_kernel (lm_step.cu; with its backward it is also banet_lm_solve_update,
+its backward, and the dense keyframe window in both directions) and the arrow's window_arrow_step(_bwd)_kernel (lm_window_batch.cu).  Each
+picks, by size, square fp64 (FULL), packed fp64 or packed fp32 storage, or rejects the size with BANET_ERR_UNSUPPORTED (-4).  The rules
+below restate step_plan (lm_step.cu), arrow_plan (lm_window_batch.cu) and lm_lambda.  tests/test_solve_edges.py ties the rejection edges
+to the built library and runs every variant on the GPU at the sizes generated here.
 
-C is the lambda-MLP width; the MLP buffers share the solver's shared memory, so C moves the switches.  Where lambda is given:
-  * banet_lm_step and the dense window pass C = 1 (lm_step_smem still reserves max(4C, 1024) floats of slice partials);
-  * the arrow (banet_lm_window_batch_solve_update and its backward) reserves nothing: Cm = 0.
+The storage variant depends on the matrix and its vectors alone.  The lambda-MLP's buffers share the matrix's storage (lm_step.cuh), so the
+MLP width C (0 when lambda is given) enters only the rejection: shared memory is vectors + max(matrix, MLP buffers).
 """
 STEP_NB = 4
 KB = 1024
 SQUARE64, PACKED64, PACKED32, REJECT = "square_fp64", "packed_fp64", "packed_fp32", "rejected"
+MLP_ONLY = "mlp_only"
 
 
-def _mlp_bytes(C):
-    return (8 * C + max(4 * C, 1024)) * 4
+def mlp_bytes(C):
+    return (8 * C + max(4 * C, 1024)) * 4 if C > 0 else 0
 
 
-def lm_step_smem(P, C, dbl, full):
-    nA = ((P + 1) * ((P + 1) | 1) if full else (P + 1) * (P + 2) // 2) + 2 * P + STEP_NB
-    return nA * (8 if dbl else 4) + _mlp_bytes(C)
+def _matrix(n, full):
+    return (n + 1) * ((n + 1) | 1) if full else (n + 1) * (n + 2) // 2
 
 
-def lm_step_plan(P, C):
-    """lm_step_kernel<S, FULL> for P = 6 + K unknowns (or the dense window's 6 nf + K) at MLP width C (1 when lambda is given)."""
-    if lm_step_smem(P, C, True, True) <= 200 * KB:
-        return SQUARE64
-    if lm_step_smem(P, C, True, False) <= 200 * KB:
-        return PACKED64
-    return PACKED32 if lm_step_smem(P, C, False, False) <= 220 * KB else REJECT
+def _plan(n, vectors, C):
+    """The variant of a matrix of n unknowns with `vectors` elements of its type beside it, or REJECT."""
+    if (_matrix(n, True) + vectors) * 8 <= 200 * KB:
+        full, elem, variant = True, 8, SQUARE64
+    elif (_matrix(n, False) + vectors) * 8 <= 200 * KB:
+        full, elem, variant = False, 8, PACKED64
+    else:
+        full, elem, variant = False, 4, PACKED32
+    return variant if max(_matrix(n, full) * elem, mlp_bytes(C)) + vectors * elem <= 220 * KB else REJECT
 
 
-def arrow_smem(K, C, dbl, full):
-    nA = (K + 1) * ((K + 1) | 1) if full else (K + 1) * (K + 2) // 2
-    return (nA + 9 * K + STEP_NB) * (8 if dbl else 4) + (_mlp_bytes(C) if C > 0 else 0)
+def step_plan(P, C=0):
+    """lm_step_kernel / lm_step_bwd_kernel <S, FULL> for P = 6 + K unknowns (or the dense window's 6 nf + K); C: the MLP width, 0 when
+    lambda is given."""
+    return _plan(P, 2 * P + STEP_NB, C)
 
 
-def arrow_plan(K, C):
-    """window_arrow_step_kernel / window_arrow_step_bwd_kernel <S, FULL> at depth size K; C = 0 when lambda is given (and in the backward)."""
+def arrow_plan(K, C=0):
+    """window_arrow_step_kernel / window_arrow_step_bwd_kernel <S, FULL> at depth size K; C: the MLP width, 0 when lambda is given."""
     if K < 1 or K > 256:
         return REJECT
-    if arrow_smem(K, C, True, True) <= 200 * KB:
-        return SQUARE64
-    if arrow_smem(K, C, True, False) <= 200 * KB:
-        return PACKED64
-    return PACKED32 if arrow_smem(K, C, False, False) <= 220 * KB else REJECT
+    return _plan(K, 9 * K + STEP_NB, C)
 
 
-def lm_solve_plan(P):
-    """lm_solve_kernel<S> (banet_lm_solve_update, the pair training forward): packed only."""
-    n = P * (P + 1) // 2 + 2 * P
-    if n * 8 <= 200 * KB:
-        return PACKED64
-    return PACKED32 if n * 4 <= 220 * KB else REJECT
-
-
-def solve_bwd_plan(P, forward_plan):
-    """lm_solve_bwd_kernel<S>: factors in the precision its forward used (forward_plan = that forward's plan at the same P)."""
-    n = P * (P + 1) // 2 + 3 * P
-    if n * 4 > 220 * KB or forward_plan == REJECT:
-        return REJECT
-    return PACKED64 if forward_plan in (SQUARE64, PACKED64) else PACKED32
-
-
-def pair_bwd_plan(P):
-    """banet_lm_solve_update_bwd: the backward of lm_solve_update."""
-    return solve_bwd_plan(P, lm_solve_plan(P))
-
-
-def dense_window_bwd_plan(Pj):
-    """banet_lm_window_solve_update_bwd: the backward of lm_step with lambda given on the assembled window (C = 1)."""
-    return solve_bwd_plan(Pj, lm_step_plan(Pj, 1))
+def lambda_plan(C):
+    """banet_lm_lambda: the MLP's buffers alone."""
+    return MLP_ONLY if mlp_bytes(C) <= 220 * KB else REJECT
 
 
 def switches(plan, lo, hi):
@@ -85,19 +63,25 @@ def switches(plan, lo, hi):
     return out
 
 
-# every kernel and every C that moves its switches: name -> (plan of the size, the range searched)
+# every C-ABI entry with a size edge: name -> (plan of the size, the range searched).  The size is P = 6 + K (the dense window's 6 nf + K),
+# the arrow's K, or, for the *_width entries, the MLP width C.
 PLANS = {
-    "lm_step_lambda_given": (lambda P: lm_step_plan(P, 1), (7, 400)),
-    "lm_step_mlp_C5": (lambda P: lm_step_plan(P, 5), (7, 400)),
-    "lm_step_mlp_C128": (lambda P: lm_step_plan(P, 128), (7, 400)),
-    "lm_step_mlp_C256": (lambda P: lm_step_plan(P, 256), (7, 400)),
-    "arrow_lambda_given": (lambda K: arrow_plan(K, 0), (1, 300)),
+    "lm_step_lambda_given": (lambda P: step_plan(P), (7, 400)),
+    "lm_step_mlp_C5": (lambda P: step_plan(P, 5), (7, 400)),
+    "lm_step_mlp_C128": (lambda P: step_plan(P, 128), (7, 400)),
+    "lm_step_mlp_C256": (lambda P: step_plan(P, 256), (7, 400)),
+    "lm_step_width_P7": (lambda C: step_plan(7, C), (1, 6000)),
+    "lm_step_width_P262": (lambda C: step_plan(262, C), (1, 6000)),
+    "lm_lambda_width": (lambda_plan, (1, 6000)),
+    "lm_solve": (lambda P: step_plan(P), (7, 400)),
+    "lm_solve_bwd_pairs": (lambda P: step_plan(P), (7, 400)),
+    "dense_window": (lambda P: step_plan(P), (7, 400)),
+    "lm_solve_bwd_dense_window": (lambda P: step_plan(P), (7, 400)),
+    "arrow_lambda_given": (lambda K: arrow_plan(K), (1, 300)),
+    "arrow_bwd": (lambda K: arrow_plan(K), (1, 300)),
     "arrow_mlp_C5": (lambda K: arrow_plan(K, 5), (1, 300)),
     "arrow_mlp_C128": (lambda K: arrow_plan(K, 128), (1, 300)),
     "arrow_mlp_C256": (lambda K: arrow_plan(K, 256), (1, 300)),
-    "lm_solve": (lm_solve_plan, (7, 400)),
-    "lm_solve_bwd_pairs": (pair_bwd_plan, (7, 400)),
-    "lm_solve_bwd_dense_window": (dense_window_bwd_plan, (7, 400)),
 }
 
 
