@@ -21,6 +21,9 @@ void set_error(const char* fmt, ...);
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 constexpr int kMaxSMs = 132;          // H100 SXM
+constexpr int kMaxGridY = 65535;      // gridDim.y limit: launches with the batch on y stride over it (blockIdx.y, += gridDim.y)
+
+static inline unsigned grid_y(long long n) { return (unsigned)(n < kMaxGridY ? n : kMaxGridY); }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -291,11 +291,10 @@ lm_build_kernel(const BuildParams prm)
 }
 
 // ---- deterministic reduction of the partial slots -> H, g, rbar_sum, nvalid ----------------------
-__global__ void __launch_bounds__(256)
-lm_reduce_kernel(const BuildParams prm, int grid_build, float* __restrict__ H, float* __restrict__ g,
-                 float* __restrict__ rbar_sum, float* __restrict__ nvalid)
+__device__ __forceinline__ void lm_reduce_pair(const BuildParams& prm, int grid_build, int b, float* __restrict__ H, float* __restrict__ g,
+                                               float* __restrict__ rbar_sum, float* __restrict__ nvalid)
 {
-    const int b = blockIdx.y, K = prm.K, C = prm.C, P = 6 + K;
+    const int K = prm.K, C = prm.C, P = 6 + K;
     const SlotLayout L{K, C};
     const long long p0 = (long long)b * prm.tiles_per_pair, p1 = p0 + prm.tiles_per_pair;
     __shared__ const float* s_slot[kMaxSlots];
@@ -336,11 +335,23 @@ lm_reduce_kernel(const BuildParams prm, int grid_build, float* __restrict__ H, f
     }
 }
 
+// One pair per blockIdx.y, striding by gridDim.y when the batch has more pairs than the y dimension allows.  Each element keeps its
+// one summation order over the pair's slots, so the result does not depend on the stride.
+__global__ void __launch_bounds__(256)
+lm_reduce_kernel(const BuildParams prm, int grid_build, float* __restrict__ H, float* __restrict__ g,
+                 float* __restrict__ rbar_sum, float* __restrict__ nvalid)
+{
+    for (int b = blockIdx.y; b < prm.nb; b += gridDim.y) {
+        lm_reduce_pair(prm, grid_build, b, H, g, rbar_sum, nvalid);
+        __syncthreads();                                    // every thread is done with this pair's slot list
+    }
+}
+
 int launch_lm_reduce(const BuildParams& prm, int grid_build, float* H, float* g, float* rbar_sum, float* nvalid, cudaStream_t st)
 {
     const int nel = prm.K * prm.K + 7 * prm.K + 32 + prm.C;
     int chunks = (nel + 2047) / 2048; if (chunks < 1) chunks = 1; if (chunks > 16) chunks = 16;
-    lm_reduce_kernel<<<dim3(chunks, prm.nb), 256, 0, st>>>(prm, grid_build, H, g, rbar_sum, nvalid);
+    lm_reduce_kernel<<<dim3(chunks, grid_y(prm.nb)), 256, 0, st>>>(prm, grid_build, H, g, rbar_sum, nvalid);
     BANET_CUDA_LAUNCH_CHECK("lm_reduce_kernel launch");
     return BANET_OK;
 }

@@ -316,11 +316,10 @@ keyframe_build_kernel(const KeyParams prm)
 }
 
 // ---- fixed-order fp64 reduction of the slots of each window -> the window-reduced per-pair system ----------------------------------
-__global__ void __launch_bounds__(256)
-keyframe_reduce_kernel(const KeyParams prm, int grid_build, float* __restrict__ H, float* __restrict__ g, float* __restrict__ rbar_sum,
-                       float* __restrict__ nvalid)
+__device__ __forceinline__ void keyframe_reduce_window(const KeyParams& prm, int grid_build, int wi, float* __restrict__ H, float* __restrict__ g,
+                                                       float* __restrict__ rbar_sum, float* __restrict__ nvalid)
 {
-    const int wi = blockIdx.y, K = prm.K, C = prm.C, nf = prm.nf, P = 6 + K;
+    const int K = prm.K, C = prm.C, nf = prm.nf, P = 6 + K;
     const KeySlot L{K, C};
     const long long p0 = (long long)wi * prm.tiles_per_win, p1 = p0 + prm.tiles_per_win;
     __shared__ const float* s_slot[kMaxSlots];
@@ -370,6 +369,18 @@ keyframe_reduce_kernel(const KeyParams prm, int grid_build, float* __restrict__ 
         } else {
             rbar_sum[b * C + (e - 7 * K - 28)] = v;
         }
+    }
+}
+
+// One window per blockIdx.y, striding by gridDim.y when there are more windows than the y dimension allows.  Each element keeps its one
+// summation order over the window's slots, so the result does not depend on the stride.
+__global__ void __launch_bounds__(256)
+keyframe_reduce_kernel(const KeyParams prm, int grid_build, float* __restrict__ H, float* __restrict__ g, float* __restrict__ rbar_sum,
+                       float* __restrict__ nvalid)
+{
+    for (int wi = blockIdx.y; wi < prm.nw; wi += gridDim.y) {
+        keyframe_reduce_window(prm, grid_build, wi, H, g, rbar_sum, nvalid);
+        __syncthreads();                                              // every thread is done with this window's slot list
     }
 }
 
@@ -663,7 +674,7 @@ int keyframe_build(const banet_keyframe_level_t* lv, const KeyframePlan& plan, c
     if (rc != BANET_OK) return rc;
     const long long nel = (long long)lv->K * lv->K + (long long)lv->nf * (7 * lv->K + 28 + lv->C);
     int chunks = (int)((nel + 2047) / 2048); if (chunks < 1) chunks = 1; if (chunks > 32) chunks = 32;
-    keyframe_reduce_kernel<<<dim3(chunks, lv->nw), 256, 0, st>>>(prm, plan.grid, H, g, rbar_sum, nvalid);
+    keyframe_reduce_kernel<<<dim3(chunks, grid_y(lv->nw)), 256, 0, st>>>(prm, plan.grid, H, g, rbar_sum, nvalid);
     BANET_CUDA_LAUNCH_CHECK("keyframe_reduce_kernel launch");
     return BANET_OK;
 }

@@ -178,33 +178,37 @@ __global__ void resample_bwd_kernel(const float* __restrict__ dout, const float*
 }
 
 // Backward of depth_compose: dinit = dout; dbasis[pt][k] = dout[pt] W[k]; dW[k] += sum_pt dout[pt] basis[pt][k] (atomics; dW zero-filled).
+// One batch entry per blockIdx.y, striding by gridDim.y when nb exceeds the y dimension's limit.
 template <typename TB>
 __global__ void depth_compose_bwd_kernel(const float* __restrict__ dout, const TB* __restrict__ basis, const float* __restrict__ W,
                                          int nb, int M, int K, float* __restrict__ dbasis, float* __restrict__ dW)
 {
-    const int b = blockIdx.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
     extern __shared__ float sacc[];              // [K]
-    for (int k = threadIdx.x; k < K; k += blockDim.x) sacc[k] = 0.f;
-    __syncthreads();
     const int per = (M + gridDim.x - 1) / gridDim.x;
     const int m0 = blockIdx.x * per, m1 = min(M, m0 + per);
-    for (int k0 = 0; k0 < K; k0 += 32) {
-        const int k = k0 + lane;
-        const float wk = k < K ? W[(size_t)b * K + k] : 0.f;
-        float acc = 0.f;
-        for (int m = m0 + warp; m < m1; m += nw) {
-            const size_t pt = (size_t)b * M + m;
-            const float gv = dout[pt];
-            if (k < K) {
-                float bv;
-                if constexpr (sizeof(TB) == 4) bv = basis[pt * K + k]; else bv = ldg_feat(basis + pt * K + k);
-                acc = fmaf(gv, bv, acc); dbasis[pt * K + k] = gv * wk;
+    for (int b = blockIdx.y; b < nb; b += gridDim.y) {
+        for (int k = threadIdx.x; k < K; k += blockDim.x) sacc[k] = 0.f;
+        __syncthreads();
+        for (int k0 = 0; k0 < K; k0 += 32) {
+            const int k = k0 + lane;
+            const float wk = k < K ? W[(size_t)b * K + k] : 0.f;
+            float acc = 0.f;
+            for (int m = m0 + warp; m < m1; m += nw) {
+                const size_t pt = (size_t)b * M + m;
+                const float gv = dout[pt];
+                if (k < K) {
+                    float bv;
+                    if constexpr (sizeof(TB) == 4) bv = basis[pt * K + k]; else bv = ldg_feat(basis + pt * K + k);
+                    acc = fmaf(gv, bv, acc); dbasis[pt * K + k] = gv * wk;
+                }
             }
+            if (k < K) atomicAdd(&sacc[k], acc);
         }
-        if (k < K) atomicAdd(&sacc[k], acc);
+        __syncthreads();
+        for (int k = threadIdx.x; k < K; k += blockDim.x) atomicAdd(dW + (size_t)b * K + k, sacc[k]);
+        __syncthreads();                         // sacc is cleared again for the next entry
     }
-    __syncthreads();
-    for (int k = threadIdx.x; k < K; k += blockDim.x) atomicAdd(dW + (size_t)b * K + k, sacc[k]);
 }
 
 }  // namespace banet
@@ -240,7 +244,7 @@ int depth_compose_bwd(const float* dout, const TB* basis, const float* W, int nb
     BANET_REQUIRE(dout && basis && W && dbasis && dW && nb > 0 && M > 0 && K > 0 && K <= 8192, BANET_ERR_BAD_ARG, "%s: bad argument", who);
     cudaMemsetAsync(dW, 0, (size_t)nb * K * sizeof(float), st);
     int gx = (M + 1023) / 1024; if (gx < 1) gx = 1; if (gx > 64) gx = 64;
-    depth_compose_bwd_kernel<TB><<<dim3(gx, nb), 256, K * sizeof(float), st>>>(dout, basis, W, nb, M, K, dbasis, dW);
+    depth_compose_bwd_kernel<TB><<<dim3(gx, grid_y(nb)), 256, K * sizeof(float), st>>>(dout, basis, W, nb, M, K, dbasis, dW);
     BANET_CUDA_LAUNCH_CHECK(who);
     return BANET_OK;
 }
