@@ -14,20 +14,22 @@ LIB_PATH = os.environ.get("BANET_LIB_PATH") or os.path.join(_HERE, "libbanet.so"
 BANET_OK = 0
 PREC_AUTO, PREC_FP32_SIMT, PREC_TF32X1, PREC_TF32X2, PREC_TF32X3, PREC_TF32_LEVELWISE = -1, 0, 1, 2, 3, 4
 DTYPE_F32, DTYPE_BF16 = 0, 1          # banet_level_t::feature_dtype (conv1 and conv2) and ::basis_dtype (B)
+ROBUST_NONE, ROBUST_HUBER, ROBUST_CAUCHY = 0, 1, 2     # banet_level_t::robust
 
 c_float_p = C.c_void_p      # raw device pointers
 c_stream = C.c_void_p
 
 
 class BanetLevel(C.Structure):
-    """struct banet_level (include/banet_abi.h).  feature_dtype, basis_dtype and weight are last, so a struct built without them keeps
-    fp32 features, an fp32 basis and no point weights."""
+    """struct banet_level (include/banet_abi.h).  feature_dtype, basis_dtype, weight, robust and robust_scale are last, so a struct built
+    without them keeps fp32 features, an fp32 basis, no point weights and the plain squared loss."""
     _fields_ = [("nb", C.c_int), ("N", C.c_int), ("C", C.c_int), ("K", C.c_int),
                 ("h", C.c_int), ("w", C.c_int), ("conv2_channels", C.c_int),
                 ("conv1", C.c_void_p), ("conv2", C.c_void_p), ("intr", C.c_void_p),
                 ("p", C.c_void_p), ("D", C.c_void_p), ("B", C.c_void_p),
                 ("grid_w", C.c_int), ("grid_h", C.c_int), ("feature_dtype", C.c_int),
-                ("basis_dtype", C.c_int), ("weight", C.c_void_p)]
+                ("basis_dtype", C.c_int), ("weight", C.c_void_p),
+                ("robust", C.c_int), ("robust_scale", C.c_float)]
 
 
 class BanetKeyframeLevel(C.Structure):

@@ -141,17 +141,18 @@ def iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_b
 class _LMBuildFn(torch.autograd.Function):
     """(H, g, rbar_sum) = banet_lm_build(...); backward = banet_lm_build_bwd.  conv2 is the [F2|gx|gy] tensor or F2 only; dconv2 comes back
     in conv2's layout.  bfloat16 features and a bfloat16 basis are saved as they are; their gradients are accumulated in fp32 by the kernel
-    and cast once.  weight [nb,N,1] (or None): the per-point weight of H and g; its gradient is banet_lm_build_bwd_weighted's dweight."""
+    and cast once.  weight [nb,N,1] (or None): the per-point weight of H and g; its gradient is banet_lm_build_bwd_weighted's dweight.
+    robust, robust_scale: the level's robust loss (ops.Level), constants; the backward differentiates its IRLS weight through the residual."""
 
     @staticmethod
-    def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, precision, exact_sym, grid, weight):
-        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=grid, weight=weight)
+    def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, precision, exact_sym, grid, weight, robust=None, robust_scale=0.0):
+        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=grid, weight=weight, robust=robust, robust_scale=robust_scale)
         H, g, rbar, nvalid = ops.lm_build(lv, R, T, W, precision)
         empty = conv1.new_empty(0)
         ctx.save_for_backward(conv1, conv2, D, B if B is not None else empty, R, T, W if W is not None else empty, intr, p,
                               weight if weight is not None else empty)
         ctx.has_basis = B is not None; ctx.has_weight = weight is not None
-        ctx.exact_sym = bool(exact_sym); ctx.grid = grid
+        ctx.exact_sym = bool(exact_sym); ctx.grid = grid; ctx.robust = (robust, robust_scale)
         ctx.mark_non_differentiable(nvalid)
         return H, g, rbar, nvalid
 
@@ -162,7 +163,7 @@ class _LMBuildFn(torch.autograd.Function):
             B = None; W = None
         if not ctx.has_weight:
             weight = None
-        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=ctx.grid, weight=weight)
+        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=ctx.grid, weight=weight, robust=ctx.robust[0], robust_scale=ctx.robust[1])
         nb = conv1.shape[0]
         P = 6 + (0 if B is None else B.shape[2])
         dH = dH.contiguous() if dH is not None else torch.zeros(nb, P, P, device=conv1.device)
@@ -173,7 +174,7 @@ class _LMBuildFn(torch.autograd.Function):
         dconv1, dconv2, dD, dB, dR, dT, dW = grads[:7]
         dweight = grads[7] if want_dw else None
         dB = None if dB is None else dB.to(B.dtype)
-        return dconv1.to(conv1.dtype), dconv2.to(conv2.dtype), dD, dB, dR, dT, dW, None, None, None, None, None, dweight
+        return dconv1.to(conv1.dtype), dconv2.to(conv2.dtype), dD, dB, dR, dT, dW, None, None, None, None, None, dweight, None, None
 
 
 class _KeyframeBuildFn(torch.autograd.Function):
@@ -282,7 +283,8 @@ def lm_run(levels: Sequence[ops.Level], iters_per_level: int, R: Tensor, T: Tens
     """Differentiable ops.lm_run: per level and iteration, the build (_LMBuildFn, the level's precision resolved as banet_lm_run resolves it)
     and the fused step (_LMStepFn: lambda-MLP, damping, solve, update in one launch), W carried across levels.  The forward runs
     ops.lm_run's kernels in its order and returns its bits.  Gradients reach every level's conv1, conv2, D, B and weight, R, T, W and each
-    level's lambda-MLP (filters, biases); intr and p are constants, as in iteration_fused.
+    level's lambda-MLP (filters, biases); intr and p are constants, as in iteration_fused.  A level's robust loss (robust, robust_scale) is
+    honoured as ops.lm_run honours it.
     mlp_params[l]: level l's [(filters [cin,cout], biases [cout])] x 5, used unless lambda_fixed is given (then lambda = lambda_fixed for every
     pair).  l2_regularizer_base None: 1000 with a depth basis, 1 pose-only (ops.lm_run's default).  Where banet_lm_run would leave the fused
     step for its three-kernel path ((K, C) beyond banet_lm_step's shared memory) this raises: it has no second path.
@@ -306,7 +308,7 @@ def lm_run(levels: Sequence[ops.Level], iters_per_level: int, R: Tensor, T: Tens
             mlp, lam = [], torch.full((nb,), float(lambda_fixed), device=R.device, dtype=torch.float32)
         for _ in range(iters_per_level):
             H, g, rbar, _nvalid = _LMBuildFn.apply(lv.conv1, lv.conv2, lv.D, lv.B, R, T, W, lv.intr.detach(), lv.p.detach(), precision, exact_sym,
-                                                   lv.grid, lv.weight)
+                                                   lv.grid, lv.weight, lv.robust, lv.robust_scale)
             out = _LMStepFn.apply(H, g, rbar, lam, R, T, W, Nl, l2_regularizer_base, damping_eps, K > 0, *mlp)
             if W is None:
                 R, T, st = out
@@ -423,16 +425,19 @@ def depth_compose(init_depth: Tensor, basis: Tensor, W: Tensor) -> Tensor:
 
 def iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base: Optional[float],
                     damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None,
-                    precision: int = 0, grid=None, return_status: bool = False, weight: Optional[Tensor] = None):
+                    precision: int = 0, grid=None, return_status: bool = False, weight: Optional[Tensor] = None,
+                    robust: Optional[str] = None, robust_scale: float = 0.0):
     """One differentiable LM iteration on the fused kernels.  Same arguments / returns as `iteration`; an F2-only conv2 [nb,h,w,C] goes
     straight into the build and its backward (the gradient stencil's adjoint runs inside banet_lm_build_bwd).
     precision: contraction mode of the FORWARD build (the backward is fp32); default FP32_SIMT, the reference's arithmetic type.
     conv1 / conv2 may be bfloat16 (both), and so may B (independently): they are read as they are, and their gradients come back in
     bfloat16.  weight [nb,N,1] float32: per-point confidence of the normal equations (H = sum w_n H_n, g = sum w_n g_n; lambda does not
-    see it); differentiable."""
+    see it); differentiable.  robust "huber" / "cauchy" with robust_scale delta > 0: the robust loss of the feature-metric error
+    (ops.Level), one IRLS step per iteration; its weight is differentiated through the residual."""
     nb, N, C = conv1.shape
     bundle = B is not None
-    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, W, intr.detach(), p.detach(), precision, exact_sym, grid, weight)
+    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, W, intr.detach(), p.detach(), precision, exact_sym, grid, weight,
+                                               robust, robust_scale)
     if lambda_override is not None:
         lam = lambda_override.reshape(nb)
     else:
@@ -466,12 +471,14 @@ def window_weights(weight: Tensor, nw: Optional[int], nf: int, N: int) -> Tensor
 
 def window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base: Optional[float],
                            damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None,
-                           precision: int = 0, grid=None, return_status: bool = False, weight: Optional[Tensor] = None):
+                           precision: int = 0, grid=None, return_status: bool = False, weight: Optional[Tensor] = None,
+                           robust: Optional[str] = None, robust_scale: float = 0.0):
     """One differentiable LM iteration of a keyframe window (the joint solve of ops.lm_window_run) on the fused kernels: nf pairs
     (keyframe -> frame f) share W [K,1]; R [nf,3,3], T [nf,3,1] and conv2 [nf,h,w,3C] (or [nf,h,w,C], F2 only) are per frame.  The keyframe tensors conv1, p, D, B
     (and intr) may be given once ([1,...]): they are broadcast to the frames and their gradients summed over them.  lambda: from the mean
     |residual| over all points of all frames through the MLP (times l2_regularizer_base), or lambda_override [1].
     weight [nf,N,1] or [1,N,1] float32: per-(frame, point) confidence of the normal equations (lambda does not see it); differentiable.
+    robust, robust_scale: the robust loss of every pair's build, as in iteration_fused.
     Returns (R', T', W' [K,1]) (, status [nf])."""
     nf = R.shape[0]
     K = B.shape[-1]
@@ -480,7 +487,8 @@ def window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_
     N = conv1.shape[1]
     wf = None if weight is None else window_weights(weight, None, nf, N)
     Wf = W.reshape(1, K, 1).expand(nf, K, 1).contiguous()                       # every pair builds with the shared W; dW sums over them
-    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, Wf, intr.detach(), p.detach(), precision, exact_sym, grid, wf)
+    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, R, T, Wf, intr.detach(), p.detach(), precision, exact_sym, grid, wf,
+                                               robust, robust_scale)
     if lambda_override is not None:
         lam = lambda_override.reshape(1)
     else:
@@ -496,7 +504,8 @@ def window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_
 
 def window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base: Optional[float],
                                  damping_eps: float = 1e-5, exact_sym: bool = False, lambda_override: Optional[Tensor] = None,
-                                 precision: int = 0, grid=None, return_status: bool = False, weight: Optional[Tensor] = None):
+                                 precision: int = 0, grid=None, return_status: bool = False, weight: Optional[Tensor] = None,
+                                 robust: Optional[str] = None, robust_scale: float = 0.0):
     """One differentiable LM iteration of a batch of nw keyframe windows of nf frames (window_iteration_fused per window, one launch each
     for the build, the step and their backwards).  R [nw,nf,3,3], T [nw,nf,3,1], conv2 [nw,nf,h,w,3C] (or [nw,nf,h,w,C], F2 only) per frame,
     W [nw,K,1] per window; the keyframe tensors conv1, p, D, B (and intr) are [nw,nf,...] or [nw,1,...] (broadcast to the frames, their gradients summed over them).
@@ -506,8 +515,13 @@ def window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_param
     FP32_SIMT there, and conv2 must be [F2|gx|gy] when it requires grad (the keyframe backward takes that layout only).
     weight [nw,nf,N,1] or [nw,1,N,1] float32, in both forms: per-(frame, point) confidence of the normal equations (lambda does not see it);
     differentiable.
+    robust, robust_scale: the robust loss of every pair's build, as in iteration_fused; the per-pair form only (the keyframe build has none).
     Returns (R' [nw,nf,3,3], T' [nw,nf,3,1], W' [nw,K,1]) (, status [nw,nf])."""
     if conv1.dim() == 3:
+        if robust is not None:
+            from . import _lib
+            raise _lib.BanetError("the keyframe form (conv1 [nw,N,C]) has no robust loss; give the keyframe tensors per frame "
+                                  "([nw,nf,...] or [nw,1,...]) to take the per-pair build, which has one")
         return _keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, mlp_params, l2_regularizer_base, damping_eps, exact_sym,
                                          lambda_override, precision, return_status, weight)
     nw, nf = R.shape[0], R.shape[1]
@@ -519,7 +533,8 @@ def window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, mlp_param
     wf = None if weight is None else window_weights(weight, nw, nf, N)
     Wf = W.reshape(nw, 1, K, 1).expand(nw, nf, K, 1).reshape(nb, K, 1).contiguous()   # every pair builds with its window's W
     Rf, Tf = R.reshape(nb, 3, 3), T.reshape(nb, 3, 1)
-    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, Rf, Tf, Wf, intr.detach(), p.detach(), precision, exact_sym, grid, wf)
+    H, g, rbar_sum, _nvalid = _LMBuildFn.apply(conv1, conv2, D, B, Rf, Tf, Wf, intr.detach(), p.detach(), precision, exact_sym, grid, wf,
+                                               robust, robust_scale)
     if lambda_override is not None:
         lam = lambda_override.reshape(nw)
     else:

@@ -14,7 +14,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, Mapping, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -106,15 +106,19 @@ class BundleNet(torch.nn.Module):
         if self.strict_status and int(status.abs().max()) != 0:
             raise RuntimeError(f"LM solve skipped a step for pairs {torch.nonzero(status).flatten().tolist()} (status {status.tolist()})")
 
-    def _iterate(self, conv1, conv2, intr, p, D, B, R, T, W, base, level, grid=None, weight=None):
-        """One iteration, differentiable or not; returns (R', T', W', aux or None).  weight [nb,N,1]: per-point weight of H and g."""
+    def _iterate(self, conv1, conv2, intr, p, D, B, R, T, W, base, level, grid=None, weight=None, robust=None, robust_scale=0.0):
+        """One iteration, differentiable or not; returns (R', T', W', aux or None).  weight [nb,N,1]: per-point weight of H and g;
+        robust, robust_scale: the robust loss of the feature-metric error (ops.Level)."""
         bundle = B is not None
+        ops.robust_kind(robust, robust_scale)                                  # argument errors before any kernel runs
         if self._wants_grad(conv1, conv2, D, B, R, T, W, weight):
             if self.vmatrix_batch_scramble:
                 raise RuntimeError("vmatrix_batch_scramble=True (the reference's batch-interleaved VMatrix, bundlenet.py:45) is not differentiable here")
             if self.training_path == "reference_split":
                 if weight is not None:
                     raise RuntimeError("training_path='reference_split' has no point weights; weighted iterations train on the fused path")
+                if robust is not None:
+                    raise RuntimeError("training_path='reference_split' has no robust loss; robust iterations train on the fused path")
                 if conv1.dtype != torch.float32 or conv2.dtype != torch.float32:
                     raise RuntimeError("training_path='reference_split' takes float32 features; bfloat16 features train on the fused path")
                 if bundle and B.dtype != torch.float32:
@@ -124,10 +128,10 @@ class BundleNet(torch.nn.Module):
                 return Rn, Tn, Wn, None
             Rn, Tn, Wn, status = _ag.iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base if bundle else None,
                                                      exact_sym=self.exact_sym_grad, precision=self.precision, grid=grid, return_status=True,
-                                                     weight=weight)
+                                                     weight=weight, robust=robust, robust_scale=robust_scale)
             self._check_status(status)
             return Rn, Tn, Wn, None
-        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=grid, weight=weight)
+        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=grid, weight=weight, robust=robust, robust_scale=robust_scale)
         H, g, rbar, nvalid = ops.lm_build(lv, R, T, W, self.precision)
         lam = ops.lm_lambda(rbar, conv1.shape[1], self.mlp_packed(str(level)), float(base) if bundle else 1.0)
         Rn, Tn, Wn, delta, status = ops.lm_solve_update(H, g, lam, R, T, W, undamped_last=bundle, vmatrix_batch_scramble=self.vmatrix_batch_scramble)
@@ -135,31 +139,36 @@ class BundleNet(torch.nn.Module):
         return Rn, Tn, Wn, dict(AtA=H, Atb=g, lam=lam, rbar_sum=rbar, nvalid=nvalid, solution=delta, status=status)
 
     def CameraIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, R, T, l2_regularizer_base=None, level=None, return_aux: bool = False, *,
-                        weight: Optional[Tensor] = None):
+                        weight: Optional[Tensor] = None, robust: Optional[str] = None, robust_scale: float = 0.0):
         """reference bundlenet.py:122-191 -> (updatedR, updatedT).  l2_regularizer_base accepted, unused (as there).
         Differentiable (fused backward kernels) whenever gradients are being recorded; `return_aux` needs the no-grad path.
         weight [nb,N,1] float32 (an extension): per-point confidence of the normal equations, H = sum_n w_n H_n, g = sum_n w_n g_n; the
-        damping lambda does not see it.  Differentiable on the fused training path."""
+        damping lambda does not see it.  Differentiable on the fused training path.
+        robust "huber" / "cauchy" (an extension) with robust_scale delta > 0 in feature units: a robust loss of the feature-metric error,
+        one IRLS step per iteration (each point's weight times rho'(|d_n|^2) at the current iterate; lambda does not see it).
+        Differentiable on the fused training path, through the residual the weight depends on."""
+        kw = dict(weight=weight, robust=robust, robust_scale=robust_scale)
         if return_aux:
             with torch.no_grad():
-                Rn, Tn, _, aux = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, None, R, T, None, 1.0, level, weight=weight)
+                Rn, Tn, _, aux = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, None, R, T, None, 1.0, level, **kw)
             return Rn, Tn, aux
-        Rn, Tn, _, _ = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, None, R, T, None, 1.0, level, weight=weight)
+        Rn, Tn, _, _ = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, None, R, T, None, 1.0, level, **kw)
         return Rn, Tn
 
     def BundleIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, l2_regularizer_base=None, level=None, return_aux: bool = False, *,
-                        weight: Optional[Tensor] = None):
-        """reference bundlenet.py:193-278 -> (updatedR, updatedT, updatedW).  weight [nb,N,1]: as in CameraIteration."""
+                        weight: Optional[Tensor] = None, robust: Optional[str] = None, robust_scale: float = 0.0):
+        """reference bundlenet.py:193-278 -> (updatedR, updatedT, updatedW).  weight [nb,N,1], robust, robust_scale: as in CameraIteration."""
         base = 1.0 if l2_regularizer_base is None else float(l2_regularizer_base)      # :252-253
+        kw = dict(weight=weight, robust=robust, robust_scale=robust_scale)
         if return_aux:
             with torch.no_grad():
-                Rn, Tn, Wn, aux = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, B, R, T, W, base, level, weight=weight)
+                Rn, Tn, Wn, aux = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, B, R, T, W, base, level, **kw)
             return Rn, Tn, Wn, aux
-        Rn, Tn, Wn, _ = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, B, R, T, W, base, level, weight=weight)
+        Rn, Tn, Wn, _ = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, B, R, T, W, base, level, **kw)
         return Rn, Tn, Wn
 
     def WindowIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, l2_regularizer_base=None, level=None, *,
-                        weight: Optional[Tensor] = None):
+                        weight: Optional[Tensor] = None, robust: Optional[str] = None, robust_scale: float = 0.0):
         """One joint LM iteration of a keyframe window (an extension; the reference's layer is 2-view): the nf pairs (keyframe -> frame f)
         share the keyframe depth D + B.W.  Arguments as BundleIteration with R [nf,3,3], T [nf,3,1], conv2 [nf,h,w,3C] (or F2 only, [nf,h,w,C]) per frame and
         W [K,1] shared; the keyframe tensors conv1, p, D, B may be given once ([1,...]) or per frame.  -> (updatedR, updatedT, updatedW [K,1]).
@@ -167,12 +176,15 @@ class BundleNet(torch.nn.Module):
         A batch of nw windows: R [nw,nf,3,3], T [nw,nf,3,1], conv2 [nw,nf,h,w,3C] (or [nw,nf,h,w,C]), W [nw,K,1], keyframe tensors and fx, fy, ox, oy
         [nw,1,...] or [nw,nf,...] -> ([nw,nf,3,3], [nw,nf,3,1], [nw,K,1]), last_status [nw,nf] (banet_lm_window_batch_*).
         weight (an extension) float32: a per-(frame, keyframe point) confidence of the normal equations (see CameraIteration), [nf|1,N,1] for
-        one window, [nw,nf|1,N,1] for a batch (a frame axis of 1 is broadcast to the frames); differentiable when it requires grad."""
+        one window, [nw,nf|1,N,1] for a batch (a frame axis of 1 is broadcast to the frames); differentiable when it requires grad.
+        robust, robust_scale (an extension): the robust loss of every pair's build, as in CameraIteration; the per-pair forms only (keyframe
+        tensors with a frame axis): the keyframe form raises."""
         base = 1.0 if l2_regularizer_base is None else float(l2_regularizer_base)
         if self.vmatrix_batch_scramble:
             raise RuntimeError("vmatrix_batch_scramble=True is a 2-view quirk (bundlenet.py:45); the window solve has per-frame VMatrix only")
+        ops.robust_kind(robust, robust_scale)
         if R.dim() == 4:
-            return self._window_batch_iteration(conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, base, level, weight)
+            return self._window_batch_iteration(conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, base, level, weight, robust, robust_scale)
         nf = R.shape[0]
         intr = _intr_from_tiled(fx, fy, ox, oy)
         if self._wants_grad(conv1, conv2, D, B, R, T, W, weight):
@@ -180,18 +192,18 @@ class BundleNet(torch.nn.Module):
                 raise RuntimeError("training_path='reference_split' has no torch-graph twin of the window solve; use training_path='fused'")
             Rn, Tn, Wn, status = _ag.window_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base,
                                                             exact_sym=self.exact_sym_grad, precision=self.precision, return_status=True,
-                                                            weight=weight)
+                                                            weight=weight, robust=robust, robust_scale=robust_scale)
             self._check_status(status)
             return Rn, Tn, Wn
         frames = lambda t: t.expand(nf, *t.shape[1:]) if t.shape[0] == 1 else t
         wf = None if weight is None else _ag.window_weights(weight, None, nf, conv1.shape[1])
-        lv = ops.Level(frames(conv1), conv2, frames(intr), frames(p), frames(D), frames(B), weight=wf)
+        lv = ops.Level(frames(conv1), conv2, frames(intr), frames(p), frames(D), frames(B), weight=wf, robust=robust, robust_scale=robust_scale)
         Rn, Tn, Wn, status = ops.lm_window_run([lv], 1, R, T, W, mlp_packed=[self.mlp_packed(str(level))], l2_regularizer_base=base,
                                                precision=self.precision)
         self._check_status(status)
         return Rn, Tn, Wn
 
-    def _window_batch_iteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, base, level, weight=None):
+    def _window_batch_iteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, base, level, weight=None, robust=None, robust_scale=0.0):
         """WindowIteration on a batch of nw windows (R [nw,nf,3,3]): the fused path when gradients are recorded, else one iteration of
         ops.lm_window_batch_run."""
         nw, nf = R.shape[0], R.shape[1]
@@ -200,18 +212,19 @@ class BundleNet(torch.nn.Module):
         if len(ranks) != 1:
             raise RuntimeError("WindowIteration: conv1, p, D, B must all carry a frame axis ([nw,1|nf,...]) or all come without one ([nw,...])")
         if conv1.dim() == 3:
+            self._require_keyframe_plain_loss(robust)
             return self._keyframe_batch_iteration(conv1, conv2, intr, p, D, B, R, T, W, base, level, weight)
         if self._wants_grad(conv1, conv2, D, B, R, T, W, weight):
             if self.training_path == "reference_split":
                 raise RuntimeError("training_path='reference_split' has no torch-graph twin of the window solve; use training_path='fused'")
             Rn, Tn, Wn, status = _ag.window_batch_iteration_fused(conv1, conv2, intr, p, D, B, R, T, W, self.mlp_params(str(level)), base,
                                                                   exact_sym=self.exact_sym_grad, precision=self.precision, return_status=True,
-                                                                  weight=weight)
+                                                                  weight=weight, robust=robust, robust_scale=robust_scale)
             self._check_status(status)
             return Rn, Tn, Wn
         pairs = lambda t: (t.expand(nw, nf, *t.shape[2:]) if t.shape[1] == 1 else t).reshape(nw * nf, *t.shape[2:])
         wf = None if weight is None else _ag.window_weights(weight, nw, nf, conv1.shape[2])
-        lv = ops.Level(pairs(conv1), pairs(conv2), pairs(intr), pairs(p), pairs(D), pairs(B), weight=wf)
+        lv = ops.Level(pairs(conv1), pairs(conv2), pairs(intr), pairs(p), pairs(D), pairs(B), weight=wf, robust=robust, robust_scale=robust_scale)
         Rn, Tn, Wn, status = ops.lm_window_batch_run([lv], nw, 1, R.reshape(nw * nf, 3, 3), T.reshape(nw * nf, 3, 1), W,
                                                      mlp_packed=[self.mlp_packed(str(level))], l2_regularizer_base=base, precision=self.precision)
         self._check_status(status.reshape(nw, nf))
@@ -252,6 +265,21 @@ class BundleNet(torch.nn.Module):
             raise RuntimeError(f"the keyframe form of WindowIteration / WindowResize takes a float32 basis only (got {basis.dtype}); give the "
                                "keyframe tensors per frame ([nw,1|nf,...]) to WindowIteration for a bfloat16 basis")
 
+    @staticmethod
+    def _require_keyframe_plain_loss(robust: Optional[str]) -> None:
+        if robust is not None:
+            raise RuntimeError(f"robust={robust!r}: the keyframe form of WindowIteration / WindowResize has no robust loss; give the keyframe "
+                               "tensors per frame ([nw,1|nf,...]) to WindowIteration, whose per-pair build has one")
+
+    @staticmethod
+    def _robust_scale_at(robust_scale, level) -> float:
+        """robust_scale of the Resize methods at one level: a float for every level, or a mapping from level name ("2") to float."""
+        if isinstance(robust_scale, Mapping):
+            if str(level) not in robust_scale:
+                raise RuntimeError(f"robust_scale has no entry for level {str(level)!r} (keys {sorted(robust_scale)})")
+            return float(robust_scale[str(level)])
+        return float(robust_scale)
+
     def _require_keyframe_precision(self) -> None:
         if self.precision not in (_lib.PREC_AUTO, _lib.PREC_FP32_SIMT):
             raise RuntimeError(f"precision {self.precision}: the keyframe form of WindowIteration has no tensor-core build; use AUTO or FP32_SIMT")
@@ -277,13 +305,18 @@ class BundleNet(torch.nn.Module):
             return torch.cat([layer[h:], layer[:h]]).contiguous()
         return gfc(layer, swap_halves=True)
 
-    def CameraResize(self, intrisic, layers, points, _depths, reuse_variables=False, weight: Optional[Tensor] = None):
+    def CameraResize(self, intrisic, layers, points, _depths, reuse_variables=False, weight: Optional[Tensor] = None, *,
+                     robust: Optional[str] = None, robust_scale: Union[float, Mapping[str, float]] = 0.0):
         """reference bundlenet.py:280-329 -> (rotations, translations), levels 0..3 x 1 iteration.  Differentiable w.r.t. the feature
         pyramid and the lambda-MLP parameters when gradients are being recorded (the depth is stop_gradient'ed, :288).
         `layers` may be bfloat16 (an autocast encoder's pyramid): conv1 is then the bfloat16 resample and conv2 the half-swapped F2 only.
         weight [nb,N,1] float32 (an extension): a per-point confidence at `points`, the same at every level (see CameraIteration);
-        differentiable when it requires grad."""
+        differentiable when it requires grad.
+        robust, robust_scale (an extension): the robust loss of every level (see CameraIteration); robust_scale is one float, or a mapping
+        from level name ("0" .. "3") to float, since feature magnitudes differ per level."""
         nb = layers[-1].shape[0]
+        for level in range(0, 4) if robust is not None else ():
+            ops.robust_kind(robust, self._robust_scale_at(robust_scale, level))
         _points, intr = self._prepare(intrisic, points)
         grad = self._wants_grad(*layers, weight)
         resample, gfc = (_ag.resample, _ag.grad_fixed_concat) if grad else (ops.resample, ops.grad_fixed_concat)
@@ -296,12 +329,14 @@ class BundleNet(torch.nn.Module):
             scale = 2 ** (3 - level)
             layer1 = resample(layers[level], _points, 1.0 / scale)             # :320
             layer2 = self._swapped_f2(layers[level], gfc)                      # :321-324
-            R, T, _, _ = self._iterate(layer1, layer2, intr / scale, p, d, None, R, T, None, 1.0, level, weight=weight)
+            R, T, _, _ = self._iterate(layer1, layer2, intr / scale, p, d, None, R, T, None, 1.0, level, weight=weight, robust=robust,
+                                       robust_scale=self._robust_scale_at(robust_scale, level) if robust is not None else 0.0)
             rotations.append(R); translations.append(T)
         return rotations, translations
 
     def BundleResize(self, intrisic, layers, points, basis, init_depth, init_rotation=None, init_translation=None,
-                     reuse_variables=False, weight: Optional[Tensor] = None):
+                     reuse_variables=False, weight: Optional[Tensor] = None, *, robust: Optional[str] = None,
+                     robust_scale: Union[float, Mapping[str, float]] = 0.0):
         """reference bundlenet.py:332-399 -> (output_rotations, output_translations, output_depths), levels 2,3.  Differentiable w.r.t.
         the feature pyramid, the basis, the initial pose and the lambda-MLP parameters when gradients are being recorded
         (init_depth enters the LM only through stop_gradient, :341, and the output depth directly, :397).
@@ -310,9 +345,13 @@ class BundleNet(torch.nn.Module):
         it is sampled by the bfloat16 resample, the output depth is composed on it (banet_depth_compose_bf16), and its gradient comes back in
         bfloat16.  init_depth stays float32.
         weight [nb,N,1] float32 (an extension): a per-point confidence at `points`, the same at both levels (see CameraIteration);
-        differentiable when it requires grad."""
+        differentiable when it requires grad.
+        robust, robust_scale (an extension): the robust loss of both levels (see CameraIteration); robust_scale is one float, or a mapping
+        from level name ("2", "3") to float, since feature magnitudes differ per level."""
         nb = layers[-1].shape[0]
         K = basis.shape[-1]
+        for level in range(2, 4) if robust is not None else ():
+            ops.robust_kind(robust, self._robust_scale_at(robust_scale, level))
         _points, intr = self._prepare(intrisic, points)
         grad = self._wants_grad(*layers, basis, init_depth, init_rotation, init_translation, weight)
         resample, gfc, compose = (_ag.resample, _ag.grad_fixed_concat, _ag.depth_compose) if grad else (ops.resample, ops.grad_fixed_concat, ops.depth_compose)
@@ -329,14 +368,15 @@ class BundleNet(torch.nn.Module):
             scale = 2 ** (3 - level)
             layer1 = resample(layers[level], _points, 1.0 / scale)             # :385
             layer2 = self._swapped_f2(layers[level], gfc)                      # :386-389
-            R, T, W, _ = self._iterate(layer1, layer2, intr / scale, p, d, b, R, T, W, 1000.0, level, weight=weight)   # :393
+            R, T, W, _ = self._iterate(layer1, layer2, intr / scale, p, d, b, R, T, W, 1000.0, level, weight=weight, robust=robust,   # :393
+                                       robust_scale=self._robust_scale_at(robust_scale, level) if robust is not None else 0.0)
             Rs.append(R); Ts.append(T)
             depth = compose(init_depth.reshape(nb, -1), basis.reshape(nb, -1, K), W)   # :397
             Ds.append(depth.reshape(nb, oh, ow, 1))
         return Rs, Ts, Ds
 
     def WindowResize(self, intrisic, key_layers, frame_layers, points, basis, init_depth, init_rotation=None, init_translation=None,
-                     weight: Optional[Tensor] = None):
+                     weight: Optional[Tensor] = None, *, robust: Optional[str] = None, robust_scale: Union[float, Mapping[str, float]] = 0.0):
         """BundleResize's schedule (reference bundlenet.py:332-399) for nw keyframe windows of nf frames (an extension): levels 2, 3 x one
         joint window iteration, the keyframe depth init_depth + basis.W shared by the window's frames.
           intrisic [nw,4,1]            one camera per window (keyframe rays and every frame's projection)
@@ -350,9 +390,11 @@ class BundleNet(torch.nn.Module):
         both pyramids, the basis, the initial pose and the lambda-MLP parameters, init_depth through the output depth only (:341, :397).
         AUTO or FP32_SIMT, float32 pyramids and a float32 basis only, like the keyframe form of WindowIteration.
         weight [nw,nf,N,1] or [nw,1,N,1] float32 (an extension): a per-(frame, point) confidence at `points`, the same at both levels (see
-        WindowIteration); differentiable when it requires grad."""
+        WindowIteration); differentiable when it requires grad.
+        robust: the keyframe build has no robust loss, so a robust loss raises; WindowIteration's per-pair form takes one."""
         if self.vmatrix_batch_scramble:
             raise RuntimeError("vmatrix_batch_scramble=True is a 2-view quirk (bundlenet.py:45); the window solve has per-frame VMatrix only")
+        self._require_keyframe_plain_loss(robust)
         self._require_keyframe_precision()
         self._require_keyframe_features(*key_layers, *frame_layers)
         self._require_keyframe_basis(basis)

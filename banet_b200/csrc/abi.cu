@@ -22,6 +22,16 @@ int num_sms()
     return n;
 }
 
+// the robust loss of a level: a known kind, and a finite positive scale when it is not BANET_ROBUST_NONE
+static int check_robust(const banet_level_t* lv, const char* who)
+{
+    BANET_REQUIRE(lv->robust == BANET_ROBUST_NONE || lv->robust == BANET_ROBUST_HUBER || lv->robust == BANET_ROBUST_CAUCHY, BANET_ERR_BAD_ARG,
+                  "%s: robust=%d must be BANET_ROBUST_NONE (0), BANET_ROBUST_HUBER (1) or BANET_ROBUST_CAUCHY (2)", who, lv->robust);
+    BANET_REQUIRE(lv->robust == BANET_ROBUST_NONE || (isfinite(lv->robust_scale) && lv->robust_scale > 0.f), BANET_ERR_BAD_ARG,
+                  "%s: robust_scale=%g must be finite and > 0 with a robust loss", who, (double)lv->robust_scale);
+    return BANET_OK;
+}
+
 static int check_level(const banet_level_t* lv, const char* who)
 {
     BANET_REQUIRE(lv, BANET_ERR_BAD_ARG, "%s: null level", who);
@@ -38,7 +48,7 @@ static int check_level(const banet_level_t* lv, const char* who)
     BANET_REQUIRE((long long)lv->h * lv->w * lv->conv2_channels < (1LL << 40), BANET_ERR_BAD_ARG, "%s: map too large", who);
     BANET_REQUIRE((lv->grid_w == 0 && lv->grid_h == 0) || (lv->grid_w > 0 && lv->grid_h > 0 && (long long)lv->grid_w * lv->grid_h == lv->N),
                   BANET_ERR_BAD_ARG, "%s: grid %dx%d does not match N=%d", who, lv->grid_w, lv->grid_h, lv->N);
-    return BANET_OK;
+    return check_robust(lv, who);
 }
 
 // Level-wise policy (BANET_PREC_TF32_LEVELWISE; measured motivation in DESIGN.md §4): the rounding error of H averages out as
@@ -126,7 +136,7 @@ extern "C" int banet_device_check(void)
 // -------------------------------------------------------------------------------------------------
 extern "C" size_t banet_lm_build_workspace_bytes(const banet_level_t* lv, int precision)
 {
-    if (!lv) return 0;
+    if (!lv || check_robust(lv, "lm_build_workspace_bytes")) return 0;
     const int res = resolve_precision(lv, precision);
     if (res < 0) return 0;
     BuildPlan plan;
@@ -258,6 +268,7 @@ int carve(const banet_level_t* levels, int nlevels, int precision, RunCarve* c)
     const int nb = levels[0].nb, K = levels[0].K, P = 6 + K;
     for (int l = 0; l < nlevels; ++l) {
         BuildPlan plan;
+        if (int rc = check_robust(&levels[l], "lm_run_workspace_bytes")) return rc;
         const int res = resolve_precision(&levels[l], precision);
         if (res < 0) return res;
         int rc = plan_for(&levels[l], res, &plan);
@@ -755,6 +766,8 @@ extern "C" int banet_lm_track_legacy(const banet_level_t* levels, int nlevels, c
                       "lm_track_legacy: level %d has bf16 features; the legacy tracker takes fp32 features only", l);
         BANET_REQUIRE(!levels[l].weight, BANET_ERR_UNSUPPORTED,
                       "lm_track_legacy: level %d has point weights; the tracker's accept / reject test re-evaluates an unweighted residual", l);
+        BANET_REQUIRE(levels[l].robust == BANET_ROBUST_NONE, BANET_ERR_UNSUPPORTED,
+                      "lm_track_legacy: level %d has a robust loss; the tracker's accept / reject test re-evaluates the plain residual", l);
         BANET_REQUIRE(levels[l].K == 0 && levels[l].nb == levels[0].nb && levels[l].conv2_channels == 3 * levels[l].C && level_iters[l] >= 0, BANET_ERR_BAD_ARG,
                       "lm_track_legacy: level %d must be pose-only (K=0) with the [F2|gx|gy] layout and the same batch size", l);
     }

@@ -31,6 +31,24 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
+// Robust loss of a point (banet_level_t::robust, robust_scale = delta) at s = |d|^2, the squared norm of its residual over the channels:
+// rho'(s), the factor of its IRLS weight, and rho''(s) (d2, for the backward).  Every kernel that weighs points by a robust loss calls
+// this one function.  BANET_ROBUST_NONE: rho(s) = s, rho' = 1 exactly, so a non-robust weight is multiplied by 1.0f.
+//   Huber   rho(s) = s (s <= delta^2), 2 delta sqrt(s) - delta^2       rho' = 1 or delta / sqrt(s)      rho'' = 0 or -rho' / (2 s)
+//   Cauchy  rho(s) = delta^2 log(1 + s / delta^2)                     rho' = delta^2 / (delta^2 + s)   rho'' = -delta^2 / (delta^2 + s)^2
+__device__ __forceinline__ float robust_rho1(int kind, float delta, float s, float* d2 = nullptr)
+{
+    float r1 = 1.f, r2 = 0.f;
+    if (kind == BANET_ROBUST_HUBER) {
+        if (s > delta * delta) { r1 = delta / sqrtf(s); r2 = -0.5f * r1 / s; }
+    } else if (kind == BANET_ROBUST_CAUCHY) {
+        const float t = delta * delta, u = t + s;
+        r1 = t / u; r2 = -r1 / u;
+    }
+    if (d2) *d2 = r2;
+    return r1;
+}
+
 // streaming 128-bit load that does not pollute L1 (read-once data: conv1, B)
 __device__ __forceinline__ float4 ld_stream_f4(const float* p) {
     float4 r;

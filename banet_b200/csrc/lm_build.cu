@@ -49,7 +49,9 @@ __device__ __forceinline__ float4 ld_stream_basis4(const bf16* p) {
 }
 
 // TB: basis element type (float, or bf16 widened exactly into the fp32 tile, so everything after S0 is the fp32 kernel's arithmetic)
-template <int KP, int VEC, typename TF, typename TB = float>
+// ROBUST: the level has a robust loss (M, q also weighted by rho'(s)); a non-robust level runs the instantiation without it, whose code is
+// that of a library without robust losses (the |d|^2 sums of TapGather are then dead code)
+template <int KP, int VEC, typename TF, typename TB = float, bool ROBUST = false>
 __global__ void __launch_bounds__(BUILD_THREADS, (KP >= 128) ? 1 : 2)
 lm_build_kernel(const BuildParams prm)
 {
@@ -217,8 +219,10 @@ lm_build_kernel(const BuildParams prm)
                     f1.load_stream(c1 + c);
                     tg.group<VEC>(f1, fly_grad, c, myRb, mq);
                 }
-                // point weight: scales M and q, i.e. every block of H and g; sum |diff| and nvalid stay unweighted (x * 1.0f is exact)
-                const float wn = prm.weight ? __ldg(prm.weight + (size_t)b * N + n0 + n) : 1.f;
+                // point weight times the robust loss's rho'(s): scales M and q, i.e. every block of H and g; sum |diff| and nvalid stay
+                // unweighted (x * 1.0f is exact)
+                float wn = prm.weight ? __ldg(prm.weight + (size_t)b * N + n0 + n) : 1.f;
+                if constexpr (ROBUST) wn *= robust_rho1(prm.robust, prm.robust_scale, warp_sum(mq.s));
                 mq.m11 = warp_sum(mq.m11) * wn; mq.m12 = warp_sum(mq.m12) * wn; mq.m22 = warp_sum(mq.m22) * wn; mq.q1 = warp_sum(mq.q1) * wn; mq.q2 = warp_sum(mq.q2) * wn;
             }
             if (lane == 0) {
@@ -382,7 +386,7 @@ template <int KP, int VEC, typename TF, typename TB>
 static int launch_build(const BuildParams& prm, int grid, cudaStream_t st)
 {
     const size_t smem = BuildSmem<KP>::bytes(prm.C);
-    auto kern = lm_build_kernel<KP, VEC, TF, TB>;
+    auto kern = prm.robust ? lm_build_kernel<KP, VEC, TF, TB, true> : lm_build_kernel<KP, VEC, TF, TB, false>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("lm_build: smem attr (%zu B): %s", smem, cudaGetErrorString(e)); return BANET_ERR_CUDA; }
     kern<<<grid, BUILD_THREADS, smem, st>>>(prm);
@@ -396,7 +400,7 @@ int lm_build_simt(const banet_level_t* lv, const BuildPlan& plan, const float* R
     BuildParams prm;
     prm.nb = lv->nb; prm.N = lv->N; prm.C = lv->C; prm.K = lv->K; prm.h = lv->h; prm.w = lv->w; prm.c2 = lv->conv2_channels;
     prm.conv1 = lv->conv1; prm.conv2 = lv->conv2; prm.intr = lv->intr; prm.p = lv->p; prm.D = lv->D; prm.B = lv->B;
-    prm.R = R; prm.T = T; prm.W = W; prm.weight = lv->weight;
+    prm.R = R; prm.T = T; prm.W = W; prm.weight = lv->weight; prm.robust = lv->robust; prm.robust_scale = lv->robust_scale;
     prm.partials = reinterpret_cast<float*>(ws);
     prm.slot_floats = plan.slot_floats; prm.max_span = plan.max_span;
     prm.tiles_per_pair = plan.tiles_per_pair; prm.total_tiles = plan.total_tiles;

@@ -22,6 +22,8 @@ struct BuildParams {
     int hdd_transposed;               // tensor-core path stores the H_dd block of a slot column-major
     int force_direct;                 // generation 7, testing: take the global-tap fallback for every tile
     long long* trace;                 // optional debug timeline buffer (NULL in production)
+    int robust;                       // BANET_ROBUST_*: M, q also weighted by rho'(|d|^2) (robust_rho1, common.cuh)
+    float robust_scale;
 };
 
 struct BuildPlan {

@@ -5,7 +5,7 @@
 //
 //   warpgroup 0    4 geometry warps, 16 pixels each per tile, run ahead of everybody:                              (48 regs)
 //                    b.W from the TMA-staged basis tile, warp / mask / tap offsets -> pixel records (ring of NREC)
-//   warpgroups 1-2 8 gather warps, 8 pixels each per tile: records -> 13 tap loads -> blend / accumulate -> M, q  (112 regs)
+//   warpgroups 1-2 8 gather warps, 8 pixels each per tile: records -> 13 tap loads -> blend / accumulate -> M, q, |d|^2  (112 regs)
 //   warpgroup 3    4 algebra warps, 16 pixels each per tile:                                                        (72 regs)
 //                    2x7 per-pixel algebra (H_cc / g_c partials in registers), R rows (A_lo, R_lo) into smem,
 //                    refill of the freed basis stage by TMA (one elected thread)
@@ -133,7 +133,7 @@ template <> struct BfTap<4> {
     }
 };
 
-template <int NCH, bool FLY, int NREC>
+template <int NCH, bool FLY, int NREC, bool ROBUST>
 __device__ __forceinline__ void gather_bf16(const BuildParams& prm, const int* sTile, float* sRec, float* sRbs, uint64_t* recs, uint64_t* gath,
                                             uint64_t* rbdump, uint64_t* rbfree, int ntiles, int g, int lane)
 {
@@ -177,7 +177,7 @@ __device__ __forceinline__ void gather_bf16(const BuildParams& prm, const int* s
         for (int u = 0; u < PXW / 2; ++u) {
             const int pl = 2 * u + hw;
             const float mask = rec[pl * REC + 4];
-            float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f;
+            float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f, ss = 0.f;
             if (mask != 0.f) {
                 const uint4 o = *reinterpret_cast<const uint4*>(rec + pl * REC);
                 const int n = __float_as_int(rec[pl * REC + 11]);
@@ -218,12 +218,15 @@ __device__ __forceinline__ void gather_bf16(const BuildParams& prm, const int* s
                     const float d = t[0] - f2;
                     m11 = fmaf(gx, gx, m11); m12 = fmaf(gx, gy, m12); m22 = fmaf(gy, gy, m22);
                     q1 = fmaf(gx, d, q1); q2 = fmaf(gy, d, q2);
+                    if constexpr (ROBUST) ss = fmaf(d, d, ss);
                     rb[i] += fabsf(d);
                 }
             }
             m11 = hsum16(m11); m12 = hsum16(m12); m22 = hsum16(m22); q1 = hsum16(q1); q2 = hsum16(q2);
+            if constexpr (ROBUST) ss = hsum16(ss);
             if (hl == 0) {           // totals overwrite dx,dy / n of this pixel's record (as the fp32 gather does), times the point weight
-                const float wn = (prm.weight && mask != 0.f) ? __ldg(prm.weight + (size_t)b * N + __float_as_int(rec[pl * REC + 11])) : 1.f;
+                float wn = (prm.weight && mask != 0.f) ? __ldg(prm.weight + (size_t)b * N + __float_as_int(rec[pl * REC + 11])) : 1.f;
+                if constexpr (ROBUST) wn *= robust_rho1(prm.robust, prm.robust_scale, ss);
                 *reinterpret_cast<float4*>(rec + pl * REC + 12) = make_float4(m11 * wn, m12 * wn, m22 * wn, q1 * wn);
                 rec[pl * REC + 11] = q2 * wn;
             }
@@ -239,7 +242,10 @@ __device__ __forceinline__ void gather_bf16(const BuildParams& prm, const int* s
 // TB: basis element type (float or bf16).  A bf16 tile is staged as it lies in HBM and widened in registers by each role that reads it:
 // the b.W walk (same fp32 order), the R rows, the MMA's A fragments.  It is exact in tf32, so MODE 1 skips its in-place rounding and
 // MODE 2 / 3 skip the split-A pass: results are bitwise those of the fp32 kernel on the widened basis.
-template <int NCH, bool FLY, int MODE, int KBLK = 4, typename TF = float, typename TB = float>
+// ROBUST: the gather warps also sum |d|^2 per pixel and weigh M, q by rho'(|d|^2) (banet_level_t::robust).  That is one more FFMA per
+// channel and one more reduction per pixel on the warps suspected to pace the tile loop, so a non-robust level runs an instantiation
+// without them: its code is that of a library without robust losses.
+template <int NCH, bool FLY, int MODE, int KBLK = 4, typename TF = float, typename TB = float, bool ROBUST = false>
 __global__ void __launch_bounds__(THREADS, 1)
 lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams prm)
 {
@@ -480,7 +486,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
     } else if (warp < W0 + GW) {
         // ===================================================================== gather warps: records -> taps -> M, q
         setmaxnreg_inc<112>();
-        if constexpr (sizeof(TF) == 2) { gather_bf16<NCH, FLY, NREC>(prm, sTile, sRec, sRbs, recs, gath, rbdump, rbfree, ntiles, warp - W0, lane); return; }
+        if constexpr (sizeof(TF) == 2) { gather_bf16<NCH, FLY, NREC, ROBUST>(prm, sTile, sRec, sRbs, recs, gath, rbdump, rbfree, ntiles, warp - W0, lane); return; }
         const int g = warp - W0, hw = lane >> 4, hl = lane & 15;
         constexpr int PXW = TILE / GW;                       // 8 pixels per warp and tile
         constexpr int NUNIT = (PXW / 2) * NCH;
@@ -488,7 +494,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
 #pragma unroll
         for (int u = 0; u < NCH * 4; ++u) rb[u] = 0.f;
         float4 tb[13];
-        float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f;
+        float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f, ss = 0.f;
         int cur_b = -1, ndump = 0;
         // L2 policy: conv1 is read exactly once (evict-first), the taps are what neighbouring tiles re-read
         const uint64_t pol_stream = prm.l2_hints >= 1 ? l2_policy_evict_first() : l2_policy_evict_normal();
@@ -544,7 +550,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                         tb[9] = ldt(rm + o0); tb[10] = ldt(rm + o1); tb[11] = ldt(rp + o0); tb[12] = ldt(rp + o1);   // a0m a1m a0p a1p
                     }
                 }
-                if (jc == 0) { m11 = m12 = m22 = q1 = q2 = 0.f; }
+                if (jc == 0) { m11 = m12 = m22 = q1 = q2 = ss = 0.f; }
                 if (mask != 0.f) {
                     const float2 dxy = *reinterpret_cast<const float2*>(rec + pl * REC + 12);
                     const float dx = dxy.x, dy = dxy.y;
@@ -559,6 +565,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                             const float d = t[0].F - f2;                                                             \
                             m11 = fmaf(gx, gx, m11); m12 = fmaf(gx, gy, m12); m22 = fmaf(gy, gy, m22);               \
                             q1 = fmaf(gx, d, q1); q2 = fmaf(gy, d, q2);                                              \
+                            if constexpr (ROBUST) ss = fmaf(d, d, ss);                                               \
                             rb[4 * jc + CI] += fabsf(d);                                                             \
                         }
                         BANET_CH(x, 0) BANET_CH(y, 1) BANET_CH(z, 2) BANET_CH(w, 3)
@@ -575,6 +582,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                             const float d = t[0].F - f2;                                                             \
                             m11 = fmaf(gx, gx, m11); m12 = fmaf(gx, gy, m12); m22 = fmaf(gy, gy, m22);               \
                             q1 = fmaf(gx, d, q1); q2 = fmaf(gy, d, q2);                                              \
+                            if constexpr (ROBUST) ss = fmaf(d, d, ss);                                               \
                             rb[4 * jc + CI] += fabsf(d);                                                             \
                         }
                         BANET_CH(x, 0) BANET_CH(y, 1) BANET_CH(z, 2) BANET_CH(w, 3)
@@ -583,9 +591,12 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
                 }
                 if (jc == NCH - 1) {
                     m11 = hsum16(m11); m12 = hsum16(m12); m22 = hsum16(m22); q1 = hsum16(q1); q2 = hsum16(q2);
+                    if constexpr (ROBUST) ss = hsum16(ss);
                     if (hl == 0) {           // totals overwrite dx,dy / n of this pixel's record (no longer needed; the tap offsets stay for the prefetcher)
-                        // point weight (M and q, i.e. every block of H and g; sum |d| stays unweighted): x * 1.0f is exact
-                        const float wn = (prm.weight && mask != 0.f) ? __ldg(prm.weight + (size_t)b * N + __float_as_int(rec[pl * REC + 11])) : 1.f;
+                        // point weight times the robust loss's rho'(s) (M and q, i.e. every block of H and g; sum |d| stays unweighted):
+                        // x * 1.0f is exact
+                        float wn = (prm.weight && mask != 0.f) ? __ldg(prm.weight + (size_t)b * N + __float_as_int(rec[pl * REC + 11])) : 1.f;
+                        if constexpr (ROBUST) wn *= robust_rho1(prm.robust, prm.robust_scale, ss);
                         *reinterpret_cast<float4*>(rec + pl * REC + 12) = make_float4(m11 * wn, m12 * wn, m22 * wn, q1 * wn);
                         rec[pl * REC + 11] = q2 * wn;
                     }
@@ -768,7 +779,7 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
 template <int NCH, bool FLY, int MODE, int KBLK, typename TF, typename TB>
 static int launch6(const CUtensorMap& tm, const BuildParams& prm, int grid, cudaStream_t st)
 {
-    auto kern = lm_build_tc6_kernel<NCH, FLY, MODE, KBLK, TF, TB>;
+    auto kern = prm.robust ? lm_build_tc6_kernel<NCH, FLY, MODE, KBLK, TF, TB, true> : lm_build_tc6_kernel<NCH, FLY, MODE, KBLK, TF, TB, false>;
     const int smem = Smem<MODE, FLY, sizeof(TB) == 2>::bytes;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) { set_error("lm_build_tc6: smem attr (%d B): %s", smem, cudaGetErrorString(e)); return BANET_ERR_CUDA; }

@@ -43,7 +43,7 @@ static banet_tuning_t g_tuning = {0, 0, 4, 0, 0, 0};
 void set_tuning(const banet_tuning_t& t) { g_tuning = t; }
 const banet_tuning_t& tuning() { return g_tuning; }
 
-// Generation 7 applies to unweighted levels with fp32 features and an fp32 basis in the F2-only layout on a dense grid (tap coordinates are packed in 16 bits), modes 1 and 2.  The default
+// Generation 7 applies to unweighted, non-robust levels with fp32 features and an fp32 basis in the F2-only layout on a dense grid (tap coordinates are packed in 16 bits), modes 1 and 2.  The default
 // (tc_generation = 0) is generation 6 everywhere: in interleaved A/B runs on an H100 80GB HBM3 (400 W power limit, 32 pairs, F2-only
 // layout) generation 7 took 25.5 vs 21.5 ms at 640x480 and 5.8 vs 5.4 ms at 320x240 in TF32X1, and 2.3x as long in TF32X2 (its
 // gather warps run on 64 registers and spill, see DESIGN.md §4).  banet_set_tuning(tc_generation = 7) forces it where it applies.
@@ -53,7 +53,7 @@ static bool use_gen7(const banet_level_t* lv, int mode, int kblk)
     const bool wanted = g_tuning.tc_generation == 7;
     int wx = 0, wy = 0;
     lm_build_tc7_window(&wx, &wy);
-    return wanted && !lv->weight && lv->feature_dtype == BANET_DTYPE_F32 && lv->basis_dtype == BANET_DTYPE_F32 && lv->conv2_channels == lv->C && lv->grid_w > 0 && lv->h < 65536 && lv->w < 65536 &&
+    return wanted && !lv->weight && !lv->robust && lv->feature_dtype == BANET_DTYPE_F32 && lv->basis_dtype == BANET_DTYPE_F32 && lv->conv2_channels == lv->C && lv->grid_w > 0 && lv->h < 65536 && lv->w < 65536 &&
            lv->h >= wy && lv->w >= wx && lm_build_tc7_supported(mode, lv->C / 64, kblk);
 }
 
@@ -105,7 +105,7 @@ int lm_build_tc(const banet_level_t* lv, const BuildPlan& plan, int mode, const 
     BuildParams prm;
     prm.nb = lv->nb; prm.N = lv->N; prm.C = lv->C; prm.K = lv->K; prm.h = lv->h; prm.w = lv->w; prm.c2 = lv->conv2_channels;
     prm.conv1 = lv->conv1; prm.conv2 = lv->conv2; prm.intr = lv->intr; prm.p = lv->p; prm.D = lv->D; prm.B = lv->B;
-    prm.R = R; prm.T = T; prm.W = W; prm.weight = lv->weight;
+    prm.R = R; prm.T = T; prm.W = W; prm.weight = lv->weight; prm.robust = lv->robust; prm.robust_scale = lv->robust_scale;
     prm.partials = reinterpret_cast<float*>(ws);
     prm.slot_floats = plan.slot_floats; prm.max_span = plan.max_span;
     prm.tiles_per_pair = plan.tiles_per_pair; prm.total_tiles = plan.total_tiles;

@@ -13,7 +13,8 @@
 //     Y_c = Jc S_cc + jd (b^T S_dc)     Y_d b = Jc (S_cd b) + jd (e.b)     db = s e + S_cd^T v + t ghat_d + dDt W
 //   then the chain rule through the sampler (features: atomics into dconv2; coordinates: tap differences), the projection, the
 //   warp (dR, dT), and the depth update (dD, dB, dW).  With point weights (H = sum w_n H_n, g = sum w_n g_n) the Ghat / ghat adjoints of
-//   pixel n are scaled by w_n and dw_n = 1/2 <M, Q> + q.z, stored by its one writer.
+//   pixel n are scaled by w_n and dw_n = 1/2 <M, Q> + q.z, stored by its one writer.  A robust level weighs by w_n = c_n rho'(s_n),
+//   s_n = d^T d: dweight_n = dw rho'(s_n) goes to the confidence c_n, and ds = dw c_n rho''(s_n) adds 2 ds d_c to each channel's dd_c.
 // pose_update_bwd_kernel: the SE(3) update's backward, thread per pair, for the dense keyframe window (lm_window.cu); the solve's backward is
 //   lm_step_bwd_kernel (lm_step.cu).
 #include "common.cuh"
@@ -41,6 +42,8 @@ struct BwdParams {
     float* dweight;                              // [nb,N] their gradient, or NULL
     int exact_sym, tiles_per_pair;
     long long total_tiles;
+    int robust;                                  // BANET_ROBUST_*: the weight is weight * rho'(s) (robust_rho1)
+    float robust_scale;
 };
 
 // conv2 layouts of the build backward.  F2-only: the gradient channels are the forward's on-the-fly stencil at each tap,
@@ -52,7 +55,9 @@ constexpr int BWD_3C = 0, BWD_F2 = 1;
 
 // smem layout (floats): S_dd [K][K] | S_cd [6][K] | S_dc [K][6] | S_cc [36] | ghat [P] | W [K] | pose [16] | rhat [C]
 // TF: feature element type (float or bf16, widened on load); dconv1 / dconv2 are fp32 for both.  TB: the same for the basis; dB is fp32.
-template <int BWD_KL, int LAYOUT, typename TF, typename TB = float>
+// ROBUST: the level has a robust loss (s, rho', rho'' and the 2 ds d_c term).  A non-robust level runs the instantiation without them: its
+// code is that of a library without robust losses (the robust work would otherwise stay live at this kernel's 128-register cap and spill).
+template <int BWD_KL, int LAYOUT, typename TF, typename TB = float, bool ROBUST = false>
 __global__ void __launch_bounds__(BWD_THREADS, 2)
 lm_build_bwd_kernel(const BwdParams prm)
 {
@@ -191,15 +196,19 @@ lm_build_bwd_kernel(const BwdParams prm)
             }
             // ---- 2 x (6+1) algebra (every lane, redundantly), the point weight, dJ and the depth terms of db --------------------------
             PointAdjoint ad(a0, a1, jd0, jd1, Scc, sg, alpha, beta, eta, gamma);
-            const float dw = ad.weigh(prm.weight ? __ldg(prm.weight + gi) : 1.f, mq);
-            if (prm.dweight && lane == 0) prm.dweight[gi] = dw;
+            const float cn = prm.weight ? __ldg(prm.weight + gi) : 1.f;
+            float r1 = 1.f, r2 = 0.f, ds2 = 0.f;
+            if constexpr (ROBUST) r1 = robust_rho1(prm.robust, prm.robust_scale, warp_sum(mq.s), &r2);
+            const float dw = ad.weigh(ROBUST ? cn * r1 : cn, mq);
+            if (prm.dweight && lane == 0) prm.dweight[gi] = ROBUST ? dw * r1 : dw;
+            if constexpr (ROBUST) ds2 = 2.f * (dw * cn * r2);                          // 2 ds: the robust weight's share of each channel's dd_c
             float dJ0[6], dJ1[6], dj0, dj1, vN[8];                 // depth terms of db: vN (6), then tN, sN
             jacobian_adjoint(mq, ad, sg, eta, dJ0, dJ1, dj0, dj1);
             depth_terms(a0, a1, jd0, jd1, mq, vN);
             const float tN = vN[6], sN = vN[7];
             // ---- pass 2: dd, dG per channel -> dconv1, scatter into dconv2, coordinate gradient ------------------------------------------
             float du, dv;
-            channel_adjoint<FLY>(img, dimg, c1, sRh, tp, h, w, C, lane, ad, [&](int c, float dd) { dc1[c] = dd; }, du, dv);
+            channel_adjoint<FLY>(img, dimg, c1, sRh, tp, h, w, C, lane, ad, ds2, [&](int c, float dd) { dc1[c] = dd; }, du, dv);
             // ---- geometry backward ----------------------------------------------------------------------------------------------------
             const GeomGrad gg(pr, fx, fy, Dt, du, dv, dJ0, dJ1, dj0, dj1);
             accT[0] += gg.gX; accT[1] += gg.gY; accT[2] += gg.gZ;
@@ -224,11 +233,16 @@ lm_build_bwd_kernel(const BwdParams prm)
     if (cur_b >= 0) commit(cur_b);
 }
 
-template <typename TF, typename TB>
-static void (*select_bwd_kernel(int K, bool c3))(const BwdParams)
+template <typename TF, typename TB, bool R>
+static void (*select_bwd_kernel_r(int K, bool c3))(const BwdParams)
 {
-    if (c3) return K <= 32 ? lm_build_bwd_kernel<1, BWD_3C, TF, TB> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_3C, TF, TB> : lm_build_bwd_kernel<8, BWD_3C, TF, TB>);
-    return K <= 32 ? lm_build_bwd_kernel<1, BWD_F2, TF, TB> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_F2, TF, TB> : lm_build_bwd_kernel<8, BWD_F2, TF, TB>);
+    if (c3) return K <= 32 ? lm_build_bwd_kernel<1, BWD_3C, TF, TB, R> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_3C, TF, TB, R> : lm_build_bwd_kernel<8, BWD_3C, TF, TB, R>);
+    return K <= 32 ? lm_build_bwd_kernel<1, BWD_F2, TF, TB, R> : (K <= 128 ? lm_build_bwd_kernel<4, BWD_F2, TF, TB, R> : lm_build_bwd_kernel<8, BWD_F2, TF, TB, R>);
+}
+template <typename TF, typename TB>
+static void (*select_bwd_kernel(int K, bool c3, bool robust))(const BwdParams)
+{
+    return robust ? select_bwd_kernel_r<TF, TB, true>(K, c3) : select_bwd_kernel_r<TF, TB, false>(K, c3);
 }
 
 int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dH, const float* dg, const float* drbar,
@@ -240,8 +254,9 @@ int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const 
     BANET_REQUIRE(smem <= 220 * 1024, BANET_ERR_UNSUPPORTED, "lm_build_bwd: K=%d, C=%d need %zu B of shared memory", K, lv->C, smem);
     void (*kern)(const BwdParams);
     const bool c3 = lv->conv2_channels == 3 * lv->C, bff = lv->feature_dtype == BANET_DTYPE_BF16, bfb = K > 0 && lv->basis_dtype == BANET_DTYPE_BF16;
-    if (bfb) kern = bff ? select_bwd_kernel<bf16, bf16>(K, c3) : select_bwd_kernel<float, bf16>(K, c3);
-    else kern = bff ? select_bwd_kernel<bf16, float>(K, c3) : select_bwd_kernel<float, float>(K, c3);
+    const bool rob = lv->robust != BANET_ROBUST_NONE;
+    if (bfb) kern = bff ? select_bwd_kernel<bf16, bf16>(K, c3, rob) : select_bwd_kernel<float, bf16>(K, c3, rob);
+    else kern = bff ? select_bwd_kernel<bf16, float>(K, c3, rob) : select_bwd_kernel<float, float>(K, c3, rob);
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("lm_build_bwd smem attr: %s", cudaGetErrorString(e)); return BANET_ERR_CUDA; }
     BwdParams prm;
@@ -250,6 +265,7 @@ int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const 
     prm.dH = dH; prm.dg = dg; prm.drbar = drbar;
     prm.dconv1 = dconv1; prm.dconv2 = dconv2; prm.dD = dD; prm.dB = dB; prm.dR = dR; prm.dT = dT; prm.dW = dW;
     prm.weight = lv->weight; prm.dweight = dweight;
+    prm.robust = lv->robust; prm.robust_scale = lv->robust_scale;
     prm.exact_sym = exact_sym;
     prm.tiles_per_pair = (lv->N + BWD_TILE - 1) / BWD_TILE;
     prm.total_tiles = (long long)lv->nb * prm.tiles_per_pair;

@@ -565,7 +565,7 @@ keyframe_build_bwd_kernel(const KeyBwdParams prm)
                         const float tN = vN[6], sN = vN[7];
                         // pass 2: dd, dG per channel -> dconv1 (summed over the frames), dconv2 (atomics), the coordinate gradient
                         float du, dv;
-                        channel_adjoint<false>(img, dimg, c1, sRh, tp, h, w, C, lane, ad, [&](int c, float dd) { myDc1[c] += dd; }, du, dv);
+                        channel_adjoint<false>(img, dimg, c1, sRh, tp, h, w, C, lane, ad, 0.f, [&](int c, float dd) { myDc1[c] += dd; }, du, dv);
                         const GeomGrad gg(pr, fx, fy, Dt, du, dv, dJ0, dJ1, dj0, dj1);
                         if (lane == 0) {
                             sRT[0] += gg.grx * p0; sRT[1] += gg.grx * p1; sRT[2] += gg.grx * p2;

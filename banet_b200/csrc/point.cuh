@@ -97,8 +97,8 @@ __device__ __forceinline__ Taps taps_at(float u, float v, int h, int w) {
     return Taps(x0, y0, dx, dy, h, w);
 }
 
-// M = G^T G (m11, m12, m22) and q = G^T d (q1, q2) of one point
-struct PointMQ { float m11, m12, m22, q1, q2; };
+// M = G^T G (m11, m12, m22) and q = G^T d (q1, q2) of one point, and s = d^T d (the argument of its robust loss)
+struct PointMQ { float m11, m12, m22, q1, q2, s; };
 
 // The feature gather of one point (bundlenet.py:230-239) from the frame's conv2 map img with c2 channels per texel: [F2 | gx | gy] (c2 = 3C),
 // or F2 only (fly, c2 = C: the gradients are central differences with REFLECT-by-one borders at each tap, bundlenet.py:92-100).
@@ -111,7 +111,7 @@ struct TapGather {
         : img(img_), t00(img_ + ((size_t)tp.y0 * w_ + tp.x0) * c2_), t01(img_ + ((size_t)tp.y0 * w_ + tp.x1) * c2_),
           t10(img_ + ((size_t)tp.y1 * w_ + tp.x0) * c2_), t11(img_ + ((size_t)tp.y1 * w_ + tp.x1) * c2_),
           x0(tp.x0), x1(tp.x1), y0(tp.y0), y1(tp.y1), h(h_), w(w_), C(C_), c2(c2_), w00(tp.w00), w01(tp.w01), w10(tp.w10), w11(tp.w11) {}
-    // channels [c, c + VEC), f1 holding conv1's: accumulates M, q into mq and |d| into the fp32 sums rb[c, c + VEC) in shared memory
+    // channels [c, c + VEC), f1 holding conv1's: accumulates M, q, s into mq and |d| into the fp32 sums rb[c, c + VEC) in shared memory
     template <int VEC>
     __device__ __forceinline__ void group(const ChanVec<VEC, TF>& f1, bool fly, int c, float* rb, PointMQ& mq) const {
         ChanVec<VEC, TF> a00, a01, a10, a11;
@@ -152,7 +152,7 @@ struct TapGather {
             const float f2 = w00 * a00.v[u] + w01 * a01.v[u] + w10 * a10.v[u] + w11 * a11.v[u];
             const float d = f1.v[u] - f2;
             mq.m11 = fmaf(gx.v[u], gx.v[u], mq.m11); mq.m12 = fmaf(gx.v[u], gy.v[u], mq.m12); mq.m22 = fmaf(gy.v[u], gy.v[u], mq.m22);
-            mq.q1 = fmaf(gx.v[u], d, mq.q1); mq.q2 = fmaf(gy.v[u], d, mq.q2);
+            mq.q1 = fmaf(gx.v[u], d, mq.q1); mq.q2 = fmaf(gy.v[u], d, mq.q2); mq.s = fmaf(d, d, mq.s);
             ra.v[u] += fabsf(d);
         }
         ra.store_smem(rb + c);
@@ -229,14 +229,15 @@ struct FlyTaps {
     }
 };
 
-// Pass 1 of the backward, lanes over channels: M, q of one point, summed over the warp.  FLY: conv2 is F2 only (the gradients from the
-// stencil at each tap); otherwise [F2 | gx | gy].
+// Pass 1 of the backward, lanes over channels: M, q of one point, summed over the warp, and s as this lane's partial (a caller that uses
+// it sums it with warp_sum; one that does not leaves no trace of it in its code).  FLY: conv2 is F2 only (the gradients from the stencil
+// at each tap); otherwise [F2 | gx | gy].
 template <bool FLY, typename TF>
 __device__ __forceinline__ PointMQ point_mq(const TF* img, const TF* c1, const Taps& tp, int h, int w, int C, int lane) {
     const int C3 = FLY ? C : 3 * C;
     const float w00 = tp.w00, w01 = tp.w01, w10 = tp.w10, w11 = tp.w11;
     const size_t o00 = ((size_t)tp.y0 * w + tp.x0) * C3, o01 = ((size_t)tp.y0 * w + tp.x1) * C3, o10 = ((size_t)tp.y1 * w + tp.x0) * C3, o11 = ((size_t)tp.y1 * w + tp.x1) * C3;
-    float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f;
+    float m11 = 0.f, m12 = 0.f, m22 = 0.f, q1 = 0.f, q2 = 0.f, s = 0.f;
     for (int c = lane; c < C; c += 32) {
         float f2, gx, gy;
         if constexpr (FLY) {
@@ -252,9 +253,9 @@ __device__ __forceinline__ PointMQ point_mq(const TF* img, const TF* c1, const T
             gy = w00 * ldg_feat(img + o00 + 2 * C + c) + w01 * ldg_feat(img + o01 + 2 * C + c) + w10 * ldg_feat(img + o10 + 2 * C + c) + w11 * ldg_feat(img + o11 + 2 * C + c);
         }
         const float d = ldg_feat(c1 + c) - f2;
-        m11 = fmaf(gx, gx, m11); m12 = fmaf(gx, gy, m12); m22 = fmaf(gy, gy, m22); q1 = fmaf(gx, d, q1); q2 = fmaf(gy, d, q2);
+        m11 = fmaf(gx, gx, m11); m12 = fmaf(gx, gy, m12); m22 = fmaf(gy, gy, m22); q1 = fmaf(gx, d, q1); q2 = fmaf(gy, d, q2); s = fmaf(d, d, s);
     }
-    return PointMQ{warp_sum(m11), warp_sum(m12), warp_sum(m22), warp_sum(q1), warp_sum(q2)};
+    return PointMQ{warp_sum(m11), warp_sum(m12), warp_sum(m22), warp_sum(q1), warp_sum(q2), s};
 }
 
 // The adjoint of one point's 2 x (6+1) algebra.  With S = the symmetrised dL/dH and ghat = dL/dg, alpha = S_cd b, beta = S_dc^T b,
@@ -299,12 +300,12 @@ __device__ __forceinline__ void jacobian_adjoint(const PointMQ& mq, const PointA
     dj0 = mq.m11 * ad.yb0 + mq.m12 * ad.yb1 + mq.q1 * eta; dj1 = mq.m12 * ad.yb0 + mq.m22 * ad.yb1 + mq.q2 * eta;
 }
 
-// Pass 2 of the backward, lanes over channels: per channel c, dd_c = G_c z + rhat_c sign(d_c) goes to put_dd(c, dd_c); the feature map's
-// adjoint (taps of -dd_c on the values, dG_c = G_c Q + d_c z^T on the gradients) is scattered into dimg with atomics; returns the gradient
-// (du, dv) of the pixel coordinates, summed over the warp.
+// Pass 2 of the backward, lanes over channels: per channel c, dd_c = G_c z + rhat_c sign(d_c) (+ ds2 d_c, the robust weight's term
+// 2 ds d_c; skipped when ds2 == 0) goes to put_dd(c, dd_c); the feature map's adjoint (taps of -dd_c on the values, dG_c = G_c Q + d_c z^T
+// on the gradients) is scattered into dimg with atomics; returns the gradient (du, dv) of the pixel coordinates, summed over the warp.
 template <bool FLY, typename TF, typename PutDd>
 __device__ __forceinline__ void channel_adjoint(const TF* img, float* dimg, const TF* c1, const float* sRh, const Taps& tp, int h, int w, int C,
-                                                int lane, const PointAdjoint& ad, PutDd put_dd, float& du_out, float& dv_out) {
+                                                int lane, const PointAdjoint& ad, float ds2, PutDd put_dd, float& du_out, float& dv_out) {
     const int C3 = FLY ? C : 3 * C;
     const float w00 = tp.w00, w01 = tp.w01, w10 = tp.w10, w11 = tp.w11, dx = tp.dx, dy = tp.dy;
     const float z0 = ad.z0, z1 = ad.z1, Q00 = ad.Q00, Q01 = ad.Q01, Q10 = ad.Q10, Q11 = ad.Q11;
@@ -326,7 +327,8 @@ __device__ __forceinline__ void channel_adjoint(const TF* img, float* dimg, cons
         const float gx = w00 * g00 + w01 * g01 + w10 * g10 + w11 * g11;
         const float gy = w00 * k00 + w01 * k01 + w10 * k10 + w11 * k11;
         const float d = ldg_feat(c1 + c) - f2;
-        const float dd = gx * z0 + gy * z1 + sRh[c] * sgn(d);
+        float dd = gx * z0 + gy * z1 + sRh[c] * sgn(d);
+        if (ds2 != 0.f) dd = fmaf(ds2, d, dd);
         const float dgx = gx * Q00 + gy * Q10 + d * z0, dgy = gx * Q01 + gy * Q11 + d * z1;
         put_dd(c, dd);
         const float df = -dd;

@@ -5,6 +5,7 @@ missing library raise.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass
 from typing import List, Optional, Sequence, Tuple
 
@@ -159,6 +160,21 @@ def depth_compose(init_depth: Tensor, basis: Tensor, W: Tensor) -> Tensor:
 
 
 # ------------------------------------------------------------------------------------------ layer level
+_ROBUST_KINDS = {None: _lib.ROBUST_NONE, "huber": _lib.ROBUST_HUBER, "cauchy": _lib.ROBUST_CAUCHY}
+
+
+def robust_kind(robust: Optional[str], robust_scale: float) -> Tuple[int, float]:
+    """(banet_level_t::robust, ::robust_scale) of a robust loss given by name: None, "huber" or "cauchy", with a finite scale > 0."""
+    if robust not in _ROBUST_KINDS:
+        raise _lib.BanetError(f"robust={robust!r}: expected None, 'huber' or 'cauchy'")
+    if robust is None:
+        return _lib.ROBUST_NONE, 0.0
+    scale = float(robust_scale)
+    if not (math.isfinite(scale) and scale > 0.0):
+        raise _lib.BanetError(f"robust_scale={robust_scale!r}: a {robust} loss needs a finite scale > 0")
+    return _ROBUST_KINDS[robust], scale
+
+
 @dataclass
 class Level:
     """One pyramid level in the reference's tensor layouts (see banet_level in include/banet_abi.h)."""
@@ -170,6 +186,8 @@ class Level:
     B: Optional[Tensor]       # [nb,N,K] or None; float32 or bfloat16, independent of the features' dtype
     grid: Optional[Tuple[int, int]] = None   # (grid_w, grid_h) if the N points are a row-major raster grid (locality hint)
     weight: Optional[Tensor] = None          # [nb,N,1] float32 per-point weight of the normal equations (H, g); None = unweighted
+    robust: Optional[str] = None             # robust loss of the feature-metric error: None (squared), "huber" or "cauchy" (IRLS weight
+    robust_scale: float = 0.0                # w_n = weight_n rho'(|d_n|^2) at each build); its scale delta > 0 in feature units
 
     def as_struct(self) -> Tuple[BanetLevel, list]:
         conv1 = _chk(self.conv1, "conv1", features=True); nb, N, Cc = conv1.shape
@@ -188,9 +206,10 @@ class Level:
         gw, gh = (0, 0) if self.grid is None else self.grid
         if gw * gh not in (0, N):
             raise _lib.BanetError(f"grid {gw}x{gh} does not match N={N}")
+        kind, scale = robust_kind(self.robust, self.robust_scale)
         return BanetLevel(nb, N, Cc, K, h, w, c2, conv1.data_ptr(), conv2.data_ptr(), intr.data_ptr(), p.data_ptr(),
                           D.data_ptr(), _ptr(B), gw, gh, _FEATURE_DTYPES[conv1.dtype], _FEATURE_DTYPES[torch.float32 if B is None else B.dtype],
-                          _ptr(wt)), keep
+                          _ptr(wt), kind, scale), keep
 
 
 def lm_build(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], precision: int = _lib.PREC_AUTO):

@@ -109,9 +109,20 @@ int banet_interpolate2d(const float* data, const float* xy, float coord_scale, i
 #define BANET_DTYPE_F32  0
 #define BANET_DTYPE_BF16 1
 
-/* feature_dtype, basis_dtype and weight are the last fields, so a zero-initialised struct keeps fp32 features, an fp32 basis and no
- * point weights.  Each of them changed sizeof(banet_level_t) and therefore the stride of every levels[] array: code compiled against a
- * header without all three fields cannot pass level arrays to this library. */
+/* Robust losses of the feature-metric error (banet_level_t::robust).  With s_n = sum_c d_c^2 point n's squared residual norm at the
+ * current iterate and delta = robust_scale > 0 (feature units):
+ *   BANET_ROBUST_HUBER   rho(s) = s for s <= delta^2, else 2 delta sqrt(s) - delta^2      rho'(s) = 1 or delta / sqrt(s)
+ *   BANET_ROBUST_CAUCHY  rho(s) = delta^2 log(1 + s / delta^2)                           rho'(s) = delta^2 / (delta^2 + s)
+ * Each build is one step of iteratively reweighted least squares: point n enters with the weight w_n = c_n rho'(s_n) (c_n: the point
+ * weight, 1 without one) on exactly the point-weight path, H = sum_n w_n J_n^T M_n J_n, g = sum_n w_n J_n^T q_n.  The weight is evaluated
+ * afresh at every build; H has no second-order (rho'') term.  rbar_sum and nvalid stay unweighted, so lambda does not see the loss. */
+#define BANET_ROBUST_NONE   0
+#define BANET_ROBUST_HUBER  1
+#define BANET_ROBUST_CAUCHY 2
+
+/* feature_dtype, basis_dtype, weight, robust and robust_scale are the last fields, so a zero-initialised struct keeps fp32 features, an
+ * fp32 basis, no point weights and the plain squared loss.  Each of them changed sizeof(banet_level_t) and therefore the stride of every
+ * levels[] array: code compiled against a header without all five fields cannot pass level arrays to this library. */
 typedef struct banet_level {
     int nb, N, C, K;          /* pairs, points per pair, feature channels, depth bases (0 = pose only) */
     int h, w;                 /* conv2 map size at this level */
@@ -139,6 +150,13 @@ typedef struct banet_level {
                                  non-finite one gives status 2.  NULL is the unweighted arithmetic bit for bit, and so are weights of
                                  ones.  Weighted levels never run generation 7 and are rejected by banet_lm_track_legacy
                                  (BANET_ERR_UNSUPPORTED); the whole-solve entries honour them per pair */
+    int robust;               /* BANET_ROBUST_NONE (0), BANET_ROBUST_HUBER (1) or BANET_ROBUST_CAUCHY (2); any other value is
+                                 BANET_ERR_BAD_ARG in every entry that takes levels.  Robust levels never run generation 7, are rejected by
+                                 banet_lm_track_legacy (BANET_ERR_UNSUPPORTED: its accept / reject test re-evaluates the plain residual),
+                                 and the whole-solve entries honour them per pair.  The backward differentiates the weight too:
+                                 dweight_n = dw rho'(s_n), and each channel's residual adjoint gains 2 dw c_n rho''(s_n) d_c (dw: the
+                                 gradient w.r.t. w_n).  BANET_ROBUST_NONE is the plain arithmetic bit for bit */
+    float robust_scale;       /* delta of the robust loss, finite and > 0 when robust != 0 (else BANET_ERR_BAD_ARG); ignored when robust == 0 */
 } banet_level_t;
 
 #define BANET_PREC_AUTO    (-1)   /* the level-wise policy (TF32_LEVELWISE) where the tensor-core path applies (K in {32,64,128}, C in {64,128}), else FP32_SIMT */
