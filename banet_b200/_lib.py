@@ -80,6 +80,9 @@ SIGNATURES = {
     "banet_lm_build_workspace_bytes": (C.c_size_t, [C.POINTER(BanetLevel), C.c_int]),
     "banet_lm_build": (C.c_int, [C.POINTER(BanetLevel)] + [c_float_p] * 3 + [C.c_int] + [c_float_p] * 4
                        + [C.c_void_p, C.c_size_t, c_stream]),
+    "banet_lm_cost_workspace_bytes": (C.c_size_t, [C.POINTER(BanetLevel)]),
+    "banet_lm_cost": (C.c_int, [C.POINTER(BanetLevel)] + [c_float_p] * 3 + [c_float_p] * 4 + [C.c_void_p, C.c_size_t, c_stream]),
+    "banet_lm_cost_bwd": (C.c_int, [C.POINTER(BanetLevel)] + [c_float_p] * 4 + [c_float_p] * 8 + [c_stream]),
     "banet_mlp_param_count": (C.c_size_t, [C.c_int]),
     "banet_lm_lambda": (C.c_int, [c_float_p, C.c_int, C.c_int, C.c_int, c_float_p, C.c_float, c_float_p, c_stream]),
     "banet_lm_solve_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),

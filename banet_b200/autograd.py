@@ -177,6 +177,47 @@ class _LMBuildFn(torch.autograd.Function):
         return dconv1.to(conv1.dtype), dconv2.to(conv2.dtype), dD, dB, dR, dT, dW, None, None, None, None, None, dweight, None, None
 
 
+class _LMCostFn(torch.autograd.Function):
+    """cost [nb] = banet_lm_cost(...); backward = banet_lm_cost_bwd, the exact derivative of the cost through the bilinear sample of F2.
+    bfloat16 features and a bfloat16 basis are saved as they are; their gradients are accumulated in fp32 by the kernel and cast once.
+    robust, robust_scale: the level's robust loss (ops.Level), constants."""
+
+    @staticmethod
+    def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, grid, weight, robust=None, robust_scale=0.0):
+        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=grid, weight=weight, robust=robust, robust_scale=robust_scale)
+        cost, _nvalid = ops.lm_cost(lv, R, T, W)
+        empty = conv1.new_empty(0)
+        ctx.save_for_backward(conv1, conv2, D, B if B is not None else empty, R, T, W if W is not None else empty, intr, p,
+                              weight if weight is not None else empty)
+        ctx.has_basis = B is not None; ctx.has_weight = weight is not None
+        ctx.grid = grid; ctx.robust = (robust, robust_scale)
+        return cost
+
+    @staticmethod
+    def backward(ctx, dcost):
+        conv1, conv2, D, B, R, T, W, intr, p, weight = ctx.saved_tensors
+        if not ctx.has_basis:
+            B = None; W = None
+        if not ctx.has_weight:
+            weight = None
+        lv = ops.Level(conv1, conv2, intr, p, D, B, grid=ctx.grid, weight=weight, robust=ctx.robust[0], robust_scale=ctx.robust[1])
+        want_dw = weight is not None and ctx.needs_input_grad[10]
+        grads = ops.lm_cost_bwd(lv, R, T, W, dcost.contiguous(), return_dweight=want_dw)
+        dconv1, dconv2, dD, dB, dR, dT, dW = grads[:7]
+        dweight = grads[7] if want_dw else None
+        dB = None if dB is None else dB.to(B.dtype)
+        return dconv1.to(conv1.dtype), dconv2.to(conv2.dtype), dD, dB, dR, dT, dW, None, None, None, dweight, None, None
+
+
+def feature_metric_cost(conv1, conv2, D, B, R, T, W, intr, p, grid=None, weight: Optional[Tensor] = None, robust: Optional[str] = None,
+                        robust_scale: float = 0.0) -> Tensor:
+    """The feature-metric cost of a level at (R, T, W), differentiable: cost [nb] = sum_n c_n rho(s_n) over the in-bounds points
+    (ops.lm_cost), with gradients w.r.t. conv1, conv2 (either layout), D, B, R, T, W and weight (banet_lm_cost_bwd).  intr and p are
+    constants.  bfloat16 features or basis are read as they are, and their gradients come back in bfloat16."""
+    ops.robust_kind(robust, robust_scale)
+    return _LMCostFn.apply(conv1, conv2, D, B, R, T, W, intr.detach(), p.detach(), grid, weight, robust, robust_scale)
+
+
 class _KeyframeBuildFn(torch.autograd.Function):
     """(H, g, rbar_sum) = banet_lm_keyframe_build(...) (the window-reduced per-pair system); backward = banet_lm_keyframe_build_bwd.
     conv1 [nw,N,C], D, B, p once per window; conv2, intr, R, T per pair; W [nw,K,1].  Saves the inputs only: no per-frame copy of the

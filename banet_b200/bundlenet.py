@@ -167,6 +167,20 @@ class BundleNet(torch.nn.Module):
         Rn, Tn, Wn, _ = self._iterate(conv1, conv2, _intr_from_tiled(fx, fy, ox, oy), p, D, B, R, T, W, base, level, **kw)
         return Rn, Tn, Wn
 
+    def FeatureMetricCost(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, weight: Optional[Tensor] = None, *,
+                          robust: Optional[str] = None, robust_scale: float = 0.0) -> Tensor:
+        """The energy BundleIteration takes one step on, at (R, T, W) (an extension): [nb] = sum_n c_n rho(|d_n|^2) over the in-bounds
+        points, d_n the point's feature-metric residual, c_n its weight [nb,N,1] (ones when None) and rho the robust loss (rho(s) = s
+        without one).  Arguments and layouts of BundleIteration (B = None, W = None for pose-only levels; conv2 [F2|gx|gy] or F2 only).
+        Differentiable in conv1, conv2, D, B, R, T, W and weight whenever gradients are being recorded (autograd.feature_metric_cost),
+        e.g. as a training loss at the solution; otherwise one no-grad kernel (ops.lm_cost)."""
+        ops.robust_kind(robust, robust_scale)                                  # argument errors before any kernel runs
+        intr = _intr_from_tiled(fx, fy, ox, oy)
+        if torch.is_grad_enabled() and any(isinstance(t, Tensor) and t.requires_grad for t in (conv1, conv2, D, B, R, T, W, weight)):
+            return _ag.feature_metric_cost(conv1, conv2, D, B, R, T, W, intr, p, weight=weight, robust=robust, robust_scale=robust_scale)
+        lv = ops.Level(conv1, conv2, intr, p, D, B, weight=weight, robust=robust, robust_scale=robust_scale)
+        return ops.lm_cost(lv, R, T, W)[0]
+
     def WindowIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, l2_regularizer_base=None, level=None, *,
                         weight: Optional[Tensor] = None, robust: Optional[str] = None, robust_scale: float = 0.0):
         """One joint LM iteration of a keyframe window (an extension; the reference's layer is 2-view): the nf pairs (keyframe -> frame f)

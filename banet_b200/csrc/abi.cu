@@ -249,6 +249,38 @@ extern "C" int banet_lm_build_bwd(const banet_level_t* lv, const float* R, const
     return banet_lm_build_bwd_weighted(lv, R, T, W, dH, dg, drbar_sum, exact_sym, dconv1, dconv2, dD, dB, dR, dT, dW, nullptr, stream);
 }
 
+// -------------------------------------------------------------------------------------------------
+extern "C" size_t banet_lm_cost_workspace_bytes(const banet_level_t* lv)
+{
+    if (check_level(lv, "lm_cost_workspace_bytes") || lv->K > 256) return 0;
+    return lm_cost_ws_bytes(lv);
+}
+
+extern "C" int banet_lm_cost(const banet_level_t* lv, const float* R, const float* T, const float* W, float* cost, float* nvalid, float* s,
+                             float* mask, void* ws, size_t ws_bytes, banet_stream_t stream)
+{
+    int rc = check_level(lv, "lm_cost");
+    if (rc) return rc;
+    BANET_REQUIRE(R && T && cost && nvalid, BANET_ERR_BAD_ARG, "lm_cost: null pointer");
+    BANET_REQUIRE(lv->K == 0 || W, BANET_ERR_BAD_ARG, "lm_cost: K=%d but W is null", lv->K);
+    BANET_REQUIRE(lv->K <= 256, BANET_ERR_UNSUPPORTED, "lm_cost: K=%d > 256 not supported", lv->K);
+    const size_t need = lm_cost_ws_bytes(lv);
+    BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_cost: workspace %zu < %zu bytes", ws_bytes, need);
+    return lm_cost(lv, R, T, W, cost, nvalid, s, mask, ws, (cudaStream_t)stream);
+}
+
+extern "C" int banet_lm_cost_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dcost,
+                                 float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, float* dweight,
+                                 banet_stream_t stream)
+{
+    int rc = check_level(lv, "lm_cost_bwd");
+    if (rc) return rc;
+    BANET_REQUIRE(R && T && dcost && dconv1 && dconv2 && dD && dR && dT, BANET_ERR_BAD_ARG, "lm_cost_bwd: null pointer");
+    BANET_REQUIRE(lv->K == 0 || (W && dB && dW), BANET_ERR_BAD_ARG, "lm_cost_bwd: K=%d but W / dB / dW is null", lv->K);
+    BANET_REQUIRE(lv->K <= 256, BANET_ERR_UNSUPPORTED, "lm_cost_bwd: K=%d > 256 not supported", lv->K);
+    return lm_cost_bwd(lv, R, T, W, dcost, dconv1, dconv2, dD, dB, dR, dT, dW, dweight, (cudaStream_t)stream);
+}
+
 extern "C" int banet_lm_solve_update_bwd(const float* H, const float* g, const float* lambda, const float* delta, int nb, int K, const banet_solve_opts_t* opts,
                                          const float* R, const float* T, const float* dR_out, const float* dT_out, const float* dW_out,
                                          float* dH, float* dg, float* dlambda, float* dR, float* dT, float* dW, banet_stream_t stream)

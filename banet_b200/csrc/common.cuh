@@ -48,6 +48,19 @@ __device__ __forceinline__ float robust_rho1(int kind, float delta, float s, flo
     if (d2) *d2 = r2;
     return r1;
 }
+// rho(s) itself, the loss whose derivative robust_rho1 gives (the same branch at s = delta^2): the feature-metric cost of a point.
+__device__ __forceinline__ float robust_rho(int kind, float delta, float s)
+{
+    if (kind == BANET_ROBUST_HUBER) {
+        const float t = delta * delta;
+        return s > t ? 2.f * delta * sqrtf(s) - t : s;
+    }
+    if (kind == BANET_ROBUST_CAUCHY) {
+        const float t = delta * delta;
+        return t * log1pf(s / t);
+    }
+    return s;
+}
 
 // streaming 128-bit load that does not pollute L1 (read-once data: conv1, B)
 __device__ __forceinline__ float4 ld_stream_f4(const float* p) {

@@ -142,6 +142,12 @@ int lm_track_legacy(const banet_level_t* levels, int nlevels, const int* level_i
 // backward of one iteration (lm_bwd.cu)
 int lm_build_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dH, const float* dg, const float* drbar,
                  int exact_sym, float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, float* dweight, cudaStream_t st);
+// feature-metric cost of a level and its backward (lm_cost.cu); ws: lm_cost_ws_bytes; s, mask, dweight may be null
+size_t lm_cost_ws_bytes(const banet_level_t* lv);
+int lm_cost(const banet_level_t* lv, const float* R, const float* T, const float* W, float* cost, float* nvalid, float* s, float* mask,
+            void* ws, cudaStream_t st);
+int lm_cost_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dcost, float* dconv1, float* dconv2,
+                float* dD, float* dB, float* dR, float* dT, float* dW, float* dweight, cudaStream_t st);
 // the SE(3) update backward of nb poses (ddelta[0:6] of pose b -> ddelta + b * P)
 int launch_pose_update_bwd(const float* delta, int nb, int P, const float* R, const float* T, const float* gRn, const float* gTn,
                            float* ddelta, float* dR, float* dT, cudaStream_t st);

@@ -1,6 +1,7 @@
-// Per-point code of the fp32 SIMT build kernels: lm_build_kernel (lm_build.cu), lm_build_bwd_kernel (lm_bwd.cu) and the keyframe build and
-// its backward (lm_window_key.cu).  Each piece is one step of one point, computed exactly as every one of those kernels needs it; the tile
-// and frame loops, the slot layouts and the way each kernel stores or commits its sums stay in the kernels.
+// Per-point code of the fp32 SIMT build kernels: lm_build_kernel (lm_build.cu), lm_build_bwd_kernel (lm_bwd.cu), the keyframe build and
+// its backward (lm_window_key.cu), and the feature-metric cost and its backward (lm_cost.cu).  Each piece is one step of one point,
+// computed exactly as every one of those kernels needs it; the tile and frame loops, the slot layouts and the way each kernel stores or
+// commits its sums stay in the kernels.
 #pragma once
 #include "common.cuh"
 #include "features.cuh"
@@ -156,6 +157,53 @@ struct TapGather {
             ra.v[u] += fabsf(d);
         }
         ra.store_smem(rb + c);
+    }
+};
+
+// b.W of a staged basis row padded to KP (a runtime value of padded_K) in basis_dot<KP>'s own arithmetic: kernels that take every K in
+// one instantiation get the build's depth, and therefore its mask, bit for bit
+__device__ __forceinline__ float basis_dot_padded(const float* brow, const float* sW, int KP) {
+    switch (KP) {
+        case 16:  return basis_dot<16>(brow, sW);
+        case 32:  return basis_dot<32>(brow, sW);
+        case 64:  return basis_dot<64>(brow, sW);
+        case 128: return basis_dot<128>(brow, sW);
+        default:  return basis_dot<256>(brow, sW);
+    }
+}
+
+// The value-only sample of one point (the feature-metric cost, lm_cost.cu): F2 at the four taps, the first C channels of each texel of a
+// map with c2 channels per texel (3C: the gradient channels are never read; C: F2 only, no stencil).  d_c = conv1_c - F2(u, v)_c with the
+// bilinear weights in TapGather's order.  Offsets are elements from the pair's map, so the same taps address conv2 and dconv2.
+struct ValueTaps {
+    size_t o00, o01, o10, o11;
+    float w00, w01, w10, w11, dx, dy;
+    __device__ __forceinline__ ValueTaps(const Taps& tp, int w, int c2)
+        : o00(((size_t)tp.y0 * w + tp.x0) * c2), o01(((size_t)tp.y0 * w + tp.x1) * c2), o10(((size_t)tp.y1 * w + tp.x0) * c2),
+          o11(((size_t)tp.y1 * w + tp.x1) * c2), w00(tp.w00), w01(tp.w01), w10(tp.w10), w11(tp.w11), dx(tp.dx), dy(tp.dy) {}
+    // channels [c, c + VEC), f1 holding conv1's: accumulates d_c^2 into s
+    template <int VEC, typename TF>
+    __device__ __forceinline__ void squares(const TF* img, const ChanVec<VEC, TF>& f1, int c, float& s) const {
+        ChanVec<VEC, TF> a00, a01, a10, a11;
+        a00.load(img + o00 + c); a01.load(img + o01 + c); a10.load(img + o10 + c); a11.load(img + o11 + c);
+#pragma unroll
+        for (int u = 0; u < VEC; ++u) {
+            const float d = f1.v[u] - (w00 * a00.v[u] + w01 * a01.v[u] + w10 * a10.v[u] + w11 * a11.v[u]);
+            s = fmaf(d, d, s);
+        }
+    }
+    // channel c alone (lanes over channels): d_c, and the tap values in t
+    template <typename TF>
+    __device__ __forceinline__ float residual(const TF* img, const TF* c1, int c, float t[4]) const {
+        t[0] = ldg_feat(img + o00 + c); t[1] = ldg_feat(img + o01 + c); t[2] = ldg_feat(img + o10 + c); t[3] = ldg_feat(img + o11 + c);
+        return ldg_feat(c1 + c) - (w00 * t[0] + w01 * t[1] + w10 * t[2] + w11 * t[3]);
+    }
+    // the adjoint of channel c's sample, given df = dL/dF2_c and the tap values t: w_tau df into the taps of dimg (atomics), and the
+    // gradient of the pixel coordinates from the tap differences added to (du, dv)
+    __device__ __forceinline__ void adjoint(float* dimg, int c, const float t[4], float df, float& du, float& dv) const {
+        atomicAdd(dimg + o00 + c, w00 * df); atomicAdd(dimg + o01 + c, w01 * df); atomicAdd(dimg + o10 + c, w10 * df); atomicAdd(dimg + o11 + c, w11 * df);
+        du += df * ((1.f - dy) * (t[1] - t[0]) + dy * (t[3] - t[2]));
+        dv += df * ((1.f - dx) * (t[2] - t[0]) + dx * (t[3] - t[1]));
     }
 };
 

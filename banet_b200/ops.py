@@ -229,6 +229,50 @@ def lm_build(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], precision:
     return H, g, rbar, nvalid
 
 
+def lm_cost(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], per_point: bool = False):
+    """Feature-metric cost of the level at (R, T, W) (banet_lm_cost): cost [nb] = sum_n c_n rho(s_n) over the in-bounds points, s_n the
+    squared norm of the build's residual, c_n the point weight and rho the level's robust loss (rho(s) = s without one), and nvalid [nb],
+    bit for bit lm_build's.  per_point=True appends s [nb,N,1] (0 at masked points) and mask [nb,N,1]."""
+    lib = load()
+    st, keep = level.as_struct()
+    nb, K, N = st.nb, st.K, st.N
+    R = _chk(R, "R", (nb, 3, 3)); T = _chk(T, "T", (nb, 3, 1))
+    Wt = None if K == 0 else _chk(W, "W", (nb, K, 1))
+    dev = R.device
+    cost = torch.empty(nb, device=dev, dtype=torch.float32); nvalid = torch.empty(nb, device=dev, dtype=torch.float32)
+    s = torch.empty(nb, N, 1, device=dev, dtype=torch.float32) if per_point else None
+    mask = torch.empty(nb, N, 1, device=dev, dtype=torch.float32) if per_point else None
+    nbytes = lib.banet_lm_cost_workspace_bytes(C.byref(st))
+    if nbytes == 0:
+        check(lib.banet_lm_cost(C.byref(st), R.data_ptr(), T.data_ptr(), _ptr(Wt), cost.data_ptr(), nvalid.data_ptr(), None, None, None, 0,
+                                _stream()), "banet_lm_cost")
+    ws = _ws(nbytes, dev)
+    check(lib.banet_lm_cost(C.byref(st), R.data_ptr(), T.data_ptr(), _ptr(Wt), cost.data_ptr(), nvalid.data_ptr(), _ptr(s), _ptr(mask),
+                            ws.data_ptr(), ws.numel(), _stream()), "banet_lm_cost")
+    return (cost, nvalid, s, mask) if per_point else (cost, nvalid)
+
+
+def lm_cost_bwd(level: Level, R: Tensor, T: Tensor, W: Optional[Tensor], dcost: Tensor, return_dweight: bool = False):
+    """Backward of lm_cost's cost (banet_lm_cost_bwd): dcost [nb] -> dconv1, dconv2, dD, dB, dR, dT, dW (+ dweight [nb,N,1] =
+    dcost rho(s_n) with return_dweight), the exact derivative of the cost through the bilinear sample of F2.  dconv2 has conv2's layout
+    (on [F2|gx|gy] its gradient channels are zero); dconv1, dconv2 and dB are float32 whatever the dtypes of the features and the basis."""
+    lib = load()
+    st, keep = level.as_struct()
+    nb, K, Cc, N = st.nb, st.K, st.C, st.N
+    R = _chk(R, "R", (nb, 3, 3)); T = _chk(T, "T", (nb, 3, 1))
+    Wt = None if K == 0 else _chk(W, "W", (nb, K, 1))
+    dc = _chk(dcost.reshape(-1), "dcost", (nb,))
+    dev = R.device
+    dconv1 = torch.empty(nb, N, Cc, device=dev); dconv2 = torch.empty(nb, st.h, st.w, st.conv2_channels, device=dev)
+    dD = torch.empty(nb, N, 1, device=dev); dB = None if K == 0 else torch.empty(nb, N, K, device=dev)
+    dR = torch.empty(nb, 3, 3, device=dev); dT = torch.empty(nb, 3, 1, device=dev); dW = None if K == 0 else torch.empty(nb, K, 1, device=dev)
+    dweight = torch.empty(nb, N, 1, device=dev) if return_dweight else None
+    check(lib.banet_lm_cost_bwd(C.byref(st), R.data_ptr(), T.data_ptr(), _ptr(Wt), dc.data_ptr(), dconv1.data_ptr(), dconv2.data_ptr(),
+                                dD.data_ptr(), _ptr(dB), dR.data_ptr(), dT.data_ptr(), _ptr(dW), _ptr(dweight), _stream()), "banet_lm_cost_bwd")
+    out = (dconv1, dconv2, dD, dB, dR, dT, dW)
+    return out + (dweight,) if return_dweight else out
+
+
 def pack_mlp(params: Sequence[Tuple[Tensor, Tensor]]) -> Tensor:
     """[(W1[cin,cout], b1[cout]), ...x5] -> packed fp32 buffer expected by banet_lm_lambda."""
     return torch.cat([t.reshape(-1).to(torch.float32) for wb in params for t in wb]).contiguous()

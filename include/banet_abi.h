@@ -210,6 +210,33 @@ int    banet_lm_step(const float* H, const float* g, const float* rbar_sum, int 
                      const float* R, const float* T, const float* W, float* R_out, float* T_out, float* W_out,
                      float* delta, float* lambda_out, int32_t* status, banet_stream_t stream);
 
+/* Feature-metric cost of a level at an iterate: the energy every build takes one (IRLS) step on, read back.  For the level's pairs at
+ * R [nb,3,3], T [nb,3,1], W [nb,K,1] (NULL when K = 0), any layout, dtypes, point weights, robust loss and grid hint, K = 0 ... 256:
+ *   s_n = sum_c d_{n,c}^2 in fp32 over the channels, d exactly the build's residual (the same warp, mask -- non-finite projections
+ *         included -- and bilinear sample of the F2 values; on the [F2|gx|gy] layout the gradient channels are never read);
+ *   cost[b] = sum_n c_n rho(s_n) over the in-bounds points of pair b: c_n the point weight (1 when weight is NULL), rho the level's loss
+ *         (rho(s) = s for BANET_ROBUST_NONE; Huber and Cauchy as stated above), each term c_n rho(s_n) in fp32, the sum in fp64 in a fixed
+ *         order, stored as fp32: bit-reproducible, independent of the workspace's contents and of the grid;
+ *   nvalid[b] = the in-bounds count, bit for bit banet_lm_build's nvalid;
+ *   s [nb,N,1] (0 at masked points) and mask [nb,N,1] (1 / 0): optional per-point outputs, not written when NULL.
+ * No precision argument: there is no contraction.  Argument errors, reported before any CUDA call: the level's (as banet_lm_build), a null
+ * R, T, cost or nvalid, K > 0 with W NULL (BANET_ERR_BAD_ARG); K > 256 (BANET_ERR_UNSUPPORTED); ws smaller than
+ * banet_lm_cost_workspace_bytes (BANET_ERR_WORKSPACE).  The workspace query returns 0 for a level it rejects. */
+size_t banet_lm_cost_workspace_bytes(const banet_level_t* lv);
+int    banet_lm_cost(const banet_level_t* lv, const float* R, const float* T, const float* W,
+                     float* cost, float* nvalid, float* s, float* mask, void* ws, size_t ws_bytes, banet_stream_t stream);
+/* Its backward, given dcost [nb] (s and mask carry no gradient): every valid point gets dd_{n,c} = 2 dcost_b c_n rho'(s_n) d_{n,c}, carried
+ * by the chain rule to dconv1 [nb,N,C], dconv2 [nb,h,w,conv2_channels] (fp32, the level's layout: on [F2|gx|gy] the gradient channels are
+ * exactly zero), and through the sampler's coordinates and the projection to dD [nb,N,1], dB [nb,N,K], dW [nb,K,1], dR [nb,3,3],
+ * dT [nb,3,1]; dweight [nb,N,1] (may be NULL) = dcost_b rho(s_n).  The exact derivative of cost as computed, through the bilinear sample of
+ * F2 (not the build's Gauss-Newton gradient from gx, gy); intr and p are constants, as in banet_lm_build_bwd, and so is robust_scale.
+ * Masked points, and every point of a pair with dcost = 0, get zero gradients.  Every output is overwritten; dconv1, dD, dB and dweight
+ * have one writer per element, dconv2, dR, dT and dW are accumulated with fp32 atomics.  Argument errors as banet_lm_cost's (with dcost,
+ * dconv1, dconv2, dD, dR, dT required, and dB, dW when K > 0), reported before any CUDA call.  No workspace. */
+int    banet_lm_cost_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dcost,
+                         float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
+                         float* dweight, banet_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * (3b) Backward of one LM iteration — the gradient signature of the reference's BA layer: TF autodiff of
  *      bundlenet.py:193-278 with the registered op gradient EquationConstructionGrad (bundlenet.py:79-82,
