@@ -116,6 +116,9 @@ SIGNATURES = {
     "banet_lm_keyframe_build": (C.c_int, [C.POINTER(BanetKeyframeLevel)] + [c_float_p] * 3 + [c_float_p] * 4 + [C.c_void_p, C.c_size_t, c_stream]),
     "banet_lm_keyframe_build_bwd": (C.c_int, [C.POINTER(BanetKeyframeLevel)] + [c_float_p] * 6 + [C.c_int] + [c_float_p] * 7 + [c_stream]),
     "banet_lm_keyframe_build_bwd_weighted": (C.c_int, [C.POINTER(BanetKeyframeLevel)] + [c_float_p] * 6 + [C.c_int] + [c_float_p] * 8 + [c_stream]),
+    "banet_lm_keyframe_cost_workspace_bytes": (C.c_size_t, [C.POINTER(BanetKeyframeLevel)]),
+    "banet_lm_keyframe_cost": (C.c_int, [C.POINTER(BanetKeyframeLevel)] + [c_float_p] * 3 + [c_float_p] * 4 + [C.c_void_p, C.c_size_t, c_stream]),
+    "banet_lm_keyframe_cost_bwd": (C.c_int, [C.POINTER(BanetKeyframeLevel)] + [c_float_p] * 4 + [c_float_p] * 8 + [c_stream]),
     "banet_lm_keyframe_run_workspace_bytes": (C.c_size_t, [C.POINTER(BanetKeyframeLevel), C.c_int, C.c_int]),
     "banet_lm_keyframe_run": (C.c_int, [C.POINTER(BanetKeyframeLevel), C.c_int, C.c_int, C.POINTER(C.c_void_p), C.c_float, C.c_float,
                                         C.POINTER(BanetSolveOpts), C.c_int] + [c_float_p] * 3 + [C.c_void_p]

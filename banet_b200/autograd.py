@@ -251,6 +251,38 @@ class _KeyframeBuildFn(torch.autograd.Function):
         return dconv1, dconv2, dD, dB, dR, dT, dW.reshape(W.shape), None, None, None, dweight
 
 
+class _KeyframeCostFn(torch.autograd.Function):
+    """cost [nw*nf] = banet_lm_keyframe_cost(...); backward = banet_lm_keyframe_cost_bwd.  conv1 [nw,N,C], D, B, p once per window; conv2,
+    intr, R, T per pair; W [nw,K,1].  Saves the inputs only: no per-frame copy of the keyframe."""
+
+    @staticmethod
+    def forward(ctx, conv1, conv2, D, B, R, T, W, intr, p, weight):
+        lv = ops.KeyframeLevel(conv1, conv2, intr, p, D, B, weight=weight)
+        cost, _nvalid = ops.lm_keyframe_cost(lv, R, T, W)
+        ctx.save_for_backward(conv1, conv2, D, B, R, T, W, intr, p, weight if weight is not None else conv1.new_empty(0))
+        ctx.has_weight = weight is not None
+        return cost
+
+    @staticmethod
+    def backward(ctx, dcost):
+        conv1, conv2, D, B, R, T, W, intr, p, weight = ctx.saved_tensors
+        if not ctx.has_weight:
+            weight = None
+        lv = ops.KeyframeLevel(conv1, conv2, intr, p, D, B, weight=weight)
+        want_dw = weight is not None and ctx.needs_input_grad[9]
+        grads = ops.lm_keyframe_cost_bwd(lv, R, T, W, dcost.contiguous(), return_dweight=want_dw)
+        dconv1, dconv2, dD, dB, dR, dT, dW = grads[:7]
+        return dconv1, dconv2, dD, dB, dR, dT, dW, None, None, grads[7] if want_dw else None
+
+
+def window_feature_metric_cost(conv1, conv2, D, B, R, T, W, intr, p, weight: Optional[Tensor] = None) -> Tensor:
+    """The feature-metric cost of keyframe windows at (R, T, W), differentiable: conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K] once
+    per window; conv2 [nw*nf,h,w,3C] or [nw*nf,h,w,C], intr [nw*nf,4], R [nw*nf,3,3], T [nw*nf,3,1] per pair; W [nw,K,1]; weight
+    [nw*nf,N,1] or None -> cost [nw*nf] (ops.lm_keyframe_cost), with gradients w.r.t. conv1, conv2 (either layout), D, B, R, T, W and weight
+    (banet_lm_keyframe_cost_bwd).  intr and p are constants.  Nothing of the keyframe is copied per frame, in the forward or for the backward."""
+    return _KeyframeCostFn.apply(conv1, conv2, D, B, R, T, W, intr.detach(), p.detach(), weight)
+
+
 class _LMSolveUpdateFn(torch.autograd.Function):
     """(R', T', W') = banet_lm_solve_update(H, g, lambda, R, T, W); backward = banet_lm_solve_update_bwd."""
 

@@ -181,6 +181,52 @@ class BundleNet(torch.nn.Module):
         lv = ops.Level(conv1, conv2, intr, p, D, B, weight=weight, robust=robust, robust_scale=robust_scale)
         return ops.lm_cost(lv, R, T, W)[0]
 
+    def WindowFeatureMetricCost(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, *, weight: Optional[Tensor] = None) -> Tensor:
+        """The energy the keyframe form of WindowIteration takes one step on, at (R, T, W) (an extension): [nw,nf], entry (w, f) = sum_n
+        c_n |d_n|^2 over the keyframe points of window w in bounds in frame f, d_n the point's feature-metric residual and c_n its weight
+        (ones when None).  Arguments as WindowIteration's keyframe form: conv1 [nw,N,C], p [nw,3,N], D [nw,N,1], B [nw,N,K] once per window,
+        conv2 [nw,nf,h,w,3C] or F2 only [nw,nf,h,w,C], fx, fy, ox, oy [nw,1|nf,...], R [nw,nf,3,3], T [nw,nf,3,1], W [nw,K,1], weight
+        [nw,nf|1,N,1]; float32 only.  Differentiable in conv1, conv2, D, B, R, T, W and weight whenever gradients are being recorded
+        (autograd.window_feature_metric_cost), e.g. as a training loss without ground-truth poses; otherwise one no-grad kernel
+        (ops.lm_keyframe_cost).  Nothing of the keyframe is copied per frame."""
+        intr = torch.stack([t.reshape(t.shape[0], t.shape[1], -1)[..., 0] for t in (fx, fy, ox, oy)], dim=-1).to(torch.float32)   # [nw,1|nf,4]
+        return self._window_cost(conv1, conv2, intr, p, D, B, R, T, W, weight)
+
+    def _window_cost(self, conv1, conv2, intr, p, D, B, R, T, W, weight=None) -> Tensor:
+        """WindowFeatureMetricCost with intr [nw,1|nf,4]; its arguments are checked against each other before any kernel runs."""
+        def fail(name, t, want):
+            got = tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__
+            raise _lib.BanetError(f"WindowFeatureMetricCost: {name} must be {want}; got {got}")
+
+        for name, t in (("conv1", conv1), ("conv2", conv2), ("D", D), ("B", B), ("R", R), ("T", T), ("W", W)):
+            if not isinstance(t, torch.Tensor) or t.dtype != torch.float32:
+                raise _lib.BanetError(f"WindowFeatureMetricCost: {name} must be a float32 tensor (the keyframe layout is fp32 only); got "
+                                      f"{getattr(t, 'dtype', type(t).__name__)}")
+        if R.dim() != 4 or tuple(R.shape[2:]) != (3, 3):
+            fail("R", R, "[nw,nf,3,3]")
+        nw, nf = R.shape[0], R.shape[1]
+        if conv1.dim() != 3 or conv1.shape[0] != nw:
+            fail("conv1", conv1, f"[nw={nw},N,C]")
+        N, C = conv1.shape[1], conv1.shape[2]
+        if B.dim() != 3 or tuple(B.shape[:2]) != (nw, N):
+            fail("B", B, f"[nw={nw},N={N},K]")
+        K = B.shape[2]
+        for name, t, want in (("p", p, (nw, 3, N)), ("D", D, (nw, N, 1)), ("T", T, (nw, nf, 3, 1)), ("W", W, (nw, K, 1))):
+            if tuple(t.shape) != want:
+                fail(name, t, f"[{','.join(map(str, want))}]")
+        if conv2.dim() != 5 or tuple(conv2.shape[:2]) != (nw, nf) or conv2.shape[4] not in (C, 3 * C):
+            fail("conv2", conv2, f"[nw={nw},nf={nf},h,w,3C|C] with C={C}")
+        if intr.dim() != 3 or intr.shape[0] != nw or intr.shape[1] not in (1, nf):
+            fail("fx, fy, ox, oy", intr, f"[nw={nw},1|nf={nf},...]")
+        nb = nw * nf
+        wf = None if weight is None else _ag.window_weights(weight, nw, nf, N)
+        intr = intr.expand(nw, nf, 4).reshape(nb, 4).contiguous()
+        conv2 = conv2.reshape(nb, *conv2.shape[2:])
+        Rf, Tf = R.reshape(nb, 3, 3), T.reshape(nb, 3, 1)
+        if torch.is_grad_enabled() and any(isinstance(t, Tensor) and t.requires_grad for t in (conv1, conv2, D, B, R, T, W, weight)):
+            return _ag.window_feature_metric_cost(conv1, conv2, D, B, Rf, Tf, W, intr, p, weight=wf).reshape(nw, nf)
+        return ops.lm_keyframe_cost(ops.KeyframeLevel(conv1, conv2, intr, p, D, B, weight=wf), Rf, Tf, W)[0].reshape(nw, nf)
+
     def WindowIteration(self, conv1, conv2, fx, fy, ox, oy, p, D, B, R, T, W, l2_regularizer_base=None, level=None, *,
                         weight: Optional[Tensor] = None, robust: Optional[str] = None, robust_scale: float = 0.0):
         """One joint LM iteration of a keyframe window (an extension; the reference's layer is 2-view): the nf pairs (keyframe -> frame f)
@@ -390,7 +436,8 @@ class BundleNet(torch.nn.Module):
         return Rs, Ts, Ds
 
     def WindowResize(self, intrisic, key_layers, frame_layers, points, basis, init_depth, init_rotation=None, init_translation=None,
-                     weight: Optional[Tensor] = None, *, robust: Optional[str] = None, robust_scale: Union[float, Mapping[str, float]] = 0.0):
+                     weight: Optional[Tensor] = None, *, robust: Optional[str] = None, robust_scale: Union[float, Mapping[str, float]] = 0.0,
+                     return_cost: bool = False):
         """BundleResize's schedule (reference bundlenet.py:332-399) for nw keyframe windows of nf frames (an extension): levels 2, 3 x one
         joint window iteration, the keyframe depth init_depth + basis.W shared by the window's frames.
           intrisic [nw,4,1]            one camera per window (keyframe rays and every frame's projection)
@@ -405,7 +452,11 @@ class BundleNet(torch.nn.Module):
         AUTO or FP32_SIMT, float32 pyramids and a float32 basis only, like the keyframe form of WindowIteration.
         weight [nw,nf,N,1] or [nw,1,N,1] float32 (an extension): a per-(frame, point) confidence at `points`, the same at both levels (see
         WindowIteration); differentiable when it requires grad.
-        robust: the keyframe build has no robust loss, so a robust loss raises; WindowIteration's per-pair form takes one."""
+        robust: the keyframe build has no robust loss, so a robust loss raises; WindowIteration's per-pair form takes one.
+        return_cost=True (an extension) -> (Rs, Ts, depths, Es): Es[i] [nw,nf] is level i's feature-metric cost (WindowFeatureMetricCost) at
+        that level's output pose and depth coefficients, on its conv1, rays, depth, basis and weight and the frames' F2 maps as given (no
+        [F2|gx|gy] copy); differentiable whenever the resize is, so it can train both pyramids without ground-truth poses.  Rs, Ts, depths and
+        last_status are those of return_cost=False."""
         if self.vmatrix_batch_scramble:
             raise RuntimeError("vmatrix_batch_scramble=True is a 2-view quirk (bundlenet.py:45); the window solve has per-frame VMatrix only")
         self._require_keyframe_plain_loss(robust)
@@ -427,7 +478,7 @@ class BundleNet(torch.nn.Module):
         T = torch.zeros(nw, nf, 3, 1, device=dev) if init_translation is None else init_translation
         W = torch.zeros(nw, K, 1, device=dev)
         oh, ow = self.geo.out_hw
-        Rs, Ts, Ds = [], [], []
+        Rs, Ts, Ds, Es = [], [], [], []
         status = None
         for level in range(2, 4):                                              # :376
             scale = 2 ** (3 - level)
@@ -442,8 +493,10 @@ class BundleNet(torch.nn.Module):
             Rs.append(R); Ts.append(T)
             depth = compose(init_depth.reshape(nw, -1), basis.reshape(nw, -1, K), W)   # :397
             Ds.append(depth.reshape(nw, oh, ow, 1))
+            if return_cost:
+                Es.append(self._window_cost(conv1, F2, (intr / scale).unsqueeze(1), p, d, b, R, T, W, weight))
         self._check_status(status)
-        return Rs, Ts, Ds
+        return (Rs, Ts, Ds, Es) if return_cost else (Rs, Ts, Ds)
 
     def _window_resize_shapes(self, intrisic, key_layers, frame_layers, points, basis, init_depth, init_rotation, init_translation):
         """WindowResize's arguments checked against each other before any kernel runs -> (nw, nf, K).  nw comes from key_layers[3], nf from

@@ -713,6 +713,33 @@ extern "C" int banet_lm_keyframe_build_bwd(const banet_keyframe_level_t* lv, con
     return banet_lm_keyframe_build_bwd_weighted(lv, R, T, W, dH, dg, drbar_sum, exact_sym, dconv1, dconv2, dD, dB, dR, dT, dW, nullptr, stream);
 }
 
+extern "C" size_t banet_lm_keyframe_cost_workspace_bytes(const banet_keyframe_level_t* lv)
+{
+    if (check_keyframe_level(lv, "lm_keyframe_cost_workspace_bytes")) return 0;
+    return keyframe_cost_ws_bytes(lv);
+}
+
+extern "C" int banet_lm_keyframe_cost(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W, float* cost, float* nvalid,
+                                      float* s, float* mask, void* ws, size_t ws_bytes, banet_stream_t stream)
+{
+    int rc = check_keyframe_level(lv, "lm_keyframe_cost");
+    if (rc) return rc;
+    BANET_REQUIRE(R && T && W && cost && nvalid, BANET_ERR_BAD_ARG, "lm_keyframe_cost: null pointer");
+    const size_t need = keyframe_cost_ws_bytes(lv);
+    BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_keyframe_cost: workspace %zu < %zu bytes", ws_bytes, need);
+    return keyframe_cost(lv, R, T, W, cost, nvalid, s, mask, ws, (cudaStream_t)stream);
+}
+
+extern "C" int banet_lm_keyframe_cost_bwd(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W, const float* dcost,
+                                          float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, float* dweight,
+                                          banet_stream_t stream)
+{
+    int rc = check_keyframe_level(lv, "lm_keyframe_cost_bwd");
+    if (rc) return rc;
+    BANET_REQUIRE(R && T && W && dcost && dconv1 && dconv2 && dD && dB && dR && dT && dW, BANET_ERR_BAD_ARG, "lm_keyframe_cost_bwd: null pointer");
+    return keyframe_cost_bwd(lv, R, T, W, dcost, dconv1, dconv2, dD, dB, dR, dT, dW, dweight, (cudaStream_t)stream);
+}
+
 extern "C" size_t banet_lm_keyframe_run_workspace_bytes(const banet_keyframe_level_t* levels, int nlevels, int precision)
 {
     if (!levels || nlevels <= 0 || check_keyframe_precision(precision, "lm_keyframe_run")) return 0;

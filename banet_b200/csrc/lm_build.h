@@ -148,6 +148,14 @@ int lm_cost(const banet_level_t* lv, const float* R, const float* T, const float
             void* ws, cudaStream_t st);
 int lm_cost_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dcost, float* dconv1, float* dconv2,
                 float* dD, float* dB, float* dR, float* dT, float* dW, float* dweight, cudaStream_t st);
+// the fixed-order fp64 sum of nb pairs' tile slots partials [nb][tiles_per_pair][2] -> cost, nvalid (lm_cost.cu)
+int launch_cost_reduce(const double* partials, int nb, int tiles_per_pair, float* cost, float* nvalid, cudaStream_t st);
+// the same cost on keyframe windows (lm_window_cost.cu): the keyframe's tiles walked over the frames; ws: keyframe_cost_ws_bytes
+size_t keyframe_cost_ws_bytes(const banet_keyframe_level_t* lv);
+int keyframe_cost(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W, float* cost, float* nvalid, float* s,
+                  float* mask, void* ws, cudaStream_t st);
+int keyframe_cost_bwd(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W, const float* dcost, float* dconv1,
+                      float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW, float* dweight, cudaStream_t st);
 // the SE(3) update backward of nb poses (ddelta[0:6] of pose b -> ddelta + b * P)
 int launch_pose_update_bwd(const float* delta, int nb, int P, const float* R, const float* T, const float* gRn, const float* gTn,
                            float* ddelta, float* dR, float* dT, cudaStream_t st);

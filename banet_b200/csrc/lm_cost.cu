@@ -18,14 +18,10 @@
 #include "features.cuh"
 #include "lm_build.h"
 #include "point.cuh"
+#include "cost_tile.cuh"
 #include <string.h>
 
 namespace banet {
-
-constexpr int COST_TILE = 64;
-constexpr int COST_THREADS = 256;
-constexpr int COST_WARPS = COST_THREADS / 32;
-enum { CR_IDX = 0, CR_X0, CR_Y0, CR_DX, CR_DY, CR_MASK, CR_DT, CR_DU, CR_DV, CR_VAL, CR_ARRAYS };
 
 struct CostParams {
     int nb, N, C, K, KP, h, w;
@@ -110,11 +106,6 @@ __device__ __forceinline__ void cost_pair_constants(const CostParams& prm, int b
     else if (tid < 12) sPose[tid] = prm.T[(size_t)b * 3 + tid - 9];
     else if (tid < 16) sPose[tid] = prm.intr[(size_t)b * 4 + tid - 12];
     for (int k = tid; k < prm.KP; k += COST_THREADS) sW[k] = (k < prm.K) ? prm.W[(size_t)b * prm.K + k] : 0.f;
-}
-
-__device__ __forceinline__ Taps cost_taps(const float* rec, int i, int h, int w) {
-    return Taps(__float_as_int(rec[CR_X0 * COST_TILE + i]), __float_as_int(rec[CR_Y0 * COST_TILE + i]), rec[CR_DX * COST_TILE + i],
-                rec[CR_DY * COST_TILE + i], h, w);
 }
 
 // TF: feature element type; TB: basis element type; FLY: conv2 is F2 only (C channels per texel), else [F2|gx|gy] (3C, only the first C
@@ -369,6 +360,14 @@ static int cost_launch(CostKernel kern, const CostParams& prm, cudaStream_t st, 
     return BANET_OK;
 }
 
+int launch_cost_reduce(const double* partials, int nb, int tiles_per_pair, float* cost, float* nvalid, cudaStream_t st)
+{
+    const long long blocks = ((long long)nb * 32 + 255) / 256;
+    lm_cost_reduce_kernel<<<(unsigned)(blocks < (1LL << 20) ? blocks : (1LL << 20)), 256, 0, st>>>(partials, nb, tiles_per_pair, cost, nvalid);
+    BANET_CUDA_LAUNCH_CHECK("lm_cost_reduce_kernel launch");
+    return BANET_OK;
+}
+
 int lm_cost(const banet_level_t* lv, const float* R, const float* T, const float* W, float* cost, float* nvalid, float* s, float* mask,
             void* ws, cudaStream_t st)
 {
@@ -376,10 +375,7 @@ int lm_cost(const banet_level_t* lv, const float* R, const float* T, const float
     prm.partials = reinterpret_cast<double*>(ws); prm.s_out = s; prm.mask_out = mask;
     int rc = cost_launch(pick_cost_kernel<PickFwd>(lv), prm, st, "lm_cost_kernel launch");
     if (rc) return rc;
-    const long long blocks = ((long long)lv->nb * 32 + 255) / 256;
-    lm_cost_reduce_kernel<<<(unsigned)(blocks < (1LL << 20) ? blocks : (1LL << 20)), 256, 0, st>>>(prm.partials, lv->nb, prm.tiles_per_pair, cost, nvalid);
-    BANET_CUDA_LAUNCH_CHECK("lm_cost_reduce_kernel launch");
-    return BANET_OK;
+    return launch_cost_reduce(prm.partials, lv->nb, prm.tiles_per_pair, cost, nvalid, st);
 }
 
 int lm_cost_bwd(const banet_level_t* lv, const float* R, const float* T, const float* W, const float* dcost, float* dconv1, float* dconv2,

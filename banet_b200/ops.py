@@ -542,6 +542,46 @@ def lm_keyframe_build_bwd(level: KeyframeLevel, R: Tensor, T: Tensor, W: Tensor,
     return dconv1, dconv2, dD, dB, dR, dT, dW, dweight
 
 
+def lm_keyframe_cost(level: KeyframeLevel, R: Tensor, T: Tensor, W: Tensor, per_point: bool = False):
+    """Feature-metric cost of keyframe windows at (R, T, W) (banet_lm_keyframe_cost): R [nw*nf,3,3], T [nw*nf,3,1], W [nw,K,1] -> cost
+    [nw*nf] = sum_n c_n s_n over the in-bounds points of each pair (w*nf + f), s_n the squared norm of the keyframe build's residual and c_n
+    the level's weight, and nvalid [nw*nf], bit for bit lm_keyframe_build's.  Bit for bit lm_cost on the keyframe replicated per frame.
+    per_point=True appends s [nw*nf,N,1] (0 at masked points) and mask [nw*nf,N,1]."""
+    lib = load()
+    st, keep = level.as_struct()
+    nw, nb, K, N = st.nw, st.nw * st.nf, st.K, st.N
+    R = _chk(R, "R", (nb, 3, 3)); T = _chk(T, "T", (nb, 3, 1)); Wt = _chk(W, "W", (nw, K, 1))
+    dev = R.device
+    cost = torch.empty(nb, device=dev); nvalid = torch.empty(nb, device=dev)
+    s = torch.empty(nb, N, 1, device=dev) if per_point else None
+    mask = torch.empty(nb, N, 1, device=dev) if per_point else None
+    ws = _ws(lib.banet_lm_keyframe_cost_workspace_bytes(C.byref(st)), dev)
+    check(lib.banet_lm_keyframe_cost(C.byref(st), R.data_ptr(), T.data_ptr(), Wt.data_ptr(), cost.data_ptr(), nvalid.data_ptr(), _ptr(s),
+                                     _ptr(mask), ws.data_ptr(), ws.numel(), _stream()), "banet_lm_keyframe_cost")
+    return (cost, nvalid, s, mask) if per_point else (cost, nvalid)
+
+
+def lm_keyframe_cost_bwd(level: KeyframeLevel, R: Tensor, T: Tensor, W: Tensor, dcost: Tensor, return_dweight: bool = False):
+    """Backward of lm_keyframe_cost's cost (banet_lm_keyframe_cost_bwd): dcost [nw*nf] -> dconv1 [nw,N,C], dconv2 (conv2's layout, zero
+    gradient channels on [F2|gx|gy]), dD [nw,N,1], dB [nw,N,K], dR, dT [nw*nf,...], dW [nw,K,1] (+ dweight [nw*nf,N,1] = dcost s_n with
+    return_dweight): the exact derivative through the bilinear sample of F2, the keyframe's gradients summed over the frames."""
+    lib = load()
+    st, keep = level.as_struct()
+    nw, nb, K, Cc, N = st.nw, st.nw * st.nf, st.K, st.C, st.N
+    R = _chk(R, "R", (nb, 3, 3)); T = _chk(T, "T", (nb, 3, 1)); Wt = _chk(W, "W", (nw, K, 1))
+    dc = _chk(dcost.reshape(-1), "dcost", (nb,))
+    dev = R.device
+    dconv1 = torch.empty(nw, N, Cc, device=dev); dconv2 = torch.empty(nb, st.h, st.w, st.conv2_channels, device=dev)
+    dD = torch.empty(nw, N, 1, device=dev); dB = torch.empty(nw, N, K, device=dev)
+    dR = torch.empty(nb, 3, 3, device=dev); dT = torch.empty(nb, 3, 1, device=dev); dW = torch.empty(nw, K, 1, device=dev)
+    dweight = torch.empty(nb, N, 1, device=dev) if return_dweight else None
+    check(lib.banet_lm_keyframe_cost_bwd(C.byref(st), R.data_ptr(), T.data_ptr(), Wt.data_ptr(), dc.data_ptr(), dconv1.data_ptr(),
+                                         dconv2.data_ptr(), dD.data_ptr(), dB.data_ptr(), dR.data_ptr(), dT.data_ptr(), dW.data_ptr(),
+                                         _ptr(dweight), _stream()), "banet_lm_keyframe_cost_bwd")
+    out = (dconv1, dconv2, dD, dB, dR, dT, dW)
+    return out + (dweight,) if return_dweight else out
+
+
 def lm_keyframe_run(levels: Sequence[KeyframeLevel], iters_per_level: int, R: Tensor, T: Tensor, W: Tensor,
                     mlp_packed: Optional[Sequence[Optional[Tensor]]] = None, l2_regularizer_base: float = 1000.0,
                     lambda_fixed: float = -1.0, damping_eps: float = 1e-5, undamped_last: bool = True,

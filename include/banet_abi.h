@@ -466,6 +466,29 @@ int    banet_lm_keyframe_build_bwd_weighted(const banet_keyframe_level_t* lv, co
                                             const float* dH, const float* dg, const float* drbar_sum, int exact_sym,
                                             float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
                                             float* dweight, banet_stream_t stream);
+/* Feature-metric cost of keyframe windows: banet_lm_cost on this layout.  At R [nw*nf,3,3], T [nw*nf,3,1], W [nw,K,1], pair b = w*nf + f:
+ *   s_{b,n} = sum_c d^2,  d = conv1[w,n] - F2_b(pi(p[w,n], D[w,n] + B[w,n].W_w; R_b, T_b)): exactly the residual the keyframe build gathers
+ *         (its depth arithmetic, projection, mask -- non-finite projections included -- and bilinear sample of the F2 values; on the
+ *         [F2|gx|gy] layout the gradient channels are never read);
+ *   cost[b] = sum_n c_{b,n} s_{b,n} over the in-bounds points of pair b, c the level's weight (1 when NULL), each term in fp32, the sum in fp64
+ *         in a fixed order, stored as fp32: bit-reproducible, independent of the workspace's contents and of the grid;
+ *   nvalid[b] = banet_lm_keyframe_build's nvalid, bit for bit;  s, mask [nw*nf,N,1]: optional, as in banet_lm_cost.
+ * cost, nvalid, s and mask equal banet_lm_cost's on the replicated layout (the keyframe tensors and W repeated per frame, no grid hint) bit
+ * for bit.  No robust loss (the keyframe layout has none: the keyframe build minimises exactly this energy); both conv2 layouts.  Argument
+ * errors, reported before any CUDA call: the level's (as banet_lm_keyframe_build), a null R, T, W, cost or nvalid (BANET_ERR_BAD_ARG); ws
+ * smaller than banet_lm_keyframe_cost_workspace_bytes (BANET_ERR_WORKSPACE).  The workspace query returns 0 for a level it rejects. */
+size_t banet_lm_keyframe_cost_workspace_bytes(const banet_keyframe_level_t* lv);
+int    banet_lm_keyframe_cost(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W,
+                              float* cost, float* nvalid, float* s, float* mask, void* ws, size_t ws_bytes, banet_stream_t stream);
+/* Its backward, given dcost [nw*nf]: the exact derivative through the bilinear sample of F2, as banet_lm_cost_bwd states it (intr and p are
+ * constants).  dconv1 [nw,N,C], dD [nw,N,1], dB [nw,N,K]: summed over the frames in frame order and stored once, one writer each,
+ * bit-reproducible; dconv2 [nw*nf,h,w,conv2_channels] (the level's layout; on [F2|gx|gy] the gradient channels are exactly zero), dR
+ * [nw*nf,3,3], dT [nw*nf,3,1] per pair and dW [nw,K,1] per window, accumulated with fp32 atomics; dweight [nw*nf,N,1] (may be NULL) =
+ * dcost_b s_{b,n}, one writer.  Masked points, and pairs with dcost = 0, contribute nothing.  Every output is overwritten.  Argument errors as
+ * banet_lm_keyframe_cost's (with dcost, dconv1, dconv2, dD, dB, dR, dT, dW required), reported before any CUDA call.  No workspace. */
+int    banet_lm_keyframe_cost_bwd(const banet_keyframe_level_t* lv, const float* R, const float* T, const float* W, const float* dcost,
+                                  float* dconv1, float* dconv2, float* dD, float* dB, float* dR, float* dT, float* dW,
+                                  float* dweight, banet_stream_t stream);
 /* Whole coarse-to-fine solve (banet_lm_window_batch_run with keyframe levels): each iteration is one keyframe-build launch (plus its fp64
  * slot reduction) and one window-step launch, the lambda-MLP or lambda_fixed as in (3d).  W [nw,K,1] is read by the build directly (no
  * per-pair copies).  levels[l].nw, nf, K must agree across levels.  precision: BANET_PREC_AUTO or BANET_PREC_FP32_SIMT (AUTO resolves to
