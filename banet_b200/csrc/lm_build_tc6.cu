@@ -320,33 +320,8 @@ lm_build_tc6_kernel(const __grid_constant__ CUtensorMap tmapB, const BuildParams
             else if (grid2d) { nxt.tx0 += 8; if (nxt.tx0 >= prm.tiles_x * 8) { nxt.tx0 = 0; nxt.ty0 += 8; } }
             else { nxt.n0 += TILE; nxt.cnt = min(TILE, N - nxt.n0); }
             const int b = tc.b;
-            if (gwi == 1 && j + 2 < ntiles) {             // L2 prefetch of the streaming inputs (conv1, p, D) two tiles ahead
-                const TileCoord tn = tile_coord(prm, t_begin + j + 2);
-                if (grid2d) {
-                    if (lane < 8) {
-                        const int gy = tn.ty0 + lane;
-                        if (gy < prm.grid_h && tn.tx0 < prm.grid_w) {
-                            const size_t n = (size_t)gy * prm.grid_w + tn.tx0;
-                            const int wpx = min(8, prm.grid_w - tn.tx0);
-                            prefetch_l2_bulk(static_cast<const TF*>(prm.conv1) + ((size_t)tn.b * N + n) * C, (uint32_t)(wpx * C * sizeof(TF)));
-                            if ((n & 3) == 0 && (N & 3) == 0) {
-                                const uint32_t by = (uint32_t)(((wpx * 4) + 15) & ~15);
-                                prefetch_l2_bulk(prm.D + (size_t)tn.b * N + n, by);
-#pragma unroll
-                                for (int k = 0; k < 3; ++k) prefetch_l2_bulk(prm.p + ((size_t)tn.b * 3 + k) * N + n, by);
-                            }
-                        }
-                    }
-                } else if (lane == 0) {
-                    prefetch_l2_bulk(static_cast<const TF*>(prm.conv1) + ((size_t)tn.b * N + tn.n0) * C, (uint32_t)(tn.cnt * C * sizeof(TF)));
-                    if ((N & 3) == 0) {
-                        const uint32_t by = (uint32_t)(((tn.cnt * 4) + 15) & ~15);
-                        prefetch_l2_bulk(prm.D + (size_t)tn.b * N + tn.n0, by);
-#pragma unroll
-                        for (int k = 0; k < 3; ++k) prefetch_l2_bulk(prm.p + ((size_t)tn.b * 3 + k) * N + tn.n0, by);
-                    }
-                }
-            }
+            // No L2 bulk prefetch of the streaming inputs (conv1, p, D) ahead of the tile: issued two tiles ahead, it made the TF32X1 build
+            // 10 % slower at 640x480 on H100, with bitwise the same outputs (DESIGN.md section 5).
             if (b != geom_b) {
                 geom_b = b;
                 __syncwarp();
