@@ -48,8 +48,7 @@ class BanetSolveOpts(C.Structure):
 
 class BanetTuning(C.Structure):
     """struct banet_tuning (include/banet_abi.h): diagnostic knobs, defaults = production."""
-    _fields_ = [("tc_generation", C.c_int), ("tc7_force_direct", C.c_int), ("tc7_band_rows", C.c_int),
-                ("tc6_band_rows", C.c_int), ("tc6_l2_hints", C.c_int), ("tc6_tap_prefetch", C.c_int)]
+    _fields_ = [("tc6_band_rows", C.c_int), ("tc6_l2_hints", C.c_int), ("tc6_tap_prefetch", C.c_int)]
 
 
 class BanetLegacyOpts(C.Structure):
@@ -169,10 +168,15 @@ def check(rc: int, what: str) -> None:
         raise BanetError(f"{what} failed (code {rc}): {msg}")
 
 
-def set_tuning(tc_generation: int = 0, tc7_force_direct: bool = False, tc7_band_rows: int = 4, tc6_band_rows: int = 0,
-               tc6_l2_hints: int = 0, tc6_tap_prefetch: int = 0) -> None:
-    """Diagnostic knobs (process-wide); call with no arguments to restore the production defaults."""
-    t = BanetTuning(int(tc_generation), int(tc7_force_direct), int(tc7_band_rows), int(tc6_band_rows), int(tc6_l2_hints), int(tc6_tap_prefetch))
+def set_tuning(tc_generation: int = 0, tc6_band_rows: int = 0, tc6_l2_hints: int = 0, tc6_tap_prefetch: int = 0) -> None:
+    """Diagnostic knobs (process-wide); call with no arguments to restore the production defaults.
+
+    tc_generation selects nothing: generation 6 is the only tensor-core build kernel.  It still accepts 0 (default), 6 and 7, which
+    all run that kernel, so that callers written when generation 7 existed (bench.py --tc-generation {0,6,7}) keep running; any
+    other value raises BanetError."""
+    if int(tc_generation) not in (0, 6, 7):
+        raise BanetError(f"set_tuning: tc_generation must be 0, 6 or 7 (all run the one tensor-core kernel), got {tc_generation}")
+    t = BanetTuning(int(tc6_band_rows), int(tc6_l2_hints), int(tc6_tap_prefetch))
     check(load().banet_set_tuning(C.byref(t)), "banet_set_tuning")
 
 

@@ -106,11 +106,10 @@ extern "C" int banet_num_sms(void) { return num_sms(); }
 
 extern "C" int banet_set_tuning(const banet_tuning_t* t)
 {
-    const banet_tuning_t def = {0, 0, 4, 0, 0, 0};
+    const banet_tuning_t def = {0, 0, 0};
     if (!t) { set_tuning(def); return BANET_OK; }
-    BANET_REQUIRE((t->tc_generation == 0 || t->tc_generation == 6 || t->tc_generation == 7) && t->tc7_band_rows >= 1 &&
-                  t->tc6_band_rows >= 0 && t->tc6_l2_hints >= 0 && t->tc6_l2_hints <= 3 && t->tc6_tap_prefetch >= 0 && t->tc6_tap_prefetch <= 3, BANET_ERR_BAD_ARG,
-                  "set_tuning: tc_generation must be 0, 6 or 7, tc7_band_rows >= 1, tc6_band_rows >= 0, tc6_l2_hints and tc6_tap_prefetch in 0..3");
+    BANET_REQUIRE(t->tc6_band_rows >= 0 && t->tc6_l2_hints >= 0 && t->tc6_l2_hints <= 3 && t->tc6_tap_prefetch >= 0 && t->tc6_tap_prefetch <= 3, BANET_ERR_BAD_ARG,
+                  "set_tuning: tc6_band_rows >= 0, tc6_l2_hints and tc6_tap_prefetch in 0..3");
     set_tuning(*t);
     return BANET_OK;
 }

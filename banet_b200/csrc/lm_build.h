@@ -20,7 +20,6 @@ struct BuildParams {
     int tap_prefetch;                 // generation 6: 0 off, 1 the geometry warps prefetch the tap footprint into L2 (halo from the tile's border pixels), 2 = every pixel also fetches its lower row
     int l2_hints;                     // generation 6: 0 none, 1 read-once streams evict-first, 2 = 1 + taps evict-last
     int hdd_transposed;               // tensor-core path stores the H_dd block of a slot column-major
-    int force_direct;                 // generation 7, testing: take the global-tap fallback for every tile
     long long* trace;                 // optional debug timeline buffer (NULL in production)
     int robust;                       // BANET_ROBUST_*: M, q also weighted by rho'(|d|^2) (robust_rho1, common.cuh)
     float robust_scale;
@@ -51,10 +50,9 @@ int lm_build_simt(const banet_level_t* lv, const BuildPlan& plan, const float* R
 
 int launch_lm_reduce(const BuildParams& prm, int grid_build, float* H, float* g, float* rbar_sum, float* nvalid, cudaStream_t st);
 
-// tensor-core path (lm_build_tc_host.cu + lm_build_tc6.cu / lm_build_tc7.cu): K in {32,64,128}, C in {64,128}
+// tensor-core path (lm_build_tc_host.cu + lm_build_tc6.cu): K in {32,64,128}, C in {64,128}
 void set_tuning(const banet_tuning_t& t);
 const banet_tuning_t& tuning();
-void lm_build_tc7_window(int* wx, int* wy);
 bool tc_supported(const banet_level_t* lv);
 int build_plan_tc(const banet_level_t* lv, int num_sms, BuildPlan* plan);
 int lm_build_tc(const banet_level_t* lv, const BuildPlan& plan, int mode, const float* R, const float* T, const float* W,

@@ -17,12 +17,8 @@
 // Tiles: 64 points.  With the dense-grid hint (banet_level_t::grid_w/h) a tile is an 8x8 pixel patch fetched by ONE 3-D TMA box;
 // without the hint a tile is 64 consecutive points (2-D TMA box).
 //
-// Kernel generations:
-//   7 (lm_build_tc7.cu)  F2-only conv2 + dense grid: the tile's F2 footprint is staged into shared memory by TMA (channel chunks),
-//                        the 12 gradient/bilinear taps of every pixel come from LDS; per-tile fallback to global taps when the
-//                        footprint of a tile does not fit the staged window.  MODE 1 and 2.
-//   6 (lm_build_tc6.cu)  everything (both conv2 layouts, dense grids and point lists, every mode, fp32 and bf16 features, fp32 and bf16
-//                        bases): taps by ld.global.
+// Kernel: generation 6 (lm_build_tc6.cu) covers everything (both conv2 layouts, dense grids and point lists, every mode, fp32 and bf16
+// features, fp32 and bf16 bases): taps by ld.global.
 #include "common.cuh"
 #include "lm_build.h"
 #include "tc_utils.cuh"
@@ -34,28 +30,11 @@ constexpr int TC_TILE = 64;
 
 int lm_build_tc6_launch(int mode, bool fly, int nch, int kblk, bool is_bf16, bool basis_bf16, const CUtensorMap& tm, const BuildParams& prm, int grid,
                         cudaStream_t st);
-int lm_build_tc7_launch(int mode, int nch, int kblk, const CUtensorMap& tmB, const CUtensorMap& tmF, const CUtensorMap& tmC, const BuildParams& prm, int grid,
-                        cudaStream_t st);
-bool lm_build_tc7_supported(int mode, int nch, int kblk);
 
 constexpr int kTc6DefaultBandRows = 1, kTc6DefaultL2Hints = 0, kTc6DefaultTapPrefetch = 0;
-static banet_tuning_t g_tuning = {0, 0, 4, 0, 0, 0};
+static banet_tuning_t g_tuning = {0, 0, 0};
 void set_tuning(const banet_tuning_t& t) { g_tuning = t; }
 const banet_tuning_t& tuning() { return g_tuning; }
-
-// Generation 7 applies to unweighted, non-robust levels with fp32 features and an fp32 basis in the F2-only layout on a dense grid (tap coordinates are packed in 16 bits), modes 1 and 2.  The default
-// (tc_generation = 0) is generation 6 everywhere: in interleaved A/B runs on an H100 80GB HBM3 (400 W power limit, 32 pairs, F2-only
-// layout) generation 7 took 25.5 vs 21.5 ms at 640x480 and 5.8 vs 5.4 ms at 320x240 in TF32X1, and 2.3x as long in TF32X2 (its
-// gather warps run on 64 registers and spill, see DESIGN.md §4).  banet_set_tuning(tc_generation = 7) forces it where it applies.
-// It also needs a map at least as large as its staged F2 window: on a 2 x 2 map it returned non-finite H (tests/test_build_edges.py).
-static bool use_gen7(const banet_level_t* lv, int mode, int kblk)
-{
-    const bool wanted = g_tuning.tc_generation == 7;
-    int wx = 0, wy = 0;
-    lm_build_tc7_window(&wx, &wy);
-    return wanted && !lv->weight && !lv->robust && lv->feature_dtype == BANET_DTYPE_F32 && lv->basis_dtype == BANET_DTYPE_F32 && lv->conv2_channels == lv->C && lv->grid_w > 0 && lv->h < 65536 && lv->w < 65536 &&
-           lv->h >= wy && lv->w >= wx && lm_build_tc7_supported(mode, lv->C / 64, kblk);
-}
 
 // The F2-only gather packs the four tap columns of a pixel into 16 bits each (lm_build_tc6.cu, the geometry warps' cx[]), so that
 // layout needs w < 65536; a wider map resolves to the SIMT kernel under AUTO and is BANET_ERR_UNSUPPORTED in an explicit TF32 mode.
@@ -115,27 +94,13 @@ int lm_build_tc(const banet_level_t* lv, const BuildPlan& plan, int mode, const 
     prm.hdd_transposed = 1;
     prm.trace = nullptr;
     const int nch = lv->C / 64;
-    prm.force_direct = g_tuning.tc7_force_direct;
-    if (use_gen7(lv, mode, kblk)) {
-        int band = g_tuning.tc7_band_rows; if (band < 1) band = 1; if (band > prm.tiles_y) band = prm.tiles_y;
-        prm.band_rows = band;
-        CUtensorMap tmF;        // staged F2 windows: 32 channels x WX x WY texels
-        int wx = 0, wy = 0; lm_build_tc7_window(&wx, &wy);
-        rc = make_tmap_f32_nhwc(&tmF, static_cast<const float*>(lv->conv2), lv->nb, lv->h, lv->w, lv->conv2_channels, 32, wx, wy);
-        if (rc) return rc;
-        CUtensorMap tmC;        // conv1 chunk of an 8x8 tile: 32 channels x 8 x 8 pixels of [nb, grid_h, grid_w, C]
-        rc = make_tmap_f32_nhwc(&tmC, static_cast<const float*>(lv->conv1), lv->nb, lv->grid_h, lv->grid_w, lv->C, 32, 8, 8);
-        if (rc) return rc;
-        rc = lm_build_tc7_launch(mode, nch, kblk, tm, tmF, tmC, prm, plan.grid, st);
-    } else {
-        // dense grid: band walk + L2 policy (diagnostic knobs, off by default)
-        int band = g_tuning.tc6_band_rows > 0 ? g_tuning.tc6_band_rows : kTc6DefaultBandRows;
-        if (band > prm.tiles_y) band = prm.tiles_y;
-        prm.band_rows = lv->grid_w > 0 && band > 1 ? band : 1;
-        prm.l2_hints = g_tuning.tc6_l2_hints > 0 ? g_tuning.tc6_l2_hints - 1 : kTc6DefaultL2Hints;
-        prm.tap_prefetch = g_tuning.tc6_tap_prefetch > 0 ? g_tuning.tc6_tap_prefetch - 1 : kTc6DefaultTapPrefetch;
-        rc = lm_build_tc6_launch(mode, fly, nch, kblk, lv->feature_dtype == BANET_DTYPE_BF16, basis_bf16, tm, prm, plan.grid, st);
-    }
+    // dense grid: band walk + L2 policy (diagnostic knobs, off by default)
+    int band = g_tuning.tc6_band_rows > 0 ? g_tuning.tc6_band_rows : kTc6DefaultBandRows;
+    if (band > prm.tiles_y) band = prm.tiles_y;
+    prm.band_rows = lv->grid_w > 0 && band > 1 ? band : 1;
+    prm.l2_hints = g_tuning.tc6_l2_hints > 0 ? g_tuning.tc6_l2_hints - 1 : kTc6DefaultL2Hints;
+    prm.tap_prefetch = g_tuning.tc6_tap_prefetch > 0 ? g_tuning.tc6_tap_prefetch - 1 : kTc6DefaultTapPrefetch;
+    rc = lm_build_tc6_launch(mode, fly, nch, kblk, lv->feature_dtype == BANET_DTYPE_BF16, basis_bf16, tm, prm, plan.grid, st);
     if (rc) return rc;
     return launch_lm_reduce(prm, plan.grid, H, g, rbar_sum, nvalid, st);
 }

@@ -1,4 +1,4 @@
-// mma_role.cuh — the MMA warpgroup of the tensor-core build kernels (generations 6 and 7): D = A^T R of every tile by mma.sync
+// mma_role.cuh — the MMA warpgroup of the tensor-core build kernel (generation 6): D = A^T R of every tile by mma.sync
 // m16n8k8 tf32, each 8-pixel product added round-to-nearest into register accumulators that live for the whole pair span, one slot
 // write per span.
 //

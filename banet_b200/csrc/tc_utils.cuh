@@ -39,14 +39,6 @@ __device__ __forceinline__ void mbar_wait_parked(uint64_t* bar, uint32_t parity)
     asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}"
                  :: "r"(smem_u32(bar)), "r"(parity), "r"(0x989680) : "memory");
 }
-__device__ __forceinline__ void mbar_wait_sleep(uint64_t* bar, uint32_t parity) {      // for single-thread role warps: back off
-    while (!mbar_try_wait(bar, parity)) { __nanosleep(40); }
-}
-// best-effort wait (for the prefetcher, which must never hang the CTA): gives up after ~max_iters polls
-__device__ __forceinline__ bool mbar_wait_bounded(uint64_t* bar, uint32_t parity, int max_iters) {
-    for (int i = 0; i < max_iters; ++i) { if (mbar_try_wait(bar, parity)) return true; __nanosleep(64); }
-    return false;
-}
 template <int NREG> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(NREG)); }
 template <int NREG> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(NREG)); }
 
@@ -92,19 +84,9 @@ __device__ __forceinline__ float4 ldg4_hint(const float* p, uint64_t pol) {
     return r;
 }
 
-__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, int c0, int c1, int c2, int c3, uint64_t* bar) {
-    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                 :: "r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-
-// L2 prefetches (no destination, no completion): a contiguous range, or a tensor-map box
+// L2 prefetch (no destination, no completion) of a contiguous range
 __device__ __forceinline__ void prefetch_l2_bulk(const void* p, uint32_t bytes) {      // bytes % 16 == 0, p 16-B aligned
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" :: "l"(p), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void prefetch_l2_line(const void* p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
-__device__ __forceinline__ void prefetch_l2_tensor_4d(const CUtensorMap* m, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];"
-                 :: "l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 
 // ---------------------------------------------------------------- warp-level tf32 MMA on the swizzled tiles
@@ -162,7 +144,6 @@ __device__ __forceinline__ float tf32_rna(float x) {          // round to neares
 }
 // round-to-nearest (ties away) for an operand whose low 13 bits the tensor core ignores anyway: one integer add, no mask
 __device__ __forceinline__ float tf32_rna_bits(float x) { return __uint_as_float(__float_as_uint(x) + 0x1000u); }
-__device__ __forceinline__ float tf32_rna_mask(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u); }
 __device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
 }}  // namespace banet::tc

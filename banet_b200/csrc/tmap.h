@@ -63,21 +63,4 @@ inline int make_tmap_basis_3d(CUtensorMap* out, const void* base, bool bf16, uin
     return BANET_OK;
 }
 
-// fp32 NHWC map [nb, h, w, c], no swizzle: box = box_c x box_w x box_h x 1 (staged F2 windows: box_c = 32 channels = 128 B rows).
-inline int make_tmap_f32_nhwc(CUtensorMap* out, const float* base, uint64_t nb, uint64_t h, uint64_t w, uint64_t c,
-                                       uint32_t box_c, uint32_t box_w, uint32_t box_h)
-{
-    PFN_encodeTiled enc = get_encode_tiled();
-    BANET_REQUIRE(enc, BANET_ERR_CUDA, "cuTensorMapEncodeTiled driver entry point not available");
-    cuuint64_t gdim[4] = {c, w, h, nb};
-    cuuint64_t gstr[3] = {c * sizeof(float), w * c * sizeof(float), h * w * c * sizeof(float)};
-    cuuint32_t box[4] = {box_c, box_w, box_h, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), gdim, gstr, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    BANET_REQUIRE(r == CUDA_SUCCESS, BANET_ERR_CUDA, "cuTensorMapEncodeTiled(nhwc) failed (%d)", (int)r);
-    return BANET_OK;
-}
-
 }  // namespace banet

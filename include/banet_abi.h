@@ -44,10 +44,7 @@ int         banet_num_sms(void);
 /* Diagnostic / test knobs (process-wide; defaults = production).  Results never depend on them beyond
  * fp32 summation order. */
 typedef struct banet_tuning {
-    int tc_generation;      /* 0: default (generation 6 everywhere; lm_build_tc_host.cu has the measurement); 6 / 7: force one wherever it applies (7: F2-only layout + dense grid, TF32X1 / X2) */
-    int tc7_force_direct;   /* 1: generation 7 takes its per-tile global-tap fallback for every tile (tests the fallback) */
-    int tc7_band_rows;      /* generation 7 walks the 8x8 tiles of a pair in bands of this many tile rows (L2 reuse of the window halos); default 4 */
-    int tc6_band_rows;      /* generation 6, dense grid: same walk (tap rows shared by vertically adjacent tiles are re-read from L2, not HBM); 0 = default, 1 = row-major */
+    int tc6_band_rows;      /* generation 6, dense grid: walk the 8x8 tiles of a pair in bands of this many tile rows (tap rows shared by vertically adjacent tiles are re-read from L2, not HBM); 0 = default, 1 = row-major */
     int tc6_l2_hints;       /* generation 6: 0 = default; 1 = no L2 policy; 2 = read-once streams (basis TMA, conv1) evict-first; 3 = 2 + taps evict-last */
     int tc6_tap_prefetch;   /* generation 6: 0 = default; 1 = off; 2 = geometry warps prefetch the tap footprint into L2 ahead of the gather; 3 = 2 with the lower tap row from every pixel */
 } banet_tuning_t;
@@ -137,23 +134,23 @@ typedef struct banet_level {
                                  are the row-major raster grid x<grid_w, y<grid_h (N == grid_w*grid_h) and the kernels walk it in
                                  8x8 tiles so that every conv2 texel is fetched from HBM about once */
     int feature_dtype;        /* BANET_DTYPE_F32 (0) or BANET_DTYPE_BF16 (1), for conv1 and conv2 together; any other value is
-                                 BANET_ERR_BAD_ARG.  bf16 levels run the fp32 SIMT build and tensor-core generation 6 (never generation 7),
-                                 are rejected by banet_lm_track_legacy (BANET_ERR_UNSUPPORTED), and their banet_lm_build_bwd writes
-                                 dconv1 / dconv2 as fp32 buffers */
+                                 BANET_ERR_BAD_ARG.  bf16 levels run the fp32 SIMT build and the tensor-core build, are rejected by
+                                 banet_lm_track_legacy (BANET_ERR_UNSUPPORTED), and their banet_lm_build_bwd writes dconv1 / dconv2 as
+                                 fp32 buffers */
     int basis_dtype;          /* BANET_DTYPE_F32 (0) or BANET_DTYPE_BF16 (1) for B, independent of feature_dtype; any other value is
                                  BANET_ERR_BAD_ARG in every entry that takes levels (also where B is not read: K = 0, the legacy tracker).
-                                 bf16 bases run the fp32 SIMT build and tensor-core generation 6 (never generation 7), and their
-                                 banet_lm_build_bwd writes dB as an fp32 buffer */
+                                 bf16 bases run the fp32 SIMT build and the tensor-core build, and their banet_lm_build_bwd writes dB as
+                                 an fp32 buffer */
     const float* weight;      /* [nb,N,1] or NULL: per-point confidence w_n of the normal equations, H = sum_n w_n J_n^T M_n J_n and
                                  g = sum_n w_n J_n^T q_n (every block: H_cc, H_cd, H_dd, g_c, g_d); rbar_sum and nvalid stay unweighted,
                                  so lambda does not see it.  Used as given: a negative weight can make H indefinite (solve status 1), a
                                  non-finite one gives status 2.  NULL is the unweighted arithmetic bit for bit, and so are weights of
-                                 ones.  Weighted levels never run generation 7 and are rejected by banet_lm_track_legacy
-                                 (BANET_ERR_UNSUPPORTED); the whole-solve entries honour them per pair */
+                                 ones.  Weighted levels are rejected by banet_lm_track_legacy (BANET_ERR_UNSUPPORTED); the whole-solve
+                                 entries honour them per pair */
     int robust;               /* BANET_ROBUST_NONE (0), BANET_ROBUST_HUBER (1) or BANET_ROBUST_CAUCHY (2); any other value is
-                                 BANET_ERR_BAD_ARG in every entry that takes levels.  Robust levels never run generation 7, are rejected by
-                                 banet_lm_track_legacy (BANET_ERR_UNSUPPORTED: its accept / reject test re-evaluates the plain residual),
-                                 and the whole-solve entries honour them per pair.  The backward differentiates the weight too:
+                                 BANET_ERR_BAD_ARG in every entry that takes levels.  Robust levels are rejected by banet_lm_track_legacy
+                                 (BANET_ERR_UNSUPPORTED: its accept / reject test re-evaluates the plain residual), and the whole-solve
+                                 entries honour them per pair.  The backward differentiates the weight too:
                                  dweight_n = dw rho'(s_n), and each channel's residual adjoint gains 2 dw c_n rho''(s_n) d_c (dw: the
                                  gradient w.r.t. w_n).  BANET_ROBUST_NONE is the plain arithmetic bit for bit */
     float robust_scale;       /* delta of the robust loss, finite and > 0 when robust != 0 (else BANET_ERR_BAD_ARG); ignored when robust == 0 */

@@ -1,5 +1,5 @@
 """Writes tests/golden/build_mma.json: SHA-256 digests of the tensor-core lm_build outputs (H, g, rbar, nvalid) on a seeded scene, in
-every precision mode, both conv2 layouts, K = 128 / 64 / 32 and both kernel generations (GPU).  tests/test_gpu_build_mma.py holds
+every precision mode, both conv2 layouts and K = 128 / 64 / 32 (GPU).  tests/test_gpu_build_mma.py holds
 the library to them bit for bit.  Run on an H100 with the library whose results are to be frozen:
 
     python tests/golden/gen_build_mma.py [OUT.json]          (BANET_LIB_PATH selects another build of the library)
@@ -19,37 +19,32 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-# (generation, K, layout, precision mode); generation 7 takes the F2-only layout in modes 1 and 2, K = 64 / 32 modes 2 and 3
-CASES = ([(6, 128, lay, m) for lay in ("3c", "f2") for m in (1, 2, 3)] + [(6, k, "3c", m) for k in (64, 32) for m in (2, 3)]
-         + [(7, 128, "f2", m) for m in (1, 2)])
+# (K, layout, precision mode); K = 64 / 32 take modes 2 and 3
+CASES = [(128, lay, m) for lay in ("3c", "f2") for m in (1, 2, 3)] + [(k, "3c", m) for k in (64, 32) for m in (2, 3)]
 
 
-def case_id(gen, K, lay, mode):
-    return f"gen{gen}_K{K}_{lay}_x{mode}"
+def case_id(K, lay, mode):
+    return f"gen6_K{K}_{lay}_x{mode}"       # gen6: the tensor-core kernel, lm_build_tc6_kernel
 
 
 def outputs():
     """{case id: {tensor name: sha256 hex}} of the library that banet_b200 loads, plus the device identity."""
-    from banet_b200 import ops, synth, _lib
+    from banet_b200 import ops, synth
     dev = torch.device("cuda")
     res = {}
     scenes = {}
-    try:
-        for gen, K, lay, mode in CASES:
-            if K not in scenes:      # 320x240, 2 pairs: 1 200 tiles per pair, spans of several pairs per CTA and pair changes inside a CTA
-                scenes[K] = synth.make_scene(nb=2, H=240, W=320, C=128, K=K, level_ids=(3,), seed=4100 + K, device=dev, dtype=torch.float32)
-            sc = scenes[K]
-            lv = sc.levels[0]
-            conv2 = lv.conv2 if lay == "3c" else lv.conv2[..., :128].contiguous()
-            L = ops.Level(lv.conv1, conv2, lv.intr, lv.p, lv.D, lv.B, grid=lv.grid)
-            W = sc.W0 + 0.01 * torch.randn(sc.W0.shape, generator=torch.Generator().manual_seed(3)).to(dev)
-            _lib.set_tuning(tc_generation=gen)
-            out = ops.lm_build(L, sc.R0, sc.T0, W, precision=mode)
-            torch.cuda.synchronize()
-            res[case_id(gen, K, lay, mode)] = {k: hashlib.sha256(v.contiguous().cpu().numpy().tobytes()).hexdigest()
-                                               for k, v in zip(("H", "g", "rbar", "nvalid"), out)}
-    finally:
-        _lib.set_tuning()
+    for K, lay, mode in CASES:
+        if K not in scenes:      # 320x240, 2 pairs: 1 200 tiles per pair, spans of several pairs per CTA and pair changes inside a CTA
+            scenes[K] = synth.make_scene(nb=2, H=240, W=320, C=128, K=K, level_ids=(3,), seed=4100 + K, device=dev, dtype=torch.float32)
+        sc = scenes[K]
+        lv = sc.levels[0]
+        conv2 = lv.conv2 if lay == "3c" else lv.conv2[..., :128].contiguous()
+        L = ops.Level(lv.conv1, conv2, lv.intr, lv.p, lv.D, lv.B, grid=lv.grid)
+        W = sc.W0 + 0.01 * torch.randn(sc.W0.shape, generator=torch.Generator().manual_seed(3)).to(dev)
+        out = ops.lm_build(L, sc.R0, sc.T0, W, precision=mode)
+        torch.cuda.synchronize()
+        res[case_id(K, lay, mode)] = {k: hashlib.sha256(v.contiguous().cpu().numpy().tobytes()).hexdigest()
+                                      for k, v in zip(("H", "g", "rbar", "nvalid"), out)}
     p = torch.cuda.get_device_properties(0)
     return {"device": p.name, "sm_count": p.multi_processor_count, "cases": res}
 

@@ -243,28 +243,6 @@ def test_tensor_core_build_is_bitwise_the_widened_build(mode, K, C, layout, poin
 
 
 @gpu
-def test_generation_7_is_never_used_for_a_bf16_basis():
-    _lib.require_device()
-    lib = _lib.load()
-    old = _lib.BanetTuning()
-    lib.banet_get_tuning(ctypes.byref(old))
-    t = _lib.BanetTuning(); ctypes.memmove(ctypes.byref(t), ctypes.byref(old), ctypes.sizeof(t)); t.tc_generation = 7
-    try:
-        _lib.check(lib.banet_set_tuning(ctypes.byref(t)), "banet_set_tuning")
-        for mode in ("X1", "X2"):
-            lb, lf, R, T, W = _build_case(128, 128, "dense", "F2", torch.float32, seed=23)
-            from banet_b200 import ops
-            ob = ops.lm_build(lb, R, T, W, MODES[mode])
-            _lib.check(lib.banet_set_tuning(ctypes.byref(old)), "banet_set_tuning")
-            of = ops.lm_build(lf, R, T, W, MODES[mode])                  # generation 6 on the widened basis
-            _lib.check(lib.banet_set_tuning(ctypes.byref(t)), "banet_set_tuning")
-            for a, b in zip(ob, of):
-                assert torch.equal(a, b)
-    finally:
-        lib.banet_set_tuning(ctypes.byref(old))
-
-
-@gpu
 @pytest.mark.parametrize("layout", ["3C", "F2"])
 @pytest.mark.parametrize("C,K", [(64, 128), (128, 64), (8, 16)])
 def test_build_backward_matches_the_widened_backward(C, K, layout):

@@ -478,18 +478,13 @@ def _edge_focal(h, w):
 EDGE_MAPS = {"2x2": (2, 2), "2x3": (2, 3), "3x2": (3, 2), "16x20": (16, 20), "wide": (2, 65600), "tall": (65600, 2)}
 
 
-def _restore_tuning():
-    from banet_b200 import _lib
-    _lib.set_tuning()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("feat", ["f32", "bf16"])
 @pytest.mark.parametrize("layout", ["3c", "f2"])
 @pytest.mark.parametrize("shape", list(EDGE_MAPS))
 def test_image_edges_forward_every_path(shape, layout, feat):
-    """Every forward path (SIMT, TF32X1/X2/X3, AUTO, with and without the grid hint, and generation 7 where it applies) with projections
-    exactly on the map's first and last rows and columns.  An F2 map 65536 texels or wider stays off the tensor cores' packed 16-bit tap
+    """Every forward path (SIMT, TF32X1/X2/X3, AUTO, with and without the grid hint) with projections exactly on the map's first and
+    last rows and columns.  An F2 map 65536 texels or wider stays off the tensor cores' packed 16-bit tap
     columns: AUTO resolves to SIMT and an explicit TF32 mode is refused with a message that names the width."""
     from banet_b200 import _lib
     h, w = EDGE_MAPS[shape]
@@ -498,14 +493,9 @@ def test_image_edges_forward_every_path(shape, layout, feat):
     ref = _oracle(c, _oracle_inputs(c, fb, False))
     assert float(ref[3].min()) < c.N and float(ref[3].min()) > 0          # some points out, some in
     wide_f2 = layout == "f2" and w >= 65536
-    runs = [(prec, hint, 0) for prec in _modes(128) for hint in (None, grid)]
-    if layout == "f2" and not fb:
-        runs += [(X1, grid, 7), (X2, grid, 7)]
-    try:
-        for prec, hint, gen in runs:
-            if gen:
-                _lib.set_tuning(tc_generation=7)
-            lab = f"edges {shape} {layout} feat={feat} {MODE_NAME[prec]} hint={int(hint is not None)} gen={gen or 6}"
+    for prec in _modes(128):
+        for hint in (None, grid):
+            lab = f"edges {shape} {layout} feat={feat} {MODE_NAME[prec]} hint={int(hint is not None)}"
             tol = TOL[SIMT] if wide_f2 and prec == AUTO else TOL[_auto(128, c.N) if prec == AUTO else prec]
             try:
                 out = _build(c, prec, fb, grid=hint)
@@ -514,10 +504,6 @@ def test_image_edges_forward_every_path(shape, layout, feat):
                 print(f"EDGE {lab}: refused (F2 width)")
                 continue
             _check_forward(lab, out, ref, tol)
-            if gen:
-                _restore_tuning()
-    finally:
-        _restore_tuning()
 
 
 @pytest.mark.gpu

@@ -1,7 +1,7 @@
-"""The MMA warpgroup of the tensor-core build kernels places its fragments by a compile-time column mapping (csrc/mma_role.cuh) but
+"""The MMA warpgroup of the tensor-core build kernel places its fragments by a compile-time column mapping (csrc/mma_role.cuh) but
 forms every element from the same 8-pixel products, added in the same order: lm_build's outputs are bitwise equal to the frozen
 digests in tests/golden/build_mma.json (written by tests/golden/gen_build_mma.py with the previous, runtime-indexed MMA role), in
-every precision mode, both conv2 layouts, K = 128 / 64 / 32 and both kernel generations."""
+every precision mode, both conv2 layouts and K = 128 / 64 / 32."""
 import json
 import os
 import sys
@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
 
-def test_build_outputs_bitwise_equal_to_golden():
+def test_generation_6_outputs_bitwise_equal_to_golden():
     import gen_build_mma
     with open(os.path.join(HERE, "golden", "build_mma.json")) as f:
         want = json.load(f)

@@ -305,25 +305,6 @@ def test_huber_above_every_residual_gives_the_plain_bits(K):
                             assert torch.equal(u, v), (layout, feat, basis, weight is None, pn, name)
 
 
-@gpu
-def test_robust_levels_run_generation_6_under_tc_generation_7():
-    from banet_b200 import ops
-    _lib.require_device()
-    sc, lv, Wt = _gpu_scene(64, 128, seed=59)
-    try:
-        for kind in ("huber", "cauchy"):
-            L = _level_of(lv, "f2", "f32", "f32", True, None, kind, 3.0)
-            for pn in ("x1", "x2"):
-                _lib.set_tuning()
-                a = ops.lm_build(L, sc.R0, sc.T0, Wt, PRECS[pn])
-                _lib.set_tuning(tc_generation=7)
-                b = ops.lm_build(L, sc.R0, sc.T0, Wt, PRECS[pn])
-                for u, v in zip(a, b):
-                    assert torch.equal(u, v), (kind, pn)
-    finally:
-        _lib.set_tuning()
-
-
 def _poisoned_ws(pattern):
     def make(nbytes, device):
         n = max(int(nbytes), 256)
