@@ -1,7 +1,9 @@
-// extern "C" entry points of libbanet.so (see include/banet_abi.h) + the LM driver loop.
+// extern "C" entry points of libbanet.so (see include/banet_abi.h) + run_solve, the coarse-to-fine schedule of the four whole-solve entries.
 #include "common.cuh"
 #include "lm_build.h"
 #include <string.h>
+#include <algorithm>
+#include <type_traits>
 
 namespace banet {
 
@@ -290,43 +292,169 @@ extern "C" int banet_lm_solve_update_bwd(const float* H, const float* g, const f
 }
 
 // -------------------------------------------------------------------------------------------------
-// whole solve
+// Whole solves.  banet_lm_run (pairs), banet_lm_window_run (one dense keyframe window), banet_lm_window_batch_run (batches of windows on
+// the block-arrow step) and banet_lm_keyframe_run (the keyframe layout) run one coarse-to-fine schedule, run_solve.  Each entry point
+// checks its own arguments first and gives run_solve the sizes of its workspace, its size rule per level, what runs once before the
+// first level and one iteration's build and step.
 namespace {
-struct RunCarve { size_t build, H, g, rbar, nvalid, lambda, delta, total; };
-int carve(const banet_level_t* levels, int nlevels, int precision, RunCarve* c)
+int check_keyframe_level(const banet_keyframe_level_t* lv, const char* who)
 {
-    size_t build = 0; int maxC = 0;
-    const int nb = levels[0].nb, K = levels[0].K, P = 6 + K;
+    BANET_REQUIRE(lv, BANET_ERR_BAD_ARG, "%s: null level", who);
+    BANET_REQUIRE(lv->nw > 0 && lv->nf > 0 && lv->N > 0 && lv->C > 0 && lv->K > 0 && lv->h >= 2 && lv->w >= 2, BANET_ERR_BAD_ARG,
+                  "%s: bad shape nw=%d nf=%d N=%d C=%d K=%d h=%d w=%d", who, lv->nw, lv->nf, lv->N, lv->C, lv->K, lv->h, lv->w);
+    BANET_REQUIRE(lv->conv2_channels == 3 * lv->C || lv->conv2_channels == lv->C, BANET_ERR_BAD_ARG,
+                  "%s: conv2_channels=%d must be 3*C (reference layout) or C (F2 only)", who, lv->conv2_channels);
+    BANET_REQUIRE(lv->conv1 && lv->p && lv->D && lv->B && lv->conv2 && lv->intr, BANET_ERR_BAD_ARG, "%s: null tensor", who);
+    BANET_REQUIRE((long long)lv->h * lv->w * lv->conv2_channels < (1LL << 40), BANET_ERR_BAD_ARG, "%s: map too large", who);
+    BANET_REQUIRE(lv->K <= 256, BANET_ERR_UNSUPPORTED, "%s: K=%d > 256 not supported", who, lv->K);
+    BANET_REQUIRE(lv->C <= 2048, BANET_ERR_UNSUPPORTED, "%s: C=%d > 2048 not supported", who, lv->C);
+    return BANET_OK;
+}
+
+// The keyframe build is fp32 SIMT only: AUTO resolves to it (as AUTO does wherever the tensor cores do not apply); the TF32 modes have no
+// keyframe kernel.
+int check_keyframe_precision(int precision, const char* who)
+{
+    BANET_REQUIRE(precision == BANET_PREC_AUTO || precision == BANET_PREC_FP32_SIMT || precision == BANET_PREC_TF32X1 || precision == BANET_PREC_TF32X2 ||
+                  precision == BANET_PREC_TF32X3 || precision == BANET_PREC_TF32_LEVELWISE, BANET_ERR_BAD_ARG, "%s: unknown precision mode %d", who, precision);
+    BANET_REQUIRE(precision == BANET_PREC_AUTO || precision == BANET_PREC_FP32_SIMT, BANET_ERR_UNSUPPORTED,
+                  "%s: precision mode %d (tensor cores) has no keyframe build; use AUTO or FP32_SIMT", who, precision);
+    return BANET_OK;
+}
+
+// a level of a whole solve: valid, and of level 0's batch shape
+int check_run_level(const banet_level_t* levels, int l, const char* who)
+{
+    if (int rc = check_level(&levels[l], who)) return rc;
+    BANET_REQUIRE(levels[l].nb == levels[0].nb && levels[l].K == levels[0].K, BANET_ERR_BAD_ARG, "%s: nb/K must agree across levels", who);
+    return BANET_OK;
+}
+int check_run_level(const banet_keyframe_level_t* levels, int l, const char* who)
+{
+    if (int rc = check_keyframe_level(&levels[l], who)) return rc;
+    BANET_REQUIRE(levels[l].nw == levels[0].nw && levels[l].nf == levels[0].nf && levels[l].K == levels[0].K, BANET_ERR_BAD_ARG,
+                  "%s: nw/nf/K must agree across levels", who);
+    return BANET_OK;
+}
+
+// A level's build plan.  `who` names the caller in the robust-loss and precision checks, which a workspace query reaches unchecked.
+struct PairPlan : BuildPlan { int res; };                          // + the precision the level resolves to
+int plan_level(const banet_level_t* lv, int precision, const char* who, PairPlan* plan)
+{
+    if (int rc = check_robust(lv, who)) return rc;
+    plan->res = resolve_precision(lv, precision);
+    return plan->res < 0 ? plan->res : plan_for(lv, plan->res, plan);
+}
+int plan_level(const banet_keyframe_level_t* lv, int precision, const char* who, KeyframePlan* plan)
+{
+    if (int rc = check_keyframe_precision(precision, who)) return rc;
+    return keyframe_plan(lv, num_sms(), plan);
+}
+template <class Level> using PlanOf = std::conditional_t<std::is_same<Level, banet_level_t>::value, PairPlan, KeyframePlan>;
+
+// The workspace of a whole solve: build | H | g | rbar | nvalid | lambda | delta | tail, every part but the tail 256-B aligned, for nb
+// pairs of P unknowns, rbar of the widest level (maxC), and the form's lambda and delta floats and tail bytes.
+struct RunSizes { size_t nb; int P, maxC; size_t lambda, delta, tail; };
+struct RunCarve { size_t build, H, g, rbar, nvalid, lambda, delta, tail, total; };
+struct RunWork { float *H, *g, *rbar, *nvalid, *lambda, *delta; char *build, *tail; };
+
+template <class Level> int max_C(const Level* levels, int nlevels)
+{
+    int C = 0;
+    for (int l = 0; l < nlevels; ++l) C = std::max(C, levels[l].C);
+    return C;
+}
+RunSizes pair_sizes(const banet_level_t* levels, int nlevels)
+{
+    const int nb = levels[0].nb, P = 6 + levels[0].K;
+    return {(size_t)nb, P, max_C(levels, nlevels), (size_t)nb, (size_t)nb * P, 0};
+}
+RunSizes window_sizes(const banet_level_t* levels, int nlevels)     // + the dense window step's matrix and factors
+{
+    RunSizes s = pair_sizes(levels, nlevels);
+    s.tail = align_up(lm_window_step_workspace_floats(levels[0].nb, levels[0].K, s.maxC) * sizeof(float), 256);
+    return s;
+}
+RunSizes batch_sizes(const banet_level_t* levels, int nlevels, int nw)  // + per-pair copies of W for the build + the step's per-frame factors
+{
+    RunSizes s = pair_sizes(levels, nlevels);
+    s.tail = align_up(s.nb * levels[0].K * sizeof(float), 256) + lm_window_batch_ws_bytes(nw, levels[0].nb / nw);
+    return s;
+}
+RunSizes keyframe_sizes(const banet_keyframe_level_t* levels, int nlevels)   // one lambda and delta [6 nf + K] per window
+{
+    const int nw = levels[0].nw, nf = levels[0].nf, K = levels[0].K;
+    return {(size_t)nw * nf, 6 + K, max_C(levels, nlevels), (size_t)nw, (size_t)nw * (6 * nf + K), lm_window_batch_ws_bytes(nw, nf)};
+}
+
+template <class Level>
+int run_carve(const Level* levels, int nlevels, int precision, const char* who, const RunSizes& s, RunCarve* c)
+{
+    size_t build = 0;
     for (int l = 0; l < nlevels; ++l) {
-        BuildPlan plan;
-        if (int rc = check_robust(&levels[l], "lm_run_workspace_bytes")) return rc;
-        const int res = resolve_precision(&levels[l], precision);
-        if (res < 0) return res;
-        int rc = plan_for(&levels[l], res, &plan);
-        if (rc) return rc;
-        if (plan.ws_bytes > build) build = plan.ws_bytes;
-        if (levels[l].C > maxC) maxC = levels[l].C;
+        PlanOf<Level> plan;
+        if (int rc = plan_level(&levels[l], precision, who, &plan)) return rc;
+        build = std::max(build, plan.ws_bytes);
     }
     size_t off = 0;
     c->build = off;  off += align_up(build, 256);
-    c->H = off;      off += align_up((size_t)nb * P * P * 4, 256);
-    c->g = off;      off += align_up((size_t)nb * P * 4, 256);
-    c->rbar = off;   off += align_up((size_t)nb * maxC * 4, 256);
-    c->nvalid = off; off += align_up((size_t)nb * 4, 256);
-    c->lambda = off; off += align_up((size_t)nb * 4, 256);
-    c->delta = off;  off += align_up((size_t)nb * P * 4, 256);
-    c->total = off;
+    c->H = off;      off += align_up(s.nb * s.P * s.P * 4, 256);
+    c->g = off;      off += align_up(s.nb * s.P * 4, 256);
+    c->rbar = off;   off += align_up(s.nb * s.maxC * 4, 256);
+    c->nvalid = off; off += align_up(s.nb * 4, 256);
+    c->lambda = off; off += align_up(s.lambda * 4, 256);
+    c->delta = off;  off += align_up(s.delta * 4, 256);
+    c->tail = off;
+    c->total = off + s.tail;
     return BANET_OK;
 }
+
 __global__ void fill_kernel(float* p, int n, float v) { int i = blockIdx.x * blockDim.x + threadIdx.x; if (i < n) p[i] = v; }
 __global__ void zero_status_kernel(int32_t* p, int n) { int i = blockIdx.x * blockDim.x + threadIdx.x; if (i < n) p[i] = 0; }
+
+// The schedule of every whole solve.  Per level: its checks, the rule "lambda-MLP weights or lambda_fixed >= 0" and the form's size rule
+// fits(level, use_mlp).  Then the carve, status zeroed and start(work) once.  Then per level its build plan, lambda_fixed in the first
+// nlambda slots when the level has no MLP, and iters_per_level x iterate(level, plan, mlp, work): one build and one step, mlp null when
+// lambda is fixed.
+template <class Level, class Fits, class Start, class Iterate>
+int run_solve(const char* who, const Level* levels, int nlevels, int iters_per_level, const float* const* mlp_weights, float lambda_fixed,
+              int precision, const float* W, int32_t* status, void* ws, size_t ws_bytes, cudaStream_t st, const RunSizes& s, int nlambda,
+              Fits fits, Start start, Iterate iterate)
+{
+    for (int l = 0; l < nlevels; ++l) {
+        if (int rc = check_run_level(levels, l, who)) return rc;
+        BANET_REQUIRE((mlp_weights && mlp_weights[l]) || lambda_fixed >= 0.f, BANET_ERR_BAD_ARG,
+                      "%s: level %d has no lambda-MLP weights and lambda_fixed < 0", who, l);
+        if (int rc = fits(levels[l], mlp_weights && mlp_weights[l] && lambda_fixed < 0.f)) return rc;
+    }
+    // a pose-only solve (K = 0) takes no W; the window forms require W with their other pointers
+    BANET_REQUIRE(levels[0].K == 0 || W, BANET_ERR_BAD_ARG, "%s: K=%d but W is null", who, levels[0].K);
+    RunCarve c;
+    if (int rc = run_carve(levels, nlevels, precision, who, s, &c)) return rc;
+    BANET_REQUIRE(ws && ws_bytes >= c.total, BANET_ERR_WORKSPACE, "%s: workspace %zu < %zu bytes", who, ws_bytes, c.total);
+    char* base = reinterpret_cast<char*>(ws);
+    const auto at = [base](size_t off) { return reinterpret_cast<float*>(base + off); };
+    const RunWork w = {at(c.H), at(c.g), at(c.rbar), at(c.nvalid), at(c.lambda), at(c.delta), base + c.build, base + c.tail};
+    const int nb = (int)s.nb;
+    zero_status_kernel<<<(nb + 255) / 256, 256, 0, st>>>(status, nb);
+    if (int rc = start(w)) return rc;
+    for (int l = 0; l < nlevels; ++l) {
+        PlanOf<Level> plan;
+        if (int rc = plan_level(&levels[l], precision, who, &plan)) return rc;
+        const float* mlp = mlp_weights && lambda_fixed < 0.f ? mlp_weights[l] : nullptr;
+        if (!mlp) fill_kernel<<<(nlambda + 255) / 256, 256, 0, st>>>(w.lambda, nlambda, lambda_fixed);
+        for (int it = 0; it < iters_per_level; ++it)
+            if (int rc = iterate(levels[l], plan, mlp, w)) return rc;
+    }
+    BANET_CUDA_LAUNCH_CHECK(who);
+    return BANET_OK;
+}
 }  // namespace
 
 extern "C" size_t banet_lm_run_workspace_bytes(const banet_level_t* levels, int nlevels, int precision)
 {
-    if (!levels || nlevels <= 0) return 0;
     RunCarve c;
-    if (carve(levels, nlevels, precision, &c) != BANET_OK) return 0;
+    if (!levels || nlevels <= 0 || run_carve(levels, nlevels, precision, "lm_run_workspace_bytes", pair_sizes(levels, nlevels), &c)) return 0;
     return c.total;
 }
 
@@ -337,63 +465,32 @@ extern "C" int banet_lm_run(const banet_level_t* levels, int nlevels, int iters_
 {
     BANET_REQUIRE(levels && nlevels > 0 && iters_per_level > 0 && opts && R && T && status, BANET_ERR_BAD_ARG, "lm_run: bad argument");
     const int nb = levels[0].nb, K = levels[0].K;
-    for (int l = 0; l < nlevels; ++l) {
-        int rc = check_level(&levels[l], "lm_run");
-        if (rc) return rc;
-        BANET_REQUIRE(levels[l].nb == nb && levels[l].K == K, BANET_ERR_BAD_ARG, "lm_run: nb/K must agree across levels");
-        BANET_REQUIRE((mlp_weights && mlp_weights[l]) || lambda_fixed >= 0.f, BANET_ERR_BAD_ARG,
-                      "lm_run: level %d has no lambda-MLP weights and lambda_fixed < 0", l);
-        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
-        BANET_REQUIRE(lm_step_supported(6 + K, use_mlp ? levels[l].C : 0), BANET_ERR_UNSUPPORTED, "lm_run: K=%d, C=%d do not fit the step kernel",
-                      K, levels[l].C);
-    }
-    BANET_REQUIRE(K == 0 || W, BANET_ERR_BAD_ARG, "lm_run: K=%d but W is null", K);
-    RunCarve c;
-    int rc = carve(levels, nlevels, precision, &c);
-    if (rc) return rc;
-    BANET_REQUIRE(ws && ws_bytes >= c.total, BANET_ERR_WORKSPACE, "lm_run: workspace %zu < %zu bytes", ws_bytes, c.total);
+    const bool scramble = opts->vmatrix_batch_scramble != 0;
     cudaStream_t st = (cudaStream_t)stream;
-    char* base = reinterpret_cast<char*>(ws);
-    float* H = reinterpret_cast<float*>(base + c.H);
-    float* g = reinterpret_cast<float*>(base + c.g);
-    float* rbar = reinterpret_cast<float*>(base + c.rbar);
-    float* nvalid = reinterpret_cast<float*>(base + c.nvalid);
-    float* lam = reinterpret_cast<float*>(base + c.lambda);
-    float* delta = reinterpret_cast<float*>(base + c.delta);
-    zero_status_kernel<<<(nb + 255) / 256, 256, 0, st>>>(status, nb);
-    for (int l = 0; l < nlevels; ++l) {
-        const banet_level_t* lv = &levels[l];
-        BuildPlan plan;
-        const int res = resolve_precision(lv, precision);
-        if (res < 0) return res;
-        rc = plan_for(lv, res, &plan);
-        if (rc) return rc;
-        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
-        if (!use_mlp) fill_kernel<<<(nb + 255) / 256, 256, 0, st>>>(lam, nb, lambda_fixed);
-        for (int it = 0; it < iters_per_level; ++it) {
-            rc = build_dispatch(lv, res, plan, R, T, W, H, g, rbar, nvalid, base + c.build, st);
-            if (rc) return rc;
+    return run_solve("lm_run", levels, nlevels, iters_per_level, mlp_weights, lambda_fixed, precision, W, status, ws, ws_bytes, st,
+                     pair_sizes(levels, nlevels), nb,
+        [&](const banet_level_t& lv, bool use_mlp) {
+            BANET_REQUIRE(lm_step_supported(6 + K, use_mlp ? lv.C : 0), BANET_ERR_UNSUPPORTED, "lm_run: K=%d, C=%d do not fit the step kernel", K, lv.C);
+            return BANET_OK;
+        },
+        [](const RunWork&) { return BANET_OK; },
+        [&](const banet_level_t& lv, const PairPlan& plan, const float* mlp, const RunWork& w) {
+            int rc = build_dispatch(&lv, plan.res, plan, R, T, W, w.H, w.g, w.rbar, w.nvalid, w.build, st);
             // one launch: lambda-MLP + damping + Cholesky + update; the batch-interleaved VMatrix updates R, T after every pair's step
-            const bool scramble = opts->vmatrix_batch_scramble != 0;
-            rc = lm_step(H, g, rbar, nb, lv->N, lv->C, K, use_mlp ? mlp_weights[l] : nullptr, l2_regularizer_base, use_mlp ? nullptr : lam,
-                         kStepBundleNet, nullptr, *opts, R, T, W, scramble ? nullptr : R, T, W, delta, lam, status, 1, st);
-            if (!rc && scramble) rc = launch_pose_update(delta, nb, 6 + K, 1, R, T, R, T, st);
-            if (rc) return rc;
-        }
-    }
-    BANET_CUDA_LAUNCH_CHECK("lm_run");
-    return BANET_OK;
+            if (!rc) rc = lm_step(w.H, w.g, w.rbar, nb, lv.N, lv.C, K, mlp, l2_regularizer_base, mlp ? nullptr : w.lambda, kStepBundleNet, nullptr,
+                                  *opts, R, T, W, scramble ? nullptr : R, T, W, w.delta, w.lambda, status, 1, st);
+            if (!rc && scramble) rc = launch_pose_update(w.delta, nb, 6 + K, 1, R, T, R, T, st);
+            return rc;
+        });
 }
 
 // ---- joint keyframe window (SURVEY.md section 8f-4; an extension, the reference is 2-view): nb = nf frame pairs sharing one W -------------
 extern "C" size_t banet_lm_window_run_workspace_bytes(const banet_level_t* levels, int nlevels, int precision)
 {
-    if (!levels || nlevels <= 0 || levels[0].K <= 0) return 0;
     RunCarve c;
-    if (carve(levels, nlevels, precision, &c) != BANET_OK) return 0;
-    int maxC = 0;
-    for (int l = 0; l < nlevels; ++l) if (levels[l].C > maxC) maxC = levels[l].C;
-    return c.total + align_up(lm_window_step_workspace_floats(levels[0].nb, levels[0].K, maxC) * sizeof(float), 256);
+    if (!levels || nlevels <= 0 || levels[0].K <= 0 ||
+        run_carve(levels, nlevels, precision, "lm_window_run_workspace_bytes", window_sizes(levels, nlevels), &c)) return 0;
+    return c.total;
 }
 
 extern "C" int banet_lm_window_run(const banet_level_t* levels, int nlevels, int iters_per_level,
@@ -404,51 +501,19 @@ extern "C" int banet_lm_window_run(const banet_level_t* levels, int nlevels, int
     BANET_REQUIRE(levels && nlevels > 0 && iters_per_level > 0 && opts && R && T && W && status, BANET_ERR_BAD_ARG, "lm_window_run: bad argument");
     const int nf = levels[0].nb, K = levels[0].K;
     BANET_REQUIRE(K > 0 && !opts->vmatrix_batch_scramble, BANET_ERR_BAD_ARG, "lm_window_run: needs a depth basis (K > 0) and vmatrix_batch_scramble = 0");
-    int maxC = 0;
-    for (int l = 0; l < nlevels; ++l) {
-        int rc = check_level(&levels[l], "lm_window_run");
-        if (rc) return rc;
-        BANET_REQUIRE(levels[l].nb == nf && levels[l].K == K, BANET_ERR_BAD_ARG, "lm_window_run: nb/K must agree across levels");
-        BANET_REQUIRE((mlp_weights && mlp_weights[l]) || lambda_fixed >= 0.f, BANET_ERR_BAD_ARG,
-                      "lm_window_run: level %d has no lambda-MLP weights and lambda_fixed < 0", l);
-        BANET_REQUIRE(lm_window_supported(nf, K, levels[l].C), BANET_ERR_UNSUPPORTED, "lm_window_run: 6*%d+%d unknowns do not fit the solve kernel", nf, K);
-        if (levels[l].C > maxC) maxC = levels[l].C;
-    }
-    RunCarve c;
-    int rc = carve(levels, nlevels, precision, &c);
-    if (rc) return rc;
-    const size_t need = c.total + align_up(lm_window_step_workspace_floats(nf, K, maxC) * sizeof(float), 256);
-    BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_window_run: workspace %zu < %zu bytes", ws_bytes, need);
     cudaStream_t st = (cudaStream_t)stream;
-    char* base = reinterpret_cast<char*>(ws);
-    float* H = reinterpret_cast<float*>(base + c.H);
-    float* g = reinterpret_cast<float*>(base + c.g);
-    float* rbar = reinterpret_cast<float*>(base + c.rbar);
-    float* nvalid = reinterpret_cast<float*>(base + c.nvalid);
-    float* lam = reinterpret_cast<float*>(base + c.lambda);
-    float* wsw = reinterpret_cast<float*>(base + c.total);
-    zero_status_kernel<<<(nf + 255) / 256, 256, 0, st>>>(status, nf);
-    rc = lm_window_broadcast_w(W, nf, K, st);                      // frame 0's W is the window's W
-    if (rc) return rc;
-    for (int l = 0; l < nlevels; ++l) {
-        const banet_level_t* lv = &levels[l];
-        BuildPlan plan;
-        const int res = resolve_precision(lv, precision);
-        if (res < 0) return res;
-        rc = plan_for(lv, res, &plan);
-        if (rc) return rc;
-        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
-        if (!use_mlp) fill_kernel<<<1, 32, 0, st>>>(lam, 1, lambda_fixed);
-        for (int it = 0; it < iters_per_level; ++it) {
-            rc = build_dispatch(lv, res, plan, R, T, W, H, g, rbar, nvalid, base + c.build, st);
-            if (rc) return rc;
-            rc = lm_window_step(H, g, rbar, nf, lv->N, lv->C, K, use_mlp ? mlp_weights[l] : nullptr, l2_regularizer_base, use_mlp ? nullptr : lam,
-                                *opts, R, T, W, nf, R, T, W, nullptr, wsw, nullptr, status, 1, st);
-            if (rc) return rc;
-        }
-    }
-    BANET_CUDA_LAUNCH_CHECK("lm_window_run");
-    return BANET_OK;
+    return run_solve("lm_window_run", levels, nlevels, iters_per_level, mlp_weights, lambda_fixed, precision, W, status, ws, ws_bytes, st,
+                     window_sizes(levels, nlevels), 1,
+        [&](const banet_level_t& lv, bool) {
+            BANET_REQUIRE(lm_window_supported(nf, K, lv.C), BANET_ERR_UNSUPPORTED, "lm_window_run: 6*%d+%d unknowns do not fit the solve kernel", nf, K);
+            return BANET_OK;
+        },
+        [&](const RunWork&) { return lm_window_broadcast_w(W, nf, K, st); },        // frame 0's W is the window's W
+        [&](const banet_level_t& lv, const PairPlan& plan, const float* mlp, const RunWork& w) {
+            const int rc = build_dispatch(&lv, plan.res, plan, R, T, W, w.H, w.g, w.rbar, w.nvalid, w.build, st);
+            return rc ? rc : lm_window_step(w.H, w.g, w.rbar, nf, lv.N, lv.C, K, mlp, l2_regularizer_base, mlp ? nullptr : w.lambda, *opts,
+                                            R, T, W, nf, R, T, W, nullptr, reinterpret_cast<float*>(w.tail), nullptr, status, 1, st);
+        });
 }
 
 extern "C" size_t banet_lm_window_solve_update_workspace_bytes(int nf, int K)
@@ -496,19 +561,12 @@ extern "C" int banet_lm_window_solve_update_bwd(const float* H, const float* g, 
 }
 
 // ---- batches of keyframe windows (section 3d): nb = nw nf pairs, pair w nf + f = (keyframe of window w -> frame f) -----------------------
-namespace {
-size_t batch_run_extra(int nw, int nf, int K)                     // per-pair copies of W for the build + the step's per-frame factors
-{
-    return align_up((size_t)nw * nf * K * sizeof(float), 256) + lm_window_batch_ws_bytes(nw, nf);
-}
-}  // namespace
-
 extern "C" size_t banet_lm_window_batch_run_workspace_bytes(const banet_level_t* levels, int nlevels, int nw, int precision)
 {
-    if (!levels || nlevels <= 0 || nw <= 0 || levels[0].K <= 0 || levels[0].nb % nw != 0) return 0;
     RunCarve c;
-    if (carve(levels, nlevels, precision, &c) != BANET_OK) return 0;
-    return c.total + batch_run_extra(nw, levels[0].nb / nw, levels[0].K);
+    if (!levels || nlevels <= 0 || nw <= 0 || levels[0].K <= 0 || levels[0].nb % nw != 0 ||
+        run_carve(levels, nlevels, precision, "lm_window_batch_run_workspace_bytes", batch_sizes(levels, nlevels, nw), &c)) return 0;
+    return c.total;
 }
 
 extern "C" int banet_lm_window_batch_run(const banet_level_t* levels, int nlevels, int nw, int iters_per_level,
@@ -523,53 +581,22 @@ extern "C" int banet_lm_window_batch_run(const banet_level_t* levels, int nlevel
     BANET_REQUIRE(K > 0 && !opts->vmatrix_batch_scramble, BANET_ERR_BAD_ARG, "lm_window_batch_run: needs a depth basis (K > 0) and vmatrix_batch_scramble = 0");
     BANET_REQUIRE(nb > 0 && nb % nw == 0, BANET_ERR_BAD_ARG, "lm_window_batch_run: nb=%d is not nw * nf with nw=%d", nb, nw);
     const int nf = nb / nw;
-    for (int l = 0; l < nlevels; ++l) {
-        int rc = check_level(&levels[l], "lm_window_batch_run");
-        if (rc) return rc;
-        BANET_REQUIRE(levels[l].nb == nb && levels[l].K == K, BANET_ERR_BAD_ARG, "lm_window_batch_run: nb/K must agree across levels");
-        BANET_REQUIRE((mlp_weights && mlp_weights[l]) || lambda_fixed >= 0.f, BANET_ERR_BAD_ARG,
-                      "lm_window_batch_run: level %d has no lambda-MLP weights and lambda_fixed < 0", l);
-        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
-        BANET_REQUIRE(lm_window_batch_supported(K, use_mlp ? levels[l].C : 0), BANET_ERR_UNSUPPORTED,
-                      "lm_window_batch_run: K=%d (C=%d) does not fit the window step (K <= 256)", K, levels[l].C);
-    }
-    RunCarve c;
-    int rc = carve(levels, nlevels, precision, &c);
-    if (rc) return rc;
-    const size_t need = c.total + batch_run_extra(nw, nf, K);
-    BANET_REQUIRE(ws && ws_bytes >= need, BANET_ERR_WORKSPACE, "lm_window_batch_run: workspace %zu < %zu bytes", ws_bytes, need);
     cudaStream_t st = (cudaStream_t)stream;
-    char* base = reinterpret_cast<char*>(ws);
-    float* H = reinterpret_cast<float*>(base + c.H);
-    float* g = reinterpret_cast<float*>(base + c.g);
-    float* rbar = reinterpret_cast<float*>(base + c.rbar);
-    float* nvalid = reinterpret_cast<float*>(base + c.nvalid);
-    float* lam = reinterpret_cast<float*>(base + c.lambda);            // [nw]
-    float* delta = reinterpret_cast<float*>(base + c.delta);          // [nw, 6 nf + K] <= [nb, 6 + K]
-    float* Wp = reinterpret_cast<float*>(base + c.total);             // [nb, K] per-pair copies of the windows' W
-    void* fws = base + c.total + align_up((size_t)nb * K * sizeof(float), 256);
-    zero_status_kernel<<<(nb + 255) / 256, 256, 0, st>>>(status, nb);
-    rc = lm_window_batch_broadcast_w(W, nw, nf, K, Wp, st);
-    if (rc) return rc;
-    for (int l = 0; l < nlevels; ++l) {
-        const banet_level_t* lv = &levels[l];
-        BuildPlan plan;
-        const int res = resolve_precision(lv, precision);
-        if (res < 0) return res;
-        rc = plan_for(lv, res, &plan);
-        if (rc) return rc;
-        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
-        if (!use_mlp) fill_kernel<<<(nw + 255) / 256, 256, 0, st>>>(lam, nw, lambda_fixed);
-        for (int it = 0; it < iters_per_level; ++it) {                // one build launch and one step launch per iteration
-            rc = build_dispatch(lv, res, plan, R, T, Wp, H, g, rbar, nvalid, base + c.build, st);
-            if (rc) return rc;
-            rc = lm_window_batch_step(H, g, rbar, nw, nf, lv->N, lv->C, K, use_mlp ? mlp_weights[l] : nullptr, l2_regularizer_base,
-                                      use_mlp ? nullptr : lam, *opts, R, T, W, R, T, W, Wp, delta, use_mlp ? lam : nullptr, status, 1, fws, st);
-            if (rc) return rc;
-        }
-    }
-    BANET_CUDA_LAUNCH_CHECK("lm_window_batch_run");
-    return BANET_OK;
+    return run_solve("lm_window_batch_run", levels, nlevels, iters_per_level, mlp_weights, lambda_fixed, precision, W, status, ws, ws_bytes, st,
+                     batch_sizes(levels, nlevels, nw), nw,
+        [&](const banet_level_t& lv, bool use_mlp) {
+            BANET_REQUIRE(lm_window_batch_supported(K, use_mlp ? lv.C : 0), BANET_ERR_UNSUPPORTED,
+                          "lm_window_batch_run: K=%d (C=%d) does not fit the window step (K <= 256)", K, lv.C);
+            return BANET_OK;
+        },
+        [&](const RunWork& w) { return lm_window_batch_broadcast_w(W, nw, nf, K, reinterpret_cast<float*>(w.tail), st); },
+        [&](const banet_level_t& lv, const PairPlan& plan, const float* mlp, const RunWork& w) {  // one build launch and one step launch
+            float* Wp = reinterpret_cast<float*>(w.tail);                   // [nb, K] per-pair copies of the windows' W
+            const int rc = build_dispatch(&lv, plan.res, plan, R, T, Wp, w.H, w.g, w.rbar, w.nvalid, w.build, st);
+            return rc ? rc : lm_window_batch_step(w.H, w.g, w.rbar, nw, nf, lv.N, lv.C, K, mlp, l2_regularizer_base, mlp ? nullptr : w.lambda,
+                                                  *opts, R, T, W, R, T, W, Wp, w.delta, mlp ? w.lambda : nullptr, status, 1,
+                                                  w.tail + align_up((size_t)nb * K * sizeof(float), 256), st);
+        });
 }
 
 extern "C" size_t banet_lm_window_batch_solve_update_workspace_bytes(int nw, int nf, int K)
@@ -616,59 +643,6 @@ extern "C" int banet_lm_window_batch_solve_update_bwd(const float* H, const floa
 }
 
 // ---- keyframe-layout window batches (section 3e): the keyframe tensors once per window ------------------------------------------------
-namespace {
-int check_keyframe_level(const banet_keyframe_level_t* lv, const char* who)
-{
-    BANET_REQUIRE(lv, BANET_ERR_BAD_ARG, "%s: null level", who);
-    BANET_REQUIRE(lv->nw > 0 && lv->nf > 0 && lv->N > 0 && lv->C > 0 && lv->K > 0 && lv->h >= 2 && lv->w >= 2, BANET_ERR_BAD_ARG,
-                  "%s: bad shape nw=%d nf=%d N=%d C=%d K=%d h=%d w=%d", who, lv->nw, lv->nf, lv->N, lv->C, lv->K, lv->h, lv->w);
-    BANET_REQUIRE(lv->conv2_channels == 3 * lv->C || lv->conv2_channels == lv->C, BANET_ERR_BAD_ARG,
-                  "%s: conv2_channels=%d must be 3*C (reference layout) or C (F2 only)", who, lv->conv2_channels);
-    BANET_REQUIRE(lv->conv1 && lv->p && lv->D && lv->B && lv->conv2 && lv->intr, BANET_ERR_BAD_ARG, "%s: null tensor", who);
-    BANET_REQUIRE((long long)lv->h * lv->w * lv->conv2_channels < (1LL << 40), BANET_ERR_BAD_ARG, "%s: map too large", who);
-    BANET_REQUIRE(lv->K <= 256, BANET_ERR_UNSUPPORTED, "%s: K=%d > 256 not supported", who, lv->K);
-    BANET_REQUIRE(lv->C <= 2048, BANET_ERR_UNSUPPORTED, "%s: C=%d > 2048 not supported", who, lv->C);
-    return BANET_OK;
-}
-
-// The keyframe build is fp32 SIMT only: AUTO resolves to it (as AUTO does wherever the tensor cores do not apply); the TF32 modes have no
-// keyframe kernel.
-int check_keyframe_precision(int precision, const char* who)
-{
-    BANET_REQUIRE(precision == BANET_PREC_AUTO || precision == BANET_PREC_FP32_SIMT || precision == BANET_PREC_TF32X1 || precision == BANET_PREC_TF32X2 ||
-                  precision == BANET_PREC_TF32X3 || precision == BANET_PREC_TF32_LEVELWISE, BANET_ERR_BAD_ARG, "%s: unknown precision mode %d", who, precision);
-    BANET_REQUIRE(precision == BANET_PREC_AUTO || precision == BANET_PREC_FP32_SIMT, BANET_ERR_UNSUPPORTED,
-                  "%s: precision mode %d (tensor cores) has no keyframe build; use AUTO or FP32_SIMT", who, precision);
-    return BANET_OK;
-}
-
-struct KeyCarve { size_t build, H, g, rbar, nvalid, lambda, delta, step, total; };
-int key_carve(const banet_keyframe_level_t* levels, int nlevels, KeyCarve* c)
-{
-    size_t build = 0; int maxC = 0;
-    const int nw = levels[0].nw, nf = levels[0].nf, K = levels[0].K, P = 6 + K;
-    const size_t nb = (size_t)nw * nf;
-    for (int l = 0; l < nlevels; ++l) {
-        KeyframePlan plan;
-        int rc = keyframe_plan(&levels[l], num_sms(), &plan);
-        if (rc) return rc;
-        if (plan.ws_bytes > build) build = plan.ws_bytes;
-        if (levels[l].C > maxC) maxC = levels[l].C;
-    }
-    size_t off = 0;
-    c->build = off;  off += align_up(build, 256);
-    c->H = off;      off += align_up(nb * P * P * 4, 256);
-    c->g = off;      off += align_up(nb * P * 4, 256);
-    c->rbar = off;   off += align_up(nb * maxC * 4, 256);
-    c->nvalid = off; off += align_up(nb * 4, 256);
-    c->lambda = off; off += align_up((size_t)nw * 4, 256);
-    c->delta = off;  off += align_up((size_t)nw * (6 * nf + K) * 4, 256);
-    c->step = off;   off += lm_window_batch_ws_bytes(nw, nf);
-    c->total = off;
-    return BANET_OK;
-}
-}  // namespace
-
 extern "C" size_t banet_lm_keyframe_build_workspace_bytes(const banet_keyframe_level_t* lv)
 {
     if (check_keyframe_level(lv, "lm_keyframe_build")) return 0;
@@ -745,9 +719,8 @@ extern "C" size_t banet_lm_keyframe_run_workspace_bytes(const banet_keyframe_lev
     for (int l = 0; l < nlevels; ++l)
         if (check_keyframe_level(&levels[l], "lm_keyframe_run") || levels[l].nw != levels[0].nw || levels[l].nf != levels[0].nf ||
             levels[l].K != levels[0].K) return 0;
-    KeyCarve c;
-    if (key_carve(levels, nlevels, &c) != BANET_OK) return 0;
-    return c.total;
+    RunCarve c;
+    return run_carve(levels, nlevels, precision, "lm_keyframe_run", keyframe_sizes(levels, nlevels), &c) ? 0 : c.total;
 }
 
 extern "C" int banet_lm_keyframe_run(const banet_keyframe_level_t* levels, int nlevels, int iters_per_level,
@@ -759,50 +732,20 @@ extern "C" int banet_lm_keyframe_run(const banet_keyframe_level_t* levels, int n
     BANET_REQUIRE(nlevels > 0 && iters_per_level > 0, BANET_ERR_BAD_ARG, "lm_keyframe_run: bad argument nlevels=%d iters=%d", nlevels, iters_per_level);
     BANET_REQUIRE(!opts->vmatrix_batch_scramble, BANET_ERR_BAD_ARG, "lm_keyframe_run: needs vmatrix_batch_scramble = 0");
     const int nw = levels[0].nw, nf = levels[0].nf, K = levels[0].K;
-    for (int l = 0; l < nlevels; ++l) {
-        int rc = check_keyframe_level(&levels[l], "lm_keyframe_run");
-        if (rc) return rc;
-        BANET_REQUIRE(levels[l].nw == nw && levels[l].nf == nf && levels[l].K == K, BANET_ERR_BAD_ARG, "lm_keyframe_run: nw/nf/K must agree across levels");
-        BANET_REQUIRE((mlp_weights && mlp_weights[l]) || lambda_fixed >= 0.f, BANET_ERR_BAD_ARG,
-                      "lm_keyframe_run: level %d has no lambda-MLP weights and lambda_fixed < 0", l);
-        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
-        BANET_REQUIRE(lm_window_batch_supported(K, use_mlp ? levels[l].C : 0), BANET_ERR_UNSUPPORTED,
-                      "lm_keyframe_run: K=%d (C=%d) does not fit the window step", K, levels[l].C);
-    }
-    int rc = check_keyframe_precision(precision, "lm_keyframe_run");
-    if (rc) return rc;
-    KeyCarve c;
-    rc = key_carve(levels, nlevels, &c);
-    if (rc) return rc;
-    BANET_REQUIRE(ws && ws_bytes >= c.total, BANET_ERR_WORKSPACE, "lm_keyframe_run: workspace %zu < %zu bytes", ws_bytes, c.total);
     cudaStream_t st = (cudaStream_t)stream;
-    char* base = reinterpret_cast<char*>(ws);
-    float* H = reinterpret_cast<float*>(base + c.H);
-    float* g = reinterpret_cast<float*>(base + c.g);
-    float* rbar = reinterpret_cast<float*>(base + c.rbar);
-    float* nvalid = reinterpret_cast<float*>(base + c.nvalid);
-    float* lam = reinterpret_cast<float*>(base + c.lambda);
-    float* delta = reinterpret_cast<float*>(base + c.delta);
-    const int nb = nw * nf;
-    zero_status_kernel<<<(nb + 255) / 256, 256, 0, st>>>(status, nb);
-    for (int l = 0; l < nlevels; ++l) {
-        const banet_keyframe_level_t* lv = &levels[l];
-        KeyframePlan plan;
-        rc = keyframe_plan(lv, num_sms(), &plan);
-        if (rc) return rc;
-        const bool use_mlp = mlp_weights && mlp_weights[l] && lambda_fixed < 0.f;
-        if (!use_mlp) fill_kernel<<<(nw + 255) / 256, 256, 0, st>>>(lam, nw, lambda_fixed);
-        for (int it = 0; it < iters_per_level; ++it) {                // one build launch and one step launch per iteration
-            rc = keyframe_build(lv, plan, R, T, W, H, g, rbar, nvalid, base + c.build, st);
-            if (rc) return rc;
-            rc = lm_window_batch_step(H, g, rbar, nw, nf, lv->N, lv->C, K, use_mlp ? mlp_weights[l] : nullptr, l2_regularizer_base,
-                                      use_mlp ? nullptr : lam, *opts, R, T, W, R, T, W, nullptr, delta, use_mlp ? lam : nullptr, status, 1,
-                                      base + c.step, st);
-            if (rc) return rc;
-        }
-    }
-    BANET_CUDA_LAUNCH_CHECK("lm_keyframe_run");
-    return BANET_OK;
+    return run_solve("lm_keyframe_run", levels, nlevels, iters_per_level, mlp_weights, lambda_fixed, precision, W, status, ws, ws_bytes, st,
+                     keyframe_sizes(levels, nlevels), nw,
+        [&](const banet_keyframe_level_t& lv, bool use_mlp) {
+            BANET_REQUIRE(lm_window_batch_supported(K, use_mlp ? lv.C : 0), BANET_ERR_UNSUPPORTED,
+                          "lm_keyframe_run: K=%d (C=%d) does not fit the window step", K, lv.C);
+            return BANET_OK;
+        },
+        [](const RunWork&) { return BANET_OK; },
+        [&](const banet_keyframe_level_t& lv, const KeyframePlan& plan, const float* mlp, const RunWork& w) {  // one build and one step launch
+            const int rc = keyframe_build(&lv, plan, R, T, W, w.H, w.g, w.rbar, w.nvalid, w.build, st);
+            return rc ? rc : lm_window_batch_step(w.H, w.g, w.rbar, nw, nf, lv.N, lv.C, K, mlp, l2_regularizer_base, mlp ? nullptr : w.lambda,
+                                                  *opts, R, T, W, R, T, W, nullptr, w.delta, mlp ? w.lambda : nullptr, status, 1, w.tail, st);
+        });
 }
 
 extern "C" size_t banet_lm_track_legacy_workspace_bytes(const banet_level_t* levels, int nlevels)

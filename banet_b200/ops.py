@@ -334,14 +334,15 @@ def lm_step(H: Tensor, g: Tensor, rbar_sum: Optional[Tensor], N: int, mlp_packed
     return Ro, To, Wo, delta, lout, status
 
 
-def _prepare_run(levels, mlp_packed, l2_regularizer_base, damping_eps, undamped_last, vmatrix_batch_scramble, precision, window: bool = False):
-    """Argument block of banet_lm_run shared by lm_run and LMRunGraph: level structs, lambda-MLP pointers, options, workspace size."""
+def _prepare_run(levels, query, query_args, mlp_packed, l2_regularizer_base, damping_eps, undamped_last, vmatrix_batch_scramble):
+    """Argument block of the whole-solve wrappers and LMRunGraph: the structs of the levels (Level or KeyframeLevel), lambda-MLP pointers,
+    options and the workspace size from the C-ABI query `query(structs, nlevels, *query_args)`, 0 when the query rejects the levels."""
     lib = load()
     structs, keep = [], []
     for lv in levels:
         s, k = lv.as_struct(); structs.append(s); keep.append(k)
-    arr = (BanetLevel * len(structs))(*structs)
-    nb, K = structs[0].nb, structs[0].K
+    arr = (type(structs[0]) * len(structs))(*structs)
+    K = structs[0].K
     if undamped_last is None:
         undamped_last = K > 0
     if l2_regularizer_base is None:              # BundleIteration scales lambda by 1000 (bundlenet.py:252-253, 393); CameraIteration ignores the base (:165-173)
@@ -356,10 +357,8 @@ def _prepare_run(levels, mlp_packed, l2_regularizer_base, damping_eps, undamped_
                 raise _lib.BanetError("mlp_packed size mismatch")
         mlp_ptrs[i] = None if m is None else m.data_ptr()
     opts = BanetSolveOpts(float(damping_eps), int(undamped_last), int(vmatrix_batch_scramble))
-    nbytes = (lib.banet_lm_window_run_workspace_bytes if window else lib.banet_lm_run_workspace_bytes)(arr, len(structs), precision)
-    if nbytes == 0:
-        check(-4, "banet_lm_window_run_workspace_bytes" if window else "banet_lm_run_workspace_bytes")
-    return arr, len(structs), nb, K, (mlp_ptrs if have else None), float(l2_regularizer_base), opts, int(nbytes), keep
+    nbytes = query(arr, len(structs), *query_args)
+    return arr, (mlp_ptrs if have else None), float(l2_regularizer_base), opts, int(nbytes), keep
 
 
 def lm_run(levels: Sequence[Level], iters_per_level: int, R: Tensor, T: Tensor, W: Optional[Tensor],
@@ -368,13 +367,16 @@ def lm_run(levels: Sequence[Level], iters_per_level: int, R: Tensor, T: Tensor, 
            vmatrix_batch_scramble: bool = False, precision: int = _lib.PREC_AUTO, workspace: Optional[Tensor] = None):
     """Whole coarse-to-fine solve on the device (banet_lm_run).  Returns new (R,T,W,status); inputs are not modified."""
     lib = load()
-    arr, nlev, nb, K, mlp_ptrs, base, opts, nbytes, _keep = _prepare_run(levels, mlp_packed, l2_regularizer_base, damping_eps, undamped_last,
-                                                                         vmatrix_batch_scramble, precision)
+    arr, mlp_ptrs, base, opts, nbytes, _keep = _prepare_run(levels, lib.banet_lm_run_workspace_bytes, (precision,), mlp_packed, l2_regularizer_base,
+                                                            damping_eps, undamped_last, vmatrix_batch_scramble)
+    if nbytes == 0:
+        check(-4, "banet_lm_run_workspace_bytes")
+    nb, K = arr[0].nb, arr[0].K
     R = _chk(R, "R", (nb, 3, 3)).clone(); T = _chk(T, "T", (nb, 3, 1)).clone()
     Wt = None if K == 0 else _chk(W, "W", (nb, K, 1)).clone()
     ws = workspace if workspace is not None and workspace.numel() >= nbytes else _ws(nbytes, R.device)
     status = torch.empty(nb, device=R.device, dtype=torch.int32)
-    check(lib.banet_lm_run(arr, nlev, int(iters_per_level), mlp_ptrs, base, float(lambda_fixed), C.byref(opts), precision,
+    check(lib.banet_lm_run(arr, len(arr), int(iters_per_level), mlp_ptrs, base, float(lambda_fixed), C.byref(opts), precision,
                            R.data_ptr(), T.data_ptr(), _ptr(Wt), status.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "banet_lm_run")
     return R, T, Wt, status
 
@@ -387,13 +389,16 @@ def lm_window_run(levels: Sequence[Level], iters_per_level: int, R: Tensor, T: T
     level are (keyframe -> frame f) and share ONE depth-coefficient vector.  R [nf,3,3], T [nf,3,1] per frame, W [K,1] (or [1,K,1]) shared.
     Returns new (R, T, W [K,1], status [nf])."""
     lib = load()
-    arr, nlev, nf, K, mlp_ptrs, base, opts, nbytes, _keep = _prepare_run(levels, mlp_packed, l2_regularizer_base, damping_eps, undamped_last,
-                                                                         False, precision, window=True)
+    arr, mlp_ptrs, base, opts, nbytes, _keep = _prepare_run(levels, lib.banet_lm_window_run_workspace_bytes, (precision,), mlp_packed,
+                                                            l2_regularizer_base, damping_eps, undamped_last, False)
+    if nbytes == 0:
+        check(-4, "banet_lm_window_run_workspace_bytes")
+    nf, K = arr[0].nb, arr[0].K
     R = _chk(R, "R", (nf, 3, 3)).clone(); T = _chk(T, "T", (nf, 3, 1)).clone()
     Wt = _chk(W.reshape(1, K, 1), "W", (1, K, 1)).repeat(nf, 1, 1).contiguous()
     ws = workspace if workspace is not None and workspace.numel() >= nbytes else _ws(nbytes, R.device)
     status = torch.empty(nf, device=R.device, dtype=torch.int32)
-    check(lib.banet_lm_window_run(arr, nlev, int(iters_per_level), mlp_ptrs, base, float(lambda_fixed), C.byref(opts), precision,
+    check(lib.banet_lm_window_run(arr, len(arr), int(iters_per_level), mlp_ptrs, base, float(lambda_fixed), C.byref(opts), precision,
                                   R.data_ptr(), T.data_ptr(), Wt.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(), _stream()),
           "banet_lm_window_run")
     return R, T, Wt[0].clone(), status
@@ -426,16 +431,16 @@ def lm_window_batch_run(levels: Sequence[Level], nw: int, iters_per_level: int, 
     w * nf + f = (keyframe of window w -> frame f).  R [nb,3,3], T [nb,3,1] per frame, W [nw,K,1] per window.  Returns new
     (R, T, W [nw,K,1], status [nb])."""
     lib = load()
-    arr, nlev, nb, K, mlp_ptrs, base, opts, _, _keep = _prepare_run(levels, mlp_packed, l2_regularizer_base, damping_eps, undamped_last,
-                                                                   False, precision)
-    nbytes = lib.banet_lm_window_batch_run_workspace_bytes(arr, nlev, int(nw), precision)
+    arr, mlp_ptrs, base, opts, nbytes, _keep = _prepare_run(levels, lib.banet_lm_window_batch_run_workspace_bytes, (int(nw), precision), mlp_packed,
+                                                            l2_regularizer_base, damping_eps, undamped_last, False)
+    nb, K = arr[0].nb, arr[0].K
     if nbytes == 0:
         check(-4 if nw > 0 and nb % nw == 0 else -1, "banet_lm_window_batch_run_workspace_bytes")
     R = _chk(R, "R", (nb, 3, 3)).clone(); T = _chk(T, "T", (nb, 3, 1)).clone()
     Wt = _chk(W.reshape(nw, K, 1), "W", (nw, K, 1)).clone()
     ws = workspace if workspace is not None and workspace.numel() >= nbytes else _ws(nbytes, R.device)
     status = torch.empty(nb, device=R.device, dtype=torch.int32)
-    check(lib.banet_lm_window_batch_run(arr, nlev, int(nw), int(iters_per_level), mlp_ptrs, base, float(lambda_fixed), C.byref(opts), precision,
+    check(lib.banet_lm_window_batch_run(arr, len(arr), int(nw), int(iters_per_level), mlp_ptrs, base, float(lambda_fixed), C.byref(opts), precision,
                                         R.data_ptr(), T.data_ptr(), Wt.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(), _stream()),
           "banet_lm_window_batch_run")
     return R, T, Wt, status
@@ -589,26 +594,14 @@ def lm_keyframe_run(levels: Sequence[KeyframeLevel], iters_per_level: int, R: Te
     """Joint coarse-to-fine solve of nw keyframe windows with the keyframe tensors once per window (banet_lm_keyframe_run): per iteration
     one keyframe build and one window step.  R [nw*nf,3,3], T [nw*nf,3,1], W [nw,K,1].  Returns new (R, T, W [nw,K,1], status [nw*nf])."""
     lib = load()
-    structs, keep = [], []
-    for lv in levels:
-        s, k = lv.as_struct(); structs.append(s); keep.append(k)
-    arr = (_lib.BanetKeyframeLevel * len(structs))(*structs)
-    nw, nb, K = structs[0].nw, structs[0].nw * structs[0].nf, structs[0].K
-    mlp_ptrs = (C.c_void_p * len(structs))()
-    have = False
-    for i in range(len(structs)):
-        m = None if mlp_packed is None else mlp_packed[i]
-        if m is not None:
-            m = _chk(m, "mlp_packed"); keep.append(m); have = True
-            if m.numel() != lib.banet_mlp_param_count(structs[i].C):
-                raise _lib.BanetError("mlp_packed size mismatch")
-        mlp_ptrs[i] = None if m is None else m.data_ptr()
-    opts = BanetSolveOpts(float(damping_eps), int(undamped_last), 0)
-    nbytes = lib.banet_lm_keyframe_run_workspace_bytes(arr, len(structs), int(precision))
+    arr, mlp_ptrs, base, opts, nbytes, _keep = _prepare_run(levels, lib.banet_lm_keyframe_run_workspace_bytes, (int(precision),), mlp_packed,
+                                                            l2_regularizer_base, damping_eps, undamped_last, False)
+    # a query of 0 is left to the run, which names the fault: the query sets no message for levels that disagree
+    nw, nb, K = arr[0].nw, arr[0].nw * arr[0].nf, arr[0].K
     R = _chk(R, "R", (nb, 3, 3)).clone(); T = _chk(T, "T", (nb, 3, 1)).clone(); Wt = _chk(W.reshape(nw, K, 1), "W", (nw, K, 1)).clone()
     ws = workspace if workspace is not None and workspace.numel() >= nbytes else _ws(nbytes, R.device)
     status = torch.empty(nb, device=R.device, dtype=torch.int32)
-    check(lib.banet_lm_keyframe_run(arr, len(structs), int(iters_per_level), mlp_ptrs if have else None, float(l2_regularizer_base), float(lambda_fixed),
+    check(lib.banet_lm_keyframe_run(arr, len(arr), int(iters_per_level), mlp_ptrs, base, float(lambda_fixed),
                                     C.byref(opts), int(precision), R.data_ptr(), T.data_ptr(), Wt.data_ptr(), status.data_ptr(), ws.data_ptr(),
                                     ws.numel(), _stream()), "banet_lm_keyframe_run")
     return R, T, Wt, status
@@ -625,8 +618,11 @@ class LMRunGraph:
                  l2_regularizer_base: Optional[float] = None, lambda_fixed: float = -1.0, damping_eps: float = 1e-5,
                  undamped_last: Optional[bool] = None, precision: int = _lib.PREC_AUTO):
         self._lib = load()
-        (self._arr, self._nlev, self.nb, self.K, self._mlp_ptrs, self._base, self._opts, nbytes, self._keep) = _prepare_run(
-            levels, mlp_packed, l2_regularizer_base, damping_eps, undamped_last, False, precision)
+        (self._arr, self._mlp_ptrs, self._base, self._opts, nbytes, self._keep) = _prepare_run(
+            levels, self._lib.banet_lm_run_workspace_bytes, (precision,), mlp_packed, l2_regularizer_base, damping_eps, undamped_last, False)
+        if nbytes == 0:
+            check(-4, "banet_lm_run_workspace_bytes")
+        self.nb, self.K = self._arr[0].nb, self._arr[0].K
         self._iters, self._lambda_fixed, self._prec = int(iters_per_level), float(lambda_fixed), int(precision)
         dev = levels[0].conv1.device
         self.R = torch.zeros(self.nb, 3, 3, device=dev); self.T = torch.zeros(self.nb, 3, 1, device=dev)
@@ -644,7 +640,7 @@ class LMRunGraph:
             self._launch()
 
     def _launch(self):
-        check(self._lib.banet_lm_run(self._arr, self._nlev, self._iters, self._mlp_ptrs, self._base, self._lambda_fixed, C.byref(self._opts),
+        check(self._lib.banet_lm_run(self._arr, len(self._arr), self._iters, self._mlp_ptrs, self._base, self._lambda_fixed, C.byref(self._opts),
                                      self._prec, self.R.data_ptr(), self.T.data_ptr(), _ptr(self.W), self.status.data_ptr(),
                                      self._ws.data_ptr(), self._ws.numel(), _stream()), "banet_lm_run")
 

@@ -59,6 +59,35 @@ def test_keyframe_entries_reject_bad_arguments_without_gpu():
     assert rws([_klevel()], 1) == 0 and rws([_klevel(K=0)]) == 0 and rws([_klevel(), _klevel(nf=3)]) == 0
 
 
+class _StructLevel:
+    """A level that is only its C struct (dummy device pointers), for the wrappers' argument path on the CPU."""
+    def __init__(self, st):
+        self.st = st
+
+    def as_struct(self):
+        return self.st, []
+
+
+def test_run_wrappers_report_the_library_message_without_gpu(monkeypatch):
+    """The whole-solve wrappers raise BanetError with the library's own message: a rejected keyframe run reaches banet_lm_keyframe_run (its
+    workspace query sets no message for levels that disagree), a bad nw of a window batch is BANET_ERR_BAD_ARG.  CPU tensors stand in for
+    the device tensors; every call fails in the library before any CUDA call."""
+    from banet_b200 import ops, _lib
+    monkeypatch.setattr(ops, "_chk", lambda t, name, shape=None, features=False: t)
+    monkeypatch.setattr(ops, "_stream", lambda: 0)
+    z = torch.zeros
+    key = [_StructLevel(_klevel(nw=2, nf=4, K=16)), _StructLevel(_klevel(nw=2, nf=2, K=16))]
+    with pytest.raises(_lib.BanetError, match=r"banet_lm_keyframe_run failed \(code -1\): lm_keyframe_run: nw/nf/K must agree across levels"):
+        ops.lm_keyframe_run(key, 1, z(8, 3, 3), z(8, 3, 1), z(2, 16, 1), lambda_fixed=0.5)
+    with pytest.raises(_lib.BanetError, match=r"banet_lm_keyframe_run failed \(code -4\): lm_keyframe_run: precision mode 1 \(tensor cores\)"):
+        ops.lm_keyframe_run(key[:1], 1, z(8, 3, 3), z(8, 3, 1), z(2, 16, 1), lambda_fixed=0.5, precision=_lib.PREC_TF32X1)
+    pair = [_StructLevel(_lib.BanetLevel(4, 4096, 64, 16, 48, 64, 192, 1, 1, 1, 1, 1, 1, 0, 0))]
+    with pytest.raises(_lib.BanetError, match=r"banet_lm_window_batch_run_workspace_bytes failed \(code -1\)"):
+        ops.lm_window_batch_run(pair, 3, 1, z(4, 3, 3), z(4, 3, 1), z(3, 16, 1), lambda_fixed=0.5)
+    with pytest.raises(_lib.BanetError, match=r"banet_lm_run_workspace_bytes failed \(code -4\): unknown precision mode 9"):
+        ops.lm_run(pair, 1, z(4, 3, 3), z(4, 3, 1), z(4, 16, 1), lambda_fixed=0.5, precision=9)
+
+
 # ------------------------------------------------------------------------------------------ GPU
 def _scene(nw, nf, C, K, n_points, seed=83, dtype=torch.float32, level_ids=None, H=120, W=160):
     """Sparse: n_points keyframe points on the 120 x 160 map of level 3; dense (n_points None): the 60 x 80 grid of level 2."""
